@@ -82,7 +82,7 @@ size_t b200gs_binning_bytes(int64_t cap, int32_t H, int32_t W, int32_t P, int32_
     const int gx = (W + GS_TILE - 1) / GS_TILE, gy = (H + GS_TILE - 1) / GS_TILE;
     return binning_layout(cap, gx * gy * V, (int64_t)P * V).total;
 }
-size_t b200gs_backward_scratch_bytes(int32_t P, int32_t V) { return gs_align((size_t)P * V * GS_SGRAD_BYTES_MAX); }
+size_t b200gs_backward_scratch_bytes(int32_t P, int32_t V) { return gs_align((size_t)P * V * sizeof(ScreenGrad)); }
 
 static int check_common(const b200gs_params *p, const float *shs, const float *colors, const float *scales,
                         const float *rots, const float *cov)
@@ -240,8 +240,7 @@ int b200gs_backward(const b200gs_params *prm, const float *means3D, const float 
     if ((((uintptr_t)geom_buf) | ((uintptr_t)binning_buf) | ((uintptr_t)image_buf) | ((uintptr_t)scratch)) & 15) return B200GS_E_BUFFER;
     const char *gb = (const char *)geom_buf, *bb = (const char *)binning_buf, *ib = (const char *)image_buf;
 
-    const size_t sg_bytes = blend_sgrad_is_moments() == 2 ? (size_t)GS_SGRAD_F64_DOUBLES * 8 : sizeof(ScreenGrad);
-    CK(cudaMemsetAsync(scratch, 0, (size_t)P * V * sg_bytes, st), "memset scratch");
+    CK(cudaMemsetAsync(scratch, 0, (size_t)P * V * sizeof(ScreenGrad), st), "memset scratch");
     BlendBwdArgs b;
     b.H = H; b.W = W; b.grid_x = gx; b.grid_y = gy; b.V = V; b.P = P;
     b.ranges = (const uint2 *)(bb + BL.ranges); b.point_list = (const uint32_t *)(bb + BL.vals_out);

@@ -21,11 +21,12 @@
 //     alpha is provably < 1/255, so images are unchanged.  Forward arithmetic follows the pinned order of
 //     common.cuh: images are bit-identical to the CPU oracle.
 //   * Backward: per-pixel terms are expressed as ten sums per Gaussian -- six moments of q = G*dL/dalpha
-//     (1, dx, dy, dx^2, dx*dy, dy^2) and four colour/depth weights -- reduced over the
-//     32 lanes with a 12-shuffle multi-value butterfly (not 10 x 5 shuffles), then ten lanes each issue one
-//     red.global.add.f32 into the Gaussian's 48-byte ScreenGrad record.  Upstream: ~10 atomics per PIXEL.
+//     (1, dx, dy, dx^2, dx*dy, dy^2) and four colour/depth weights.  The hit loop parks each pixel's (q, w) in shared
+//     memory; every BWD_PARK hits a transposed pass (lane = hit, walking pixels) forms the ten sums in registers and
+//     writes them with three vector REDs (v4 + v4 + v2) into the Gaussian's 48-byte ScreenGrad record.  Upstream:
+//     ~10 atomics per PIXEL.
 //   * The compile-time switches below are the A/B experiments DESIGN.md section 5 lists: the
-//     product is BWD_T_DIV=1, everything else 0.
+//     product is BWD_T_DIV=1 and BWD_PARK=16, everything else 0.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -34,15 +35,21 @@
 #define WARPS_PER_CTA 2 // independent patches per CTA (1, 2, 4 or 8); H100 (400 W) bench step: 1 and 2 within noise, 4 is 26 % slower
 #endif
 #ifndef BWD_MIN_BLOCKS
-#define BWD_MIN_BLOCKS 16 // caps the backward kernel at 64 registers (32 warps/SM); H100 (400 W): 12 within noise, 20 blocks 2.5 % slower
+#define BWD_MIN_BLOCKS 16 // caps the backward kernel at 64 registers (32 warps/SM), no spills.  H100 80GB HBM3, 700 W, bench step
+                          // with the park buffer: 12 blocks (80 registers) bwd 14.3 ms against 13.1 ms at 16.  Before it (400 W):
+                          // 12 within noise, 20 blocks 2.5 % slower
 #endif
 #define CTAS_PER_TILE (8 / WARPS_PER_CTA)
 #ifndef FWD_BULK
 #define FWD_BULK 0 // 1: forward blend with cp.async.bulk + mbarrier staging of the id runs (A/B experiment; see DESIGN.md)
 #endif
-#ifndef SGRAD_F64
-#define SGRAD_F64 0 // 1: per-Gaussian accumulators in double (red.global.add.f64).  At BASELINE sizes the worst gradient rows do
-                    // not move (they are not accumulation-order errors) and the scratch doubles: off.
+#ifndef BWD_PARK
+#define BWD_PARK 16 // backward: hits parked per flush (8 or 16); 32 / BWD_PARK lanes share a hit in the flush pass.  H100 80GB
+                    // HBM3, 700 W, bench step, bwd: 16 -> 13.1 ms (13.1 KB smem per CTA), 8 -> 14.0 ms (8.7 KB; 15.2-15.5 ms
+                    // at 12 blocks)
+#endif
+#if BWD_PARK != 8 && BWD_PARK != 16
+#error "BWD_PARK must be 8 or 16"
 #endif
 #ifndef BWD_T_DIV
 #define BWD_T_DIV 1 // transmittance recovery T <- T/(1-alpha): 0 = MUFU reciprocal, 1 = + one Newton step, 2 = IEEE division.
@@ -387,62 +394,84 @@ void launch_blend_fwd(const BlendArgs &a, cudaStream_t st)
 // ------------------------------------------------------------------------------------------------
 // B1
 // ------------------------------------------------------------------------------------------------
-// Lane selectors of the butterfly as all-ones / all-zero words: a select on a register mask is one LOP3 and needs no
-// predicate register, so the selectors stay live across the hit loop instead of being re-derived from the lane id per hit.
-// opaque() hides where a value came from, so that the compiler keeps it in a register instead of recomputing it.
-__device__ __forceinline__ uint32_t opaque(uint32_t x)
-{
-    asm volatile("" : "+r"(x));
-    return x;
-}
-struct LaneSel {
-    uint32_t m16, m8, m4, m2;
-    __device__ __forceinline__ explicit LaneSel(int lane)
-        : m16(opaque(0u - ((lane >> 4) & 1u))), m8(opaque(0u - ((lane >> 3) & 1u))), m4(opaque(0u - ((lane >> 2) & 1u))),
-          m2(opaque(0u - ((lane >> 1) & 1u))) {}
+// The hit loop parks every pixel's (q, w) of a hit here instead of reducing across lanes once per hit.  A flush then sums
+// BWD_PARK parked hits at once with a lane per (hit, block of BWD_PARK pixels), so no value crosses a lane until the
+// (32 / BWD_PARK)-lane exchange that ends the flush.
+#define PARK_LANES (32 / BWD_PARK) // lanes that share one parked hit in the flush
+struct __align__(16) WarpPark {
+    float2 qw[BWD_PARK][33];     // (q, w) of park slot s at pixel p.  Rows are padded to 33 so that both the lane-per-pixel
+                                 // STS.64 of the hit loop and the lane-per-slot LDS.64 of the flush are free of bank conflicts
+    float4 pix[32 + PARK_LANES]; // (gC0, gC1, gC2, gD) of pixel p at pix[p + p / BWD_PARK]: the PARK_LANES pixels one flush
+                                 // step reads lie in distinct banks
+    float4 hit[BWD_PARK];        // slot s: the hit's slab word 0 (px, py, list position, record index)
 };
-__device__ __forceinline__ float sel(uint32_t m, float x, float y) // m ? y : x
+// vector atomic adds without a return value (sm_90): a 16-byte (or 8-byte) aligned run of floats in one L2 request
+__device__ __forceinline__ void red_add_v4(float *p, float a, float b, float c, float d)
 {
-    return __uint_as_float((__float_as_uint(x) & ~m) | (__float_as_uint(y) & m));
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
-// Sum ten per-lane values over the warp with 12 shuffles.  After the call, lanes with bit0 == 0 and a valid
-// slot hold the warp total of value `slot` (slot_of_lane below); other lanes hold junk.
-__device__ __forceinline__ float butterfly10(float v0, float v1, float v2, float v3, float v4, float v5, float v6, float v7,
-                                             float v8, float v9, const LaneSel &L)
+__device__ __forceinline__ void red_add_v2(float *p, float a, float b)
 {
-    // xor 16: lower half keeps v0..v4, upper half keeps v5..v9
-    float a0 = sel(L.m16, v0, v5) + __shfl_xor_sync(FULL, sel(L.m16, v5, v0), 16);
-    float a1 = sel(L.m16, v1, v6) + __shfl_xor_sync(FULL, sel(L.m16, v6, v1), 16);
-    float a2 = sel(L.m16, v2, v7) + __shfl_xor_sync(FULL, sel(L.m16, v7, v2), 16);
-    float a3 = sel(L.m16, v3, v8) + __shfl_xor_sync(FULL, sel(L.m16, v8, v3), 16);
-    float a4 = sel(L.m16, v4, v9) + __shfl_xor_sync(FULL, sel(L.m16, v9, v4), 16);
-    // xor 8: h8 == 0 keeps a0,a1,a2 ; h8 == 1 keeps a3,a4.  c2 is only read on h8 == 0 lanes: no select needed
-    float c0 = sel(L.m8, a0, a3) + __shfl_xor_sync(FULL, sel(L.m8, a3, a0), 8);
-    float c1 = sel(L.m8, a1, a4) + __shfl_xor_sync(FULL, sel(L.m8, a4, a1), 8);
-    float c2 = a2 + __shfl_xor_sync(FULL, a2, 8);
-    // xor 4: h4 == 0 keeps c0,c1 ; h4 == 1 keeps c2.  d1 is only read on h4 == 0 lanes
-    float d0 = sel(L.m4, c0, c2) + __shfl_xor_sync(FULL, sel(L.m4, c2, c0), 4);
-    float d1 = c1 + __shfl_xor_sync(FULL, c1, 4);
-    // xor 2: h2 == 0 keeps d0 ; h2 == 1 keeps d1
-    float e = sel(L.m2, d0, d1) + __shfl_xor_sync(FULL, sel(L.m2, d1, d0), 2);
-    e += __shfl_xor_sync(FULL, e, 1);
-    return e;
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
-// atomicAdd without a return value.  The address is global: sg_col below is opaque to the compiler, which would otherwise
-// emit a generic-address atomic.
-__device__ __forceinline__ void red_add(float *p, float v) { asm volatile("red.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory"); }
-__device__ __forceinline__ void red_add(double *p, double v) { asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory"); }
-__device__ __forceinline__ int slot_of_lane(int lane)
+
+// Sums the first n park slots into ScreenGrad.  Lane l takes slot h = l % BWD_PARK over the pixels
+// [BWD_PARK*part, BWD_PARK*part + BWD_PARK), part = l / BWD_PARK: BWD_PARK / 8 rows of the 8x4 patch.  Within a row dy is
+// constant, so the row accumulates sum q, sum q*dx, sum q*dx^2 and folds dy in once per row; dx and dy are the hit loop's
+// expressions.  The parts' sums meet in a (32 / BWD_PARK)-lane exchange, and the lanes of slot h write its record with a
+// v4 + v4 + v2 of vector REDs.
+__device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, float fx0, float fy_part, float *sgrad)
 {
-    const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4, h2 = lane & 2;
-    if (lane & 1) return -1;
-    if ((h4 && h2) || (h8 && h4)) return -1;
-    return (h16 ? 5 : 0) + (h8 ? 3 : 0) + (h4 ? 2 : 0) + (h2 ? 1 : 0);
+    __syncwarp();
+    const int h = lane % BWD_PARK, part = lane / BWD_PARK;
+    const float4 s = pk.hit[h];
+    float dxk[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) dxk[k] = fsub(s.x, fadd(fx0, (float)k));
+    float S0 = 0.f, Sx = 0.f, Sy = 0.f, Sxx = 0.f, Sxy = 0.f, Syy = 0.f, W0 = 0.f, W1 = 0.f, W2 = 0.f, W3 = 0.f;
+#pragma unroll
+    for (int r = 0; r < BWD_PARK / 8; r++) {
+        const int p0 = BWD_PARK * part + 8 * r; // first pixel of the row
+        float R0 = 0.f, Rx = 0.f, Rxx = 0.f;
+#pragma unroll
+        for (int k = 0; k < 8; k++) {
+            const float2 v = pk.qw[h][p0 + k];
+            const float4 g = pk.pix[p0 + k + part];
+            const float qx = v.x * dxk[k];
+            R0 += v.x;
+            Rx += qx;
+            Rxx = fmaf(qx, dxk[k], Rxx);
+            W0 = fmaf(v.y, g.x, W0); W1 = fmaf(v.y, g.y, W1); W2 = fmaf(v.y, g.z, W2); W3 = fmaf(v.y, g.w, W3);
+        }
+        const float dy = fsub(s.y, fadd(fy_part, (float)r));
+        const float qy = R0 * dy;
+        S0 += R0; Sx += Rx; Sxx += Rxx; Sy += qy;
+        Sxy = fmaf(Rx, dy, Sxy);
+        Syy = fmaf(qy, dy, Syy);
+    }
+#pragma unroll
+    for (int o = BWD_PARK; o < 32; o <<= 1) {
+        S0 += __shfl_xor_sync(FULL, S0, o); Sx += __shfl_xor_sync(FULL, Sx, o); Sy += __shfl_xor_sync(FULL, Sy, o);
+        Sxx += __shfl_xor_sync(FULL, Sxx, o); Sxy += __shfl_xor_sync(FULL, Sxy, o); Syy += __shfl_xor_sync(FULL, Syy, o);
+        W0 += __shfl_xor_sync(FULL, W0, o); W1 += __shfl_xor_sync(FULL, W1, o); W2 += __shfl_xor_sync(FULL, W2, o);
+        W3 += __shfl_xor_sync(FULL, W3, o);
+    }
+    if (h < n) {
+        // ScreenGrad as moments: S0, Sx, Sy, Sxx | Sxy, Syy, w.gC0, w.gC1 | w.gC2, w.gD
+        float *rec = sgrad + (size_t)__float_as_uint(s.w) * (sizeof(ScreenGrad) / sizeof(float));
+        if (part < 2) {
+            const bool hi = part == 1;
+            red_add_v4(rec + (hi ? 4 : 0), hi ? Sxy : S0, hi ? Syy : Sx, hi ? W0 : Sy, hi ? W1 : Sxx);
+        }
+        if (part == (PARK_LANES > 2 ? 2 : 0)) red_add_v2(rec + 8, W2, W3);
+    }
+    __syncwarp();
 }
 
 __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_kernel(BlendBwdArgs a)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
+    __shared__ WarpPark parks[WARPS_PER_CTA];
 
     const int ntiles = a.grid_x * a.grid_y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -457,6 +486,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
     const bool inside = px < a.W && py < a.H;
     const float fpx = (float)px, fpy = (float)py;
     WarpSlab &sl = slabs[warp];
+    WarpPark &pk = parks[warp];
     const uint2 range = a.ranges[(size_t)v * ntiles + tile];
     const float4 *recs4 = reinterpret_cast<const float4 *>(a.recs);
     const uint32_t *plist = a.point_list + range.x;
@@ -486,19 +516,10 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
     if (wmax == 0) return;
 
     const float bg_dot = a.bg[0] * gC0 + a.bg[1] * gC1 + a.bg[2] * gC2;
-    const LaneSel lsel(lane);
-    const int slot = slot_of_lane(lane);
-    const bool red_lane = slot >= 0;
-    // this lane's column of ScreenGrad (or of the double accumulator record): record rid is at sg_col + rid * SG_STRIDE bytes
-#if SGRAD_F64
-    typedef double sg_t;
-    constexpr size_t SG_STRIDE = GS_SGRAD_F64_DOUBLES * sizeof(double);
-#else
-    typedef float sg_t;
-    constexpr size_t SG_STRIDE = sizeof(ScreenGrad);
-#endif
-    char *sg_col = reinterpret_cast<char *>(a.sgrad) + sizeof(sg_t) * (red_lane ? slot : 0);
-    asm volatile("" : "+l"(sg_col)); // computed once: the RED address in the loop is then one IMAD.WIDE.U32
+    pk.pix[lane + lane / BWD_PARK] = make_float4(gC0, gC1, gC2, gD); // read by the flushes, after their __syncwarp
+    int np = 0;                                                      // park slots in use (warp-uniform)
+    const float fx0 = (float)x0, fy_part = (float)(y0 + (lane / BWD_PARK) * (BWD_PARK / 8)); // the flush lane's first row
+    float *const sgrad = reinterpret_cast<float *>(a.sgrad);
     // Per-pixel state of the back-to-front replay.  Upstream keeps five "accumulated colour behind" recurrences
     // (r,g,b,depth,alpha), each rec = last_alpha*last_c + (1-last_alpha)*rec, and forms sum_ch (c_ch - rec_ch)*g_ch.
     // The recurrences are linear with identical coefficients, so their dot product with the pixel's fixed upstream
@@ -537,7 +558,6 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
         for (int i = 0; i < cnt; i++) {
             const float4 g0 = sl.rec[3 * i], q1 = sl.rec[3 * i + 1];
             const int pos = (int)__float_as_uint(g0.z); // 0-based position in the tile list
-            const uint32_t rid = __float_as_uint(g0.w);
             const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
             const float power = power_prescaled(q1.x, q1.y, q1.z, dx, dy);
             const float G = gs_exp(power);
@@ -566,14 +586,18 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
                 const float dL_dalpha = fmaf(T, cg - rg, -(Kbg * inv));
                 q = G * dL_dalpha;
             }
-            // six moments of q over the patch: 1, dx, dy, dx^2, dx*dy, dy^2 (the conic / mean combination is linear
-            // and happens once per Gaussian in B2)
-            const float qx = q * dx, qy = q * dy;
-            const float e = butterfly10(q, qx, qy, qx * dx, qx * dy, qy * dy, w * gC0, w * gC1, w * gC2, w * gD, lsel);
-            if (red_lane) red_add(reinterpret_cast<sg_t *>(sg_col + (size_t)rid * SG_STRIDE), (sg_t)e);
+            // park (q, w); the flush forms the six moments of q over the patch (1, dx, dy, dx^2, dx*dy, dy^2; the conic /
+            // mean combination is linear and happens once per Gaussian in B2) and the four weights of w
+            pk.qw[np][lane] = make_float2(q, w);
+            if (lane == 0) pk.hit[np] = g0;
+            if (++np == BWD_PARK) {
+                park_flush(pk, np, lane, fx0, fy_part, sgrad);
+                np = 0;
+            }
         }
         __syncwarp();
     }
+    if (np > 0) park_flush(pk, np, lane, fx0, fy_part, sgrad);
 }
 
 void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st)
@@ -584,7 +608,7 @@ void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st)
 
 // ScreenGrad holds moments of q = G*dL/dalpha here: S0, Sx, Sy, Sxx, Sxy, Syy = sum q*{1, dx, dy, dx^2, dx*dy, dy^2};
 // then colour(3) and depth weights.
-int blend_sgrad_is_moments() { return SGRAD_F64 ? 2 : 1; }
+int blend_sgrad_is_moments() { return 1; }
 
 __global__ void test_exp_kernel(const float *x, float *y, int64_t n)
 {

@@ -86,9 +86,6 @@ struct __align__(16) ScreenGrad {
     float pad0, pad1;
 };
 static_assert(sizeof(ScreenGrad) == 48, "ScreenGrad must be 48 bytes");
-// doubles per (view, Gaussian) of the optional double accumulators of the backward blend (blend.cu: SGRAD_F64)
-#define GS_SGRAD_F64_DOUBLES 12
-#define GS_SGRAD_BYTES_MAX 96
 
 __host__ __device__ inline size_t gs_align(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 

@@ -32,10 +32,9 @@ struct PreBwdArgs {
     float tanfovx[GS_MAX_VIEWS], tanfovy[GS_MAX_VIEWS];
     const int32_t *radii;
     const uint8_t *clamped;
-    const void *sgrad;       // [V*P] ScreenGrad (float, 48 B) or 12 doubles (96 B), see `moments`
+    const void *sgrad;       // [V*P] ScreenGrad (48 B of floats), see `moments`
     const GeomRec *recs;     // [V*P] forward records (conic, opacity) -- used when sgrad holds moments
-    int moments;             // 0: classic float (dx,dy,dA,dBh,dC,dO,dr,dg,db,dd); 1: float moments (S0,Sx,Sy,Sxx,Sxy,Syy,cr,cg,cb,cd);
-                             // 2: the same ten moments as doubles
+    int moments;             // 0: classic float (dx,dy,dA,dBh,dC,dO,dr,dg,db,dd); 1: float moments (S0,Sx,Sy,Sxx,Sxy,Syy,cr,cg,cb,cd)
     float *dL_dmeans3D, *dL_dmeans2D, *dL_dsh, *dL_dcolors, *dL_dopacity, *dL_dscales, *dL_drots, *dL_dcov3D;
 };
 

@@ -345,20 +345,10 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
     // Software pipeline over the views: the kernel is latency-bound (one dependent gather per view), so the radius of view
     // v+2 and the 64 bytes of per-view state of view v+1 are requested before view v is reduced.
     const float4 *sg4 = reinterpret_cast<const float4 *>(a.sgrad);
-    const double2 *sd2 = reinterpret_cast<const double2 *>(a.sgrad);
     const float4 *rc4 = reinterpret_cast<const float4 *>(a.recs);
-    const bool f64 = a.moments == 2;
-    // the ten accumulated sums of one (view, Gaussian): 3 x 16 B of floats, or 5 x 16 B of doubles rounded to float here
+    // the ten accumulated sums of one (view, Gaussian): 3 x 16 B of floats
     auto load_sums = [&](size_t rec, float4 &o0, float4 &o1, float4 &o2) {
-        if (f64) {
-            const double2 d0 = __ldg(sd2 + 6 * rec), d1 = __ldg(sd2 + 6 * rec + 1), d2 = __ldg(sd2 + 6 * rec + 2),
-                          d3 = __ldg(sd2 + 6 * rec + 3), d4 = __ldg(sd2 + 6 * rec + 4);
-            o0 = make_float4((float)d0.x, (float)d0.y, (float)d1.x, (float)d1.y);
-            o1 = make_float4((float)d2.x, (float)d2.y, (float)d3.x, (float)d3.y);
-            o2 = make_float4((float)d4.x, (float)d4.y, 0.f, 0.f);
-        } else {
-            o0 = __ldg(sg4 + 3 * rec); o1 = __ldg(sg4 + 3 * rec + 1); o2 = __ldg(sg4 + 3 * rec + 2);
-        }
+        o0 = __ldg(sg4 + 3 * rec); o1 = __ldg(sg4 + 3 * rec + 1); o2 = __ldg(sg4 + 3 * rec + 2);
     };
     int rad_n = a.radii[i], rad_nn = a.V > 1 ? a.radii[(size_t)a.P + i] : 0;
     float4 n0 = make_float4(0, 0, 0, 0), n1 = n0, n2 = n0, nr = n0;
