@@ -303,6 +303,9 @@ int b200gs_describe_state(const b200gs_params *prm, const void *geom_buf, const 
     out->ranges = (const uint32_t *)(bb + BL.ranges);
     out->final_T = (const float *)(ib + IL.final_T);
     out->n_contrib = (const uint32_t *)(ib + IL.n_contrib);
+    out->contributor_masks = (const uint32_t *)(bb + BL.cmask);
+    const int64_t cap = instance_capacity > 0 ? instance_capacity : 1;
+    out->contributor_mask_words = ((cap >> 5) + (int64_t)gx * gy * V + 1) * 8; // BinLayout::cmask's extent
     return B200GS_OK;
 }
 

@@ -76,13 +76,18 @@ struct __align__(16) GeomRec {
 };
 static_assert(sizeof(GeomRec) == 48, "GeomRec must be 48 bytes");
 
-// per-(view,Gaussian) screen-space gradient accumulator written by the backward blend: 48 B
+// per-(view,Gaussian) screen-space gradient accumulator written by the backward blend: 48 B, ten floats + padding.
+// blend_sgrad_is_moments() tells which of two formats the linked blend writes (fields below: classic | product):
+//   product blend (blend.cu, moments of q = G*dL/dalpha, dx = px_gauss - px, dy = py_gauss - py; w = alpha*T):
+//     S0, Sx, Sy, Sxx | Sxy, Syy, W0, W1 | W2, W3  =  sum q*{1, dx, dy, dx^2 | dx*dy, dy^2}, sum w*{gC0, gC1 | gC2, gD}
+//   classic comparator (baseline/classic_blend.cu): the screen-space gradients themselves, as named below.
+// preprocess_bwd turns the moments into the classic quantities (the conic / mean combination is linear).
 struct __align__(16) ScreenGrad {
-    float dx, dy;        // dL/dmean2D (NDC-scaled)
-    float dA, dBh, dC;   // dL/dconic (dBh = half of d/dB)
-    float dO;            // dL/dopacity
-    float dr, dg, db;    // dL/dcolour
-    float dDepth;        // dL/ddepth
+    float dx, dy;        // dL/dmean2D (NDC-scaled)              | product: S0, Sx
+    float dA, dBh, dC;   // dL/dconic (dBh = half of d/dB)        | product: Sy, Sxx, Sxy
+    float dO;            // dL/dopacity                           | product: Syy
+    float dr, dg, db;    // dL/dcolour                            | product: W0, W1, W2 = sum w*gC
+    float dDepth;        // dL/ddepth                             | product: W3 = sum w*gD
     float pad0, pad1;
 };
 static_assert(sizeof(ScreenGrad) == 48, "ScreenGrad must be 48 bytes");

@@ -28,7 +28,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200GS_LIB selects another build of the SAME C-ABI (only used to time baseline/libb200gs_classic.so, the
 # classic-structure comparator, through the identical host path).  It is not a fallback: the default is the product.
 LIB_PATH = os.environ.get("B200GS_LIB") or os.path.join(_HERE, "libb200gs.so")
-ABI_VERSION = 3
+ABI_VERSION = 4
 MAX_VIEWS = 64
 MAX_INSTANCES = 0x7FFFFFFF  # (Gaussian, tile) instances per call (B200GS_MAX_INSTANCES); larger batches are split by views
 
@@ -55,7 +55,8 @@ class _Params(C.Structure):
 
 class _StateView(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("geom_records", "tiles_touched", "offsets", "clamped", "sorted_tile_keys",
-                                          "depth_order", "point_list", "ranges", "final_T", "n_contrib")]
+                                          "depth_order", "point_list", "ranges", "final_T", "n_contrib",
+                                          "contributor_masks")] + [("contributor_mask_words", C.c_int64)]
 
 
 _lib = None
@@ -624,12 +625,32 @@ def forward_with_state(**kw):
         ranges=view(st.binning, sv.ranges, torch.int32, V * ntiles * 2).reshape(V * ntiles, 2),
         final_T=view(st.image, sv.final_T, torch.float32, V * H * W).reshape(V, H, W),
         n_contrib=view(st.image, sv.n_contrib, torch.int32, V * H * W).reshape(V, H, W),
+        # the forward blend's contributor masks (int32 words; layout in include/b200gs.h, b200gs_state_view)
+        contributor_masks=view(st.binning, sv.contributor_masks, torch.int32, sv.contributor_mask_words),
     )
     # the reference's 64-bit sort key of every instance: (view*tiles + tile) << 32 | depth bits of its Gaussian
     dbits = state["recs"][:, 11].contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
     pl = state["point_list"].to(torch.int64) & 0xFFFFFFFF
     state["sorted_keys"] = ((state["sorted_tile_keys"].to(torch.int64) & 0xFFFFFFFF) << 32) | dbits[pl]
     return color, radii, depth, alpha, state, st
+
+
+def forward_backward_with_state(g_color, g_depth, g_alpha, **kw):
+    """forward_with_state(**kw), then the backward of that same call for the image gradients g_color [V,3,H,W],
+    g_depth [V,1,H,W], g_alpha [V,1,H,W].  Returns (color, radii, depth, alpha, state, sums): `sums` [V,P,12] float32 is
+    the backward blend's ScreenGrad record of every (view, Gaussian) -- record v*P + g, in the format
+    blend_sgrad_is_moments() names (csrc/common.cuh) -- copied out before the state buffers can be re-used."""
+    color, radii, depth, alpha, state, st = forward_with_state(**kw)
+    dev = kw["means3D"].device
+    V, P = st.V, st.P
+    t = lambda k: _f32c(kw.get(k), dev)
+    g = [_f32c(x, dev).reshape(V, c, st.H, st.W) for x, c in ((g_color, 3), (g_depth, 1), (g_alpha, 1))]
+    _backward_impl(st, t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"),
+                   t("cov3D_precomp"), _f32c(kw["bg"], dev), t("viewmatrix").reshape(V, 4, 4), t("projmatrix").reshape(V, 4, 4),
+                   t("campos").reshape(V, 3), *g)
+    nbytes = V * P * 48
+    sums = st.scratch[:nbytes].view(torch.float32).reshape(V, P, 12).clone()
+    return color, radii, depth, alpha, state, sums
 
 
 def device_sort_pairs(keys: torch.Tensor, vals: torch.Tensor, nbits: int):

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define B200GS_ABI_VERSION 3
+#define B200GS_ABI_VERSION 4
 #define B200GS_MAX_VIEWS 64 /* per call; callers chunk larger batches */
 
 typedef enum b200gs_status {
@@ -210,6 +210,12 @@ typedef struct b200gs_state_view {
     const uint32_t *ranges;       /* [V*tiles][2] */
     const float *final_T;         /* [V,H,W] */
     const uint32_t *n_contrib;    /* [V,H,W] */
+    const uint32_t *contributor_masks; /* [contributor_mask_words] written by the forward blend: word
+                                          ((range.x >> 5) + vt + c) * 8 + patch, for tile vt = view*tiles + tile, is chunk c
+                                          (list positions [32c, 32c+32)) of that tile and patch = ((py % 16) / 4) * 2 +
+                                          (px % 16) / 8; bit l = entry 32c+l was blended by a pixel of the patch.  Defined
+                                          for c <= (max n_contrib over the patch - 1) / 32; later words are unspecified */
+    int64_t contributor_mask_words;
 } b200gs_state_view;
 int b200gs_describe_state(const b200gs_params *prm, const void *geom_buf, const void *binning_buf,
                           int64_t instance_capacity, const void *image_buf, b200gs_state_view *out);

@@ -116,6 +116,7 @@ typedef struct gso_ctx {
     /* image state */
     float *final_T;
     uint32_t *n_contrib;
+    uint8_t *contrib_patches; /* [D]: bit p = some in-image pixel of 8x4 patch p of the entry's tile blended it */
     int capP, capD, capPix, capTiles;
     int threads;
 } gso_ctx;
@@ -132,7 +133,7 @@ static void free_all(gso_ctx *c)
     free(c->xy); free(c->depth); free(c->conic_o); free(c->rgb); free(c->cov3d); free(c->radii);
     free(c->tiles_touched); free(c->offsets); free(c->rect); free(c->clamped);
     free(c->keys); free(c->keys_tmp); free(c->vals); free(c->vals_tmp); free(c->ranges);
-    free(c->final_T); free(c->n_contrib);
+    free(c->final_T); free(c->n_contrib); free(c->contrib_patches);
 }
 void gso_destroy(gso_ctx *c)
 {
@@ -393,6 +394,8 @@ int gso_forward(gso_ctx *c, int P, int deg, int M, int H, int W, float tanfovx, 
     REALLOC(c->keys, uint64_t, D); REALLOC(c->keys_tmp, uint64_t, D);
     REALLOC(c->vals, uint32_t, D); REALLOC(c->vals_tmp, uint32_t, D);
     REALLOC(c->ranges, uint32_t, 2 * c->ntiles);
+    REALLOC(c->contrib_patches, uint8_t, D);
+    memset(c->contrib_patches, 0, (size_t)D);
     /* F3 duplicate with keys: row-major over the tile rectangle */
 #pragma omp parallel for schedule(static)
     for (int i = 0; i < P; i++) {
@@ -441,6 +444,9 @@ int gso_forward(gso_ctx *c, int P, int deg, int M, int H, int W, float tanfovx, 
                 float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, Dd = 0.f, Aa = 0.f;
                 uint32_t contributor = 0, last = 0;
                 float fx = (float)px, fy = (float)py;
+                /* the CUDA blend's patch numbering: bit 0 = x half of the tile, bits 1-2 = band of four rows */
+                const uint8_t pbit = (uint8_t)(1u << (((py % TILE) / 4) * 2 + (px % TILE) / 8));
+                uint8_t *cp = c->contrib_patches + r0;
                 for (int j = 0; j < n; j++) {
                     const float *l = loc + 10 * j;
                     contributor++;
@@ -457,6 +463,7 @@ int gso_forward(gso_ctx *c, int P, int deg, int M, int H, int W, float tanfovx, 
                     Aa = Aa + w;
                     T = test_T;
                     last = contributor;
+                    cp[j] |= pbit;
                 }
                 size_t pix = (size_t)py * W + px;
                 c->final_T[pix] = T;
@@ -488,6 +495,7 @@ const int *gso_rect(gso_ctx *c) { return c->rect; }
 const uint8_t *gso_clamped(gso_ctx *c) { return c->clamped; }
 const float *gso_final_T(gso_ctx *c) { return c->final_T; }
 const uint32_t *gso_n_contrib(gso_ctx *c) { return c->n_contrib; }
+const uint8_t *gso_contrib_patches(gso_ctx *c) { return c->contrib_patches; }
 
 /* ------------------------------------------------------------------------------------------
  * backward  (SURVEY.md Appendix A.5-A.7).  Uses the state of the last gso_forward.
@@ -497,10 +505,24 @@ const uint32_t *gso_n_contrib(gso_ctx *c) { return c->n_contrib; }
  * sums and their reduction to per-Gaussian sums are carried in double and rounded to float32 once.
  * Partials are formed in parallel, then reduced sequentially in sorted-list order: deterministic
  * for any thread count.
+ *
+ * Optional export (sums_out / err_out non-NULL, each [P][10]): the per-Gaussian sums in the CUDA backward blend's
+ * moments format, in double, for checking that intermediate directly:
+ *   S0, Sx, Sy, Sxx, Sxy, Syy = sum q*{1, dx, dy, dx^2, dx*dy, dy^2},  q = G*dL/dalpha (the float32 product used for o[5]),
+ *   dx = px_gauss - px, dy = py_gauss - py;   W0..W3 = sum w*{gC0, gC1, gC2, gD},  w = alpha*T (float32).
+ * and an error scale per component: the sum over the terms of |term magnitude| * (r + err_const + N_g), where r is the
+ * replay depth (transmittance recoveries T <- T/(1-alpha) done for the pixel so far, this one included) and N_g the
+ * number of (tile, patch) pairs the Gaussian contributes to (contrib_patches bits of its entries: how many partial sums
+ * the CUDA flush writes into its record).  The magnitude of a q moment is
+ *   |phi_k(dx,dy)| * G * (T*(|cg|_abs + |rg|_abs) + T_final*|bg.gC|_abs/(1-alpha)),
+ * |.|_abs being the same expression on absolute values (cg = c.gC + depth*gD + gA, rg its back-to-front recurrence);
+ * that of W_k is |w*g_k|.  tests/test_gpu_parity.py derives err_const and the bound's factor.
+ * screen_out (optional, [P][10]): the double per-Gaussian sums o[0..9] below, before their rounding to float32.
  * ---------------------------------------------------------------------------------------- */
 int gso_backward(gso_ctx *c, const float *dL_dcolor, const float *dL_ddepth_img, const float *dL_dalpha_img,
                  float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                 float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D)
+                 float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                 double err_const, double *sums_out, double *err_out, double *screen_out)
 {
     const int P = c->P, H = c->H, W = c->W;
     const int64_t D = c->D;
@@ -508,6 +530,14 @@ int gso_backward(gso_ctx *c, const float *dL_dcolor, const float *dL_ddepth_img,
     /* every tile owns the slice [r0, r1) of `part`: it zeroes it itself (parallel first touch; a calloc of D*80 bytes
      * followed by a serial reduction made the backward 0.7 s serial per 1024^2 view of 300 k Gaussians) */
     double *part = (double *)malloc((size_t)(D > 0 ? D : 1) * 10 * sizeof(double));
+    /* moments export: per instance 10 sums + 10 error scales, laid out and reduced like `part` */
+    const int want_sums = sums_out != NULL && err_out != NULL;
+    double *sp = want_sums ? (double *)malloc((size_t)(D > 0 ? D : 1) * 20 * sizeof(double)) : NULL;
+    double *ng = NULL; /* N_g: (tile, patch) pairs Gaussian g contributes to */
+    if (want_sums) {
+        ng = (double *)calloc((size_t)(P > 0 ? P : 1), sizeof(double));
+        for (int64_t j = 0; j < D; j++) ng[c->vals[j]] += (double)__builtin_popcount(c->contrib_patches[j]);
+    }
 #pragma omp parallel for schedule(dynamic, 1)
     for (int t = 0; t < c->ntiles; t++) {
         int tx0 = (t % c->gx) * TILE, ty0 = (t / c->gx) * TILE;
@@ -515,6 +545,7 @@ int gso_backward(gso_ctx *c, const float *dL_dcolor, const float *dL_ddepth_img,
         int n = (int)(r1 - r0);
         if (n == 0) continue;
         memset(part + (size_t)r0 * 10, 0, sizeof(double) * 10 * (size_t)n);
+        if (sp) memset(sp + (size_t)r0 * 20, 0, sizeof(double) * 20 * (size_t)n);
         float *loc = (float *)malloc(sizeof(float) * 10 * n);
         for (int j = 0; j < n; j++) {
             uint32_t g = c->vals[r0 + j];
@@ -538,6 +569,10 @@ int gso_backward(gso_ctx *c, const float *dL_dcolor, const float *dL_ddepth_img,
                 float last_alpha = 0.f, last_c[3] = {0, 0, 0}, last_d = 0.f;
                 float acc_c[3] = {0, 0, 0}, acc_d = 0.f, acc_a = 0.f;
                 float fx = (float)px, fy = (float)py;
+                /* moments export: |cg| recurrence on absolute values, replay depth */
+                const double bgg_abs = fabs((double)bg[0] * gC[0]) + fabs((double)bg[1] * gC[1]) + fabs((double)bg[2] * gC[2]);
+                double rg_abs = 0.0, last_cg_abs = 0.0;
+                int depth = 0;
                 for (int j = last - 1; j >= 0; j--) {
                     const float *l = loc + 10 * j;
                     float dx = l[0] - fx, dy = l[1] - fy;
@@ -548,6 +583,15 @@ int gso_backward(gso_ctx *c, const float *dL_dcolor, const float *dL_ddepth_img,
                     if (alpha < ALPHA_MIN) continue;
                     T = T / (1.0f - alpha);
                     float w = alpha * T;
+                    double mq = 0.0; /* magnitude of this term's q, without phi_k */
+                    if (sp) {
+                        const double cg_abs = fabs((double)l[6] * gC[0]) + fabs((double)l[7] * gC[1]) + fabs((double)l[8] * gC[2]) +
+                                              fabs((double)l[9] * gD) + fabs((double)gA);
+                        rg_abs = (double)last_alpha * last_cg_abs + (1.0 - (double)last_alpha) * rg_abs;
+                        last_cg_abs = cg_abs;
+                        depth++;
+                        mq = (double)G * ((double)T * (cg_abs + rg_abs) + (double)T_final * bgg_abs / (1.0 - (double)alpha));
+                    }
                     float dL_dalpha = 0.f;
                     double *o = part + (size_t)(r0 + j) * 10;
                     for (int ch = 0; ch < 3; ch++) {
@@ -577,6 +621,22 @@ int gso_backward(gso_ctx *c, const float *dL_dcolor, const float *dL_ddepth_img,
                     o[3] += -0.5f * gdx * dy * dL_dG; /* HALF of d/dB; doubled in the conic backward */
                     o[4] += -0.5f * gdy * dy * dL_dG;
                     o[5] += G * dL_dalpha;
+                    if (sp) {
+                        double *s = sp + (size_t)(r0 + j) * 20;
+                        const double q = (double)(G * dL_dalpha), ddx = dx, ddy = dy;
+                        const double phi[6] = {1.0, ddx, ddy, ddx * ddx, ddx * ddy, ddy * ddy};
+                        const double wt = (double)depth + err_const + ng[c->vals[r0 + j]];
+                        for (int k = 0; k < 6; k++) {
+                            s[k] += q * phi[k];
+                            s[10 + k] += fabs(phi[k]) * mq * wt;
+                        }
+                        const double gk[4] = {gC[0], gC[1], gC[2], gD};
+                        for (int k = 0; k < 4; k++) {
+                            const double t = (double)w * gk[k];
+                            s[6 + k] += t;
+                            s[16 + k] += fabs(t) * wt;
+                        }
+                    }
                 }
             }
         free(loc);
@@ -601,8 +661,26 @@ int gso_backward(gso_ctx *c, const float *dL_dcolor, const float *dL_ddepth_img,
             const double *s = part + (size_t)j * 10;
             for (int k = 0; k < 10; k++) d[k] += s[k];
         }
+        if (sp) {
+            if (hi > lo) {
+                memset(sums_out + (size_t)lo * 10, 0, sizeof(double) * 10 * (size_t)(hi - lo));
+                memset(err_out + (size_t)lo * 10, 0, sizeof(double) * 10 * (size_t)(hi - lo));
+            }
+            for (int64_t j = 0; j < D; j++) {
+                const uint32_t g = c->vals[j];
+                if (g < lo || g >= hi) continue;
+                const double *s = sp + (size_t)j * 20;
+                for (int k = 0; k < 10; k++) {
+                    sums_out[(size_t)g * 10 + k] += s[k];
+                    err_out[(size_t)g * 10 + k] += s[10 + k];
+                }
+            }
+        }
     }
     free(part);
+    free(sp);
+    free(ng);
+    if (screen_out) memcpy(screen_out, gs, sizeof(double) * 10 * (size_t)P);
 
     const int Mc = c->M;
     const float *V = c->view, *PV = c->proj;

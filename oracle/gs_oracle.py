@@ -42,11 +42,11 @@ def lib():
         L.gso_forward.restype = C.c_int
         L.gso_forward.argtypes = [C.c_void_p] + [C.c_int] * 5 + [C.c_float] * 3 + [C.c_void_p] * 15
         L.gso_backward.restype = C.c_int
-        L.gso_backward.argtypes = [C.c_void_p] * 12
+        L.gso_backward.argtypes = [C.c_void_p] * 12 + [C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gso_num_rendered.restype = C.c_int64
         L.gso_num_rendered.argtypes = [C.c_void_p]
         for name in ("keys", "point_list", "ranges", "xy", "depths", "conic_opacity", "rgb", "cov3d",
-                     "tiles_touched", "rect", "clamped", "final_T", "n_contrib"):
+                     "tiles_touched", "rect", "clamped", "final_T", "n_contrib", "contrib_patches"):
             fn = getattr(L, "gso_" + name)
             fn.restype = C.c_void_p
             fn.argtypes = [C.c_void_p]
@@ -142,10 +142,17 @@ class Oracle:
             clamped=_view(L.gso_clamped(h), np.uint8, 3 * P).reshape(-1, 3),
             final_T=_view(L.gso_final_T(h), np.float32, self.H * self.W).reshape(self.H, self.W),
             n_contrib=_view(L.gso_n_contrib(h), np.uint32, self.H * self.W).reshape(self.H, self.W),
+            # per sorted instance: bit p = an in-image pixel of patch p = ((py % 16) // 4) * 2 + (px % 16) // 8 blended it
+            contrib_patches=_view(L.gso_contrib_patches(h), np.uint8, D),
         )
 
-    def backward(self, dL_dcolor, dL_ddepth, dL_dalpha):
-        """Gradients in the order GaussianRasterizer.backward returns them (SURVEY.md A.8)."""
+    def backward(self, dL_dcolor, dL_ddepth, dL_dalpha, sums_err_const=None):
+        """Gradients in the order GaussianRasterizer.backward returns them (SURVEY.md A.8).
+
+        sums_err_const (optional float): also return out["sums"] [P,10], the float64 per-Gaussian sums in the CUDA backward
+        blend's moments format (S0, Sx, Sy, Sxx, Sxy, Syy, W0..W3), and out["sums_err"] [P,10], their error scales with
+        this constant in the per-term weight (gs_oracle.c, gso_backward); and out["screen_sums"] [P,10], the float64 sums the
+        oracle's own screen-space gradients are rounded from (dL/dmean2D x/y, dL/dA, dL/dB / 2, dL/dC, dL/dopacity, colour, depth)."""
         P, M = self.P, self.M
         a = self._keep
         gc, gd, ga = _f32(dL_dcolor), _f32(dL_ddepth), _f32(dL_dalpha)
@@ -156,9 +163,14 @@ class Oracle:
         out["scales"] = np.zeros((P, 3), np.float32) if a["scales"] is not None else None
         out["rotations"] = np.zeros((P, 4), np.float32) if a["rots"] is not None else None
         out["cov3D_precomp"] = np.zeros((P, 6), np.float32) if a["cov"] is not None else None
+        if sums_err_const is not None:
+            out["sums"], out["sums_err"] = np.zeros((P, 10), np.float64), np.zeros((P, 10), np.float64)
+            out["screen_sums"] = np.zeros((P, 10), np.float64)
         rc = self.L.gso_backward(self.h, _ptr(gc), _ptr(gd), _ptr(ga), _ptr(out["means3D"]), _ptr(out["means2D"]),
                                  _ptr(out["shs"]), _ptr(out["colors_precomp"]), _ptr(out["opacities"]),
-                                 _ptr(out["scales"]), _ptr(out["rotations"]), _ptr(out["cov3D_precomp"]))
+                                 _ptr(out["scales"]), _ptr(out["rotations"]), _ptr(out["cov3D_precomp"]),
+                                 float(sums_err_const or 0.0), _ptr(out.get("sums")), _ptr(out.get("sums_err")),
+                                 _ptr(out.get("screen_sums")))
         if rc != 0:
             raise RuntimeError(f"gso_backward failed with code {rc}")
         return out

@@ -29,13 +29,18 @@ def test_every_declared_symbol_is_exported(lib):
     assert set(rasterizer.EXPORTS) == declared
 
 
-def test_size_queries_are_sane(lib):
+def test_abi_version_4_and_size_queries_are_sane(lib):
+    """ABI 4: b200gs_state_view ends with the contributor-mask region.  The library, the header and the ctypes mirror agree."""
     sz, i32, i64 = ctypes.c_size_t, ctypes.c_int32, ctypes.c_int64
     lib.b200gs_geom_bytes.restype = sz; lib.b200gs_geom_bytes.argtypes = [i32, i32]
     lib.b200gs_image_bytes.restype = sz; lib.b200gs_image_bytes.argtypes = [i32, i32, i32]
     lib.b200gs_binning_bytes.restype = sz; lib.b200gs_binning_bytes.argtypes = [i64, i32, i32, i32, i32]
     lib.b200gs_backward_scratch_bytes.restype = sz; lib.b200gs_backward_scratch_bytes.argtypes = [i32, i32]
-    assert lib.b200gs_abi_version() == 3
+    from humangaussian_b200 import rasterizer
+    hdr = open(os.path.join(ROOT, "include", "b200gs.h")).read()
+    assert re.search(r"#define B200GS_ABI_VERSION 4\b", hdr)
+    assert lib.b200gs_abi_version() == 4 and rasterizer.ABI_VERSION == 4
+    assert [f[0] for f in rasterizer._StateView._fields_][-2:] == ["contributor_masks", "contributor_mask_words"]
     assert lib.b200gs_geom_bytes(1000, 1) >= 1000 * (48 + 4 + 4 + 8 + 1)
     assert lib.b200gs_geom_bytes(1000, 4) >= 4 * 1000 * 65
     assert lib.b200gs_image_bytes(64, 64, 2) >= 2 * 64 * 64 * 8

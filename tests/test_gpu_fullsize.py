@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_parity import DEV, _check_backward, _check_forward_state, _oracle
+from test_gpu_parity import DEV, _check_backward, _check_backward_sums, _check_forward_state, _oracle
 from util import grad_images, grads_agree
 
 pytestmark = pytest.mark.gpu
@@ -43,8 +43,9 @@ FULL_SIZE = dict(min_rows=1.0 - 1e-4, row_cap=4.0, min_elementwise=0.999)
 def _full_check(inp, seed, min_instances):
     o_out, o_st, gimg, o_grads = _oracle(inp, seed)
     assert o_st["num_rendered"] >= min_instances, o_st["num_rendered"]
-    _check_forward_state(inp, o_out, o_st)
+    _check_forward_state(inp, o_out, o_st)  # includes the contributor masks, bit for bit
     _check_backward(inp, o_out, gimg, o_grads, criterion=FULL_SIZE)
+    _check_backward_sums(inp, gimg, o_grads)  # the backward blend's sums: the derived bound, no exceptions
     return o_st
 
 

@@ -3,7 +3,9 @@
 Bar (BASELINE.json north_star): bit-exact on tile / sort indices; 1e-5 abs / 1e-4 rel on RGB, depth, alpha and
 all gradients.  Because both sides follow the same pinned float operation order the forward pass is in fact
 compared BIT-FOR-BIT (images included); the backward (different summation order) uses the 1e-5 / 1e-4 tolerance in the
-form util.grads_agree states: per-Gaussian gradient vectors row-wise with no exceptions, elementwise for >= 99.9 %."""
+form util.grads_agree states: per-Gaussian gradient vectors row-wise with no exceptions, elementwise for >= 99.9 %.
+The backward blend's own intermediates are checked directly as well (below _oracle): the forward's contributor masks bit
+for bit, and its per-Gaussian sums against float64 sums within a derived error bound, with no exceptions."""
 import math
 
 import numpy as np
@@ -40,8 +42,111 @@ def _oracle(inp, seed=0, threads=0):
     out = o.forward(**inp)
     st = o.state()
     gimg = grad_images(inp["image_height"], inp["image_width"], seed)
-    grads = o.backward(*gimg)
+    grads = o.backward(*gimg, sums_err_const=SUMS_K)
     return out, st, gimg, grads
+
+
+# ---- the backward blend's intermediates -------------------------------------------------------------------------------
+#
+# Contributor masks.  The forward writes one u32 per (32-entry chunk, patch); the backward walks only their set bits.  They
+# are integer state of a bit-exact forward, so every word the backward reads -- chunks c <= (wmax - 1) >> 5, wmax = the
+# largest n_contrib over the patch's pixels -- must equal the word packed from the oracle's per-entry contrib_patches.
+#
+# Sums.  The backward blend leaves, per (view, Gaussian), ten float32 sums in the ScreenGrad record: six moments of
+# q = G*dL/dalpha (1, dx, dy, dx^2, dx*dy, dy^2) and W0..W3 = sum w*(gC, gD), w = alpha*T.  The oracle exports the same
+# sums in float64 and an error scale per component, E_k = sum over terms of m * (r + K + N_g), where m is the term's
+# magnitude (gs_oracle.c: |phi_k| * G * (T*(|cg|_abs + |rg|_abs) + T_final*|bg.gC|_abs/(1-alpha)) for a q moment, |w*g_k|
+# for W_k), r its replay depth (transmittance recoveries done for the pixel so far, this one included) and N_g the number of
+# (tile, patch) partial sums the kernel adds into the Gaussian's record.  The check is |gpu - ref| <= C * u * E_k for every
+# (Gaussian, component), u = 2^-24, no exceptions.  Both sides compute G, alpha, dx, dy, the colours and the upstream
+# gradients bit-identically; the error model counts, in units of u * m and to first order (r*u <= 2e-3 even for the
+# 17 k-deep tiles), the three ways they differ:
+#   transmittance chain -- the oracle divides (IEEE, 1 rounding per recovery), the kernel multiplies by a Newton-refined
+#     reciprocal (<= 1 for the reciprocal + 1 for the product): 3r between the two.
+#   the cg - rg cancellation -- the kernel folds the five colour/depth/alpha recurrences into one scalar (fma form, <= 3 per
+#     step), the oracle keeps five (<= 4 per step, relative to their absolute sum): 7r; forming cg, the difference and the
+#     background term 1/(1-alpha) * T_final * bg.gC: kernel 4 + 1 + 6 + 2, oracle 6 + 7 + 1: 27.
+#   summation order -- the oracle sums in float64 (negligible); the kernel forms phi_k * q in float32 (<= 2), sums a row of
+#     8 pixels, two rows and the two half-warps (<= 9; W_k: 16 fmas + 1 = 17), then adds the Gaussian's N_g partial sums with
+#     float atomics in any order (<= N_g - 1, relative to the sum of |partials|).
+# q moments: 10r + 27 + 2 + 9 + N_g - 1 = 10r + 37 + N_g;  W_k: 3r + 2 (w = alpha*T on both sides) + 17 + N_g - 1.
+# Both are <= 10 * (r + 4 + N_g): K = 4, C = 10.
+SUMS_K = 4.0
+SUMS_C = 10.0
+U = 2.0 ** -24
+SUM_NAMES = ("S0", "Sx", "Sy", "Sxx", "Sxy", "Syy", "W0", "W1", "W2", "W3")
+
+
+def _patch_wmax(n_contrib, H, W):
+    """[tiles, 8]: largest n_contrib over the in-image pixels of each 8x4 patch (patch = band * 2 + x half)"""
+    gx, gy = (W + 15) // 16, (H + 15) // 16
+    nc = np.zeros((gy * 16, gx * 16), np.int64)
+    nc[:H, :W] = n_contrib
+    return nc.reshape(gy, 4, 4, gx, 2, 8).max(axis=(2, 5)).transpose(0, 2, 1, 3).reshape(gx * gy, 8)
+
+
+def _packed_masks(contrib_patches, r0, r1, nch):
+    """[nch, 8] u32: the contributor-mask words of one tile packed from the oracle's per-entry patch bits"""
+    bits = np.zeros(nch * 32, np.uint8)
+    seg = contrib_patches[r0:min(r1, r0 + nch * 32)]
+    bits[:len(seg)] = seg
+    b = (bits[:, None] >> np.arange(8, dtype=np.uint8)) & 1
+    return (b.reshape(nch, 32, 8).astype(np.uint64) << np.arange(32, dtype=np.uint64)[None, :, None]).sum(1).astype(np.uint32)
+
+
+def _check_masks(masks, ranges, n_contrib, o_st, H, W, v=0):
+    """Contributor masks of view v (GPU words, GPU ranges of the batch, GPU n_contrib [H,W] of the view) against the
+    oracle's state of that view, bit for bit.  Returns (words compared, per-tile [8] wmax) for coverage assertions."""
+    masks = np.ascontiguousarray(masks).view(np.uint32)
+    ntiles = ((W + 15) // 16) * ((H + 15) // 16)
+    wmax = _patch_wmax(n_contrib, H, W)
+    checked = 0
+    for t in np.nonzero(wmax.max(1) > 0)[0]:
+        vt = v * ntiles + int(t)
+        nch = (int(wmax[t].max()) + 31) >> 5
+        r0, r1 = (int(x) for x in o_st["ranges"][t])
+        want = _packed_masks(o_st["contrib_patches"], r0, r1, nch)
+        base = ((int(ranges[vt, 0]) >> 5) + vt) * 8
+        got = masks[base + 8 * np.arange(nch)[:, None] + np.arange(8)[None, :]]
+        read = np.arange(nch)[:, None] <= (wmax[t][None, :] - 1) >> 5  # the words the backward reads
+        bad = read & (got != want)
+        if bad.any():
+            c, p = np.argwhere(bad)[0]
+            raise AssertionError(f"view {v} tile {t}: {int(bad.sum())} contributor-mask words differ; first: chunk {c} patch {p} "
+                                 f"gpu {got[c, p]:#010x} oracle {want[c, p]:#010x} (wmax {wmax[t][p]})")
+        checked += int(read.sum())
+    return checked, wmax
+
+
+def _check_sums(gpu_sums, o_grads, what=""):
+    """gpu_sums [P,12] (one view's ScreenGrad records) against the oracle's float64 sums and error scales: no exceptions."""
+    ref, E = o_grads["sums"], o_grads["sums_err"]
+    err = np.abs(gpu_sums[:, :10].astype(np.float64) - ref)
+    lim = SUMS_C * U * E
+    bad = err > lim
+    if bad.any():
+        ratio = err / np.maximum(lim, 1e-300)
+        worst = np.unravel_index(np.argmax(np.where(bad, ratio, 0)), bad.shape)
+        per = {SUM_NAMES[k]: int(bad[:, k].sum()) for k in range(10) if bad[:, k].any()}
+        raise AssertionError(f"{what}backward-blend sums outside C*u*E in {int(bad.any(1).sum())} Gaussians {per}; worst: Gaussian "
+                             f"{worst[0]} {SUM_NAMES[worst[1]]} gpu {gpu_sums[worst[0], worst[1]]:.9g} ref {ref[worst]:.9g} "
+                             f"|diff| {err[worst]:.3g} = {ratio[worst]:.3g}x the bound")
+    assert np.abs(gpu_sums[:, 10:]).max(initial=0.0) == 0.0, "ScreenGrad padding written"
+
+
+def _gpu_blend_state(inp, gimg):
+    """One forward + backward through the library: (state dict as numpy, sums [V,P,12])."""
+    from humangaussian_b200.rasterizer import forward_backward_with_state
+    kw = {k: (torch.tensor(v, device=DEV) if isinstance(v, np.ndarray) else v) for k, v in inp.items()}
+    gC, gD, gA = (torch.tensor(g, device=DEV) for g in gimg)
+    *_, st, sums = forward_backward_with_state(gC, gD, gA, **kw)
+    return {k: (v.cpu().numpy() if torch.is_tensor(v) else v) for k, v in st.items()}, sums.cpu().numpy()
+
+
+def _check_backward_sums(inp, gimg, o_grads):
+    """The backward blend's sums of a single-view call against the oracle's (beside _check_backward, same inputs)."""
+    _, sums = _gpu_blend_state(inp, gimg)
+    _check_sums(sums[0], o_grads)
 
 
 def test_exp_bit_exact():
@@ -82,6 +187,8 @@ def _check_forward_state(inp, o_out, o_st):
     assert np.array_equal(f(color[0].cpu().numpy()), f(col)), "RGB not bit-identical"
     assert np.array_equal(f(depth[0].cpu().numpy()), f(dep)), "depth image not bit-identical"
     assert np.array_equal(f(alpha[0].cpu().numpy()), f(alp)), "alpha image not bit-identical"
+    _check_masks(st["contributor_masks"].cpu().numpy(), st["ranges"].cpu().numpy(), st["n_contrib"][0].cpu().numpy(), o_st,
+                 inp["image_height"], inp["image_width"])
 
 
 def _check_backward(inp, o_out, gimg, o_grads, keys=("means3D", "opacities", "shs", "scales", "rotations"), extra=None, criterion=None):
@@ -111,6 +218,7 @@ def test_small_scene_fwd_bwd(deg, seed):
     o_out, o_st, gimg, o_grads = _oracle(inp, seed)
     _check_forward_state(inp, o_out, o_st)
     _check_backward(inp, o_out, gimg, o_grads)
+    _check_backward_sums(inp, gimg, o_grads)
 
 
 def test_dense_opaque_scene_terminates():
@@ -122,6 +230,7 @@ def test_dense_opaque_scene_terminates():
     assert (o_st["final_T"] < 1e-3).mean() > 0.05, "scene is not opaque enough to test early termination"
     _check_forward_state(inp, o_out, o_st)
     _check_backward(inp, o_out, gimg, o_grads)
+    _check_backward_sums(inp, gimg, o_grads)
 
 
 def test_precomputed_cov_and_colors():
@@ -138,6 +247,7 @@ def test_precomputed_cov_and_colors():
     o_out, o_st, gimg, o_grads = _oracle(inp2, 3)
     _check_forward_state(inp2, o_out, o_st)
     _check_backward(inp2, o_out, gimg, o_grads, keys=("means3D", "opacities", "colors_precomp", "cov3D_precomp"))
+    _check_backward_sums(inp2, gimg, o_grads)
 
 
 def test_behind_camera_and_empty():
@@ -148,6 +258,7 @@ def test_behind_camera_and_empty():
     assert o_st["num_rendered"] == 0
     _check_forward_state(inp, o_out, o_st)
     _check_backward(inp, o_out, gimg, o_grads)
+    _check_backward_sums(inp, gimg, o_grads)
     # P == 0
     s = _settings(inp)
     z = lambda *shape: torch.zeros(*shape, device=DEV, requires_grad=True)
@@ -208,6 +319,36 @@ def test_batched_views_equal_per_view_loop():
         assert ok
 
 
+def test_batched_views_masks_and_sums_per_camera():
+    """V = 3 cameras in one call: each view's contributor masks (inside the batch's shared mask region, tile vt = v*tiles +
+    tile) and ScreenGrad records (record v*P + g) against that camera's own oracle run."""
+    from humangaussian_b200.cameras import sample_orbit_cameras
+    from humangaussian_b200.rasterizer import forward_backward_with_state
+    from humangaussian_b200.renderer import stack_cameras
+    V, H, W = 3, 72, 104
+    inp, _, _ = small_scene(P=1500, deg=1, seed=6, H=H, W=W)
+    cams = sample_orbit_cameras(V, H, W, seed=4)
+    vm, pm, cp, tanx, tany = stack_cameras(cams, "cpu")
+    views = []
+    for v in range(V):
+        iv = dict(inp, viewmatrix=vm[v].numpy(), projmatrix=pm[v].numpy(), campos=cp[v].numpy(), tanfovx=float(tanx[v]),
+                  tanfovy=float(tany[v]))
+        views.append(_oracle(iv, 40 + v))
+    kw = {k: (torch.tensor(x, device=DEV) if isinstance(x, np.ndarray) else x) for k, x in inp.items()}
+    kw.update(viewmatrix=vm.to(DEV), projmatrix=pm.to(DEV), campos=cp.to(DEV), tanfovx=[float(t) for t in tanx],
+              tanfovy=[float(t) for t in tany])
+    gimg = [torch.tensor(np.stack([views[v][2][k] for v in range(V)]), device=DEV) for k in range(3)]
+    *_, st, sums = forward_backward_with_state(*gimg, **kw)
+    masks, ranges, nc = (st[k].cpu().numpy() for k in ("contributor_masks", "ranges", "n_contrib"))
+    sums = sums.cpu().numpy()
+    for v, (o_out, o_st, _, o_grads) in enumerate(views):
+        assert np.array_equal(nc[v].view(np.uint32), o_st["n_contrib"])
+        checked, _ = _check_masks(masks, ranges, nc[v], o_st, H, W, v=v)
+        assert checked > 100
+        _check_sums(sums[v], o_grads, what=f"view {v}: ")
+        assert np.abs(o_grads["sums"]).max() > 0
+
+
 def test_medium_scene_512():
     """BASELINE config 2 shape: 512x512, forward+backward, tens of thousands of Gaussians (synthetic body)."""
     inp, _, _ = small_scene(P=60000, deg=0, seed=11, H=512, W=512, big=False, dist=2.0, fovy_deg=70.0, elev=15.0, azim=0.0)
@@ -215,6 +356,7 @@ def test_medium_scene_512():
     assert o_st["num_rendered"] > 50000
     _check_forward_state(inp, o_out, o_st)
     _check_backward(inp, o_out, gimg, o_grads)
+    _check_backward_sums(inp, gimg, o_grads)
 
 
 def test_render_wrapper_dict_and_densification_signal():
@@ -271,6 +413,7 @@ def test_real_scene_512_config2():
     assert o_st["num_rendered"] > 20000 and (o_out[1] > 0).all()
     _check_forward_state(inp, o_out, o_st)
     _check_backward(inp, o_out, gimg, o_grads)
+    _check_backward_sums(inp, gimg, o_grads)
 
 
 def test_render_views_feeds_reference_optimizer_hook():

@@ -35,6 +35,38 @@ def small_scene(P=200, deg=1, seed=0, H=40, W=56, elev=12.0, azim=35.0, dist=1.6
     return inp, cam, p
 
 
+def screen_scene(px, py, depth, sigma, opacity, color=None, cov2d=None, H=64, W=128, fovy_deg=60.0):
+    """Activated inputs (colors_precomp / cov3D_precomp) of Gaussians given in screen space, for scenes that must hit exact
+    list and patch positions.  Per Gaussian: pixel centre (px, py), view depth, isotropic screen sigma in pixels (or a
+    screen-space 2x2 covariance cov2d [N,2,2], overriding sigma), opacity, colour.  The camera sits at the origin looking
+    down +z (identity view matrix); each Gaussian is unprojected through it, with a negligible depth extent.  The rasteriser
+    adds 0.3 px^2 to the screen covariance, so with sigma < 0.3 px that dilation sets the footprint: a Gaussian centred in
+    an 8x4 patch stays inside it.  Colours default to a fixed pseudo-random draw."""
+    from humangaussian_b200.cameras import getProjectionMatrix
+    px, py, z = (np.asarray(a, np.float64).reshape(-1) for a in (px, py, depth))
+    n = len(px)
+    tany = math.tan(math.radians(fovy_deg) / 2)
+    tanx = tany * W / H
+    f = W / (2 * tanx)  # = H / (2 * tany): square pixels
+    x = ((2 * px + 1) / W - 1) * tanx * z
+    y = ((2 * py + 1) / H - 1) * tany * z
+    if cov2d is None:
+        s = np.broadcast_to(np.asarray(sigma, np.float64), (n,))
+        cov2d = np.zeros((n, 2, 2))
+        cov2d[:, 0, 0] = cov2d[:, 1, 1] = s * s
+    k = (z / f) ** 2
+    cov = np.stack([cov2d[:, 0, 0] * k, cov2d[:, 0, 1] * k, np.zeros(n), cov2d[:, 1, 1] * k, np.zeros(n), 1e-4 * k], 1)
+    if color is None:
+        color = np.random.RandomState(n).rand(n, 3) * 0.8 + 0.1
+    proj = getProjectionMatrix(0.01, 100.0, 2 * math.atan(tanx), 2 * math.atan(tany)).transpose(0, 1).numpy()
+    return dict(means3D=np.stack([x, y, z], 1).astype(np.float32),
+                opacities=np.broadcast_to(np.asarray(opacity, np.float32), (n,)).reshape(n, 1).copy(),
+                colors_precomp=np.asarray(color, np.float32).reshape(n, 3).copy(), cov3D_precomp=cov.astype(np.float32),
+                sh_degree=0, viewmatrix=np.eye(4, dtype=np.float32), projmatrix=proj.astype(np.float32),
+                campos=np.zeros(3, np.float32), bg=np.array([0.1, 0.4, 0.7], np.float32), image_height=H, image_width=W,
+                tanfovx=tanx, tanfovy=tany, scale_modifier=1.0)
+
+
 def grad_images(H, W, seed=0):
     rng = np.random.RandomState(seed)
     return (rng.randn(3, H, W).astype(np.float32), rng.randn(1, H, W).astype(np.float32),
