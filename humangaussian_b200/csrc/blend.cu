@@ -25,6 +25,13 @@
 //     memory; every BWD_PARK hits a transposed pass (lane = hit, walking pixels) forms the ten sums in registers and
 //     writes them with three vector REDs (v4 + v4 + v2) into the Gaussian's 48-byte ScreenGrad record.  Upstream:
 //     ~10 atomics per PIXEL.
+//   * Both hit loops are branch-free: the per-pixel decisions (skip, done, blend / contribute) are predicates and the
+//     updates are predicated or selected, because a warp that diverges issues both sides.  What ptxas makes of them
+//     (CUDA 12.9, sm_90a, -O3; static SASS counts): forward 56 registers, 3 KB smem, no spills; 81 instructions per
+//     unrolled pair of hits (40.5 per hit, loop control and two constant moves included; 49 per hit with branches),
+//     no BSSY/BSYNC/BRA inside the pair, about 96 per 32-entry chunk of bookkeeping.  Backward 64 registers, 13.1 KB smem,
+//     no spills; 107 per unrolled pair of hits (53.5 per hit; about 65 with a branch around the contributing-lane block
+//     and separate slot / hit counters), plus the flush.
 //   * The compile-time switches below are the A/B experiments DESIGN.md section 5 lists: the
 //     product is BWD_T_DIV=1 and BWD_PARK=16, everything else 0.
 #include "common.cuh"
@@ -43,6 +50,11 @@
 #ifndef FWD_BULK
 #define FWD_BULK 0 // 1: forward blend with cp.async.bulk + mbarrier staging of the id runs (A/B experiment; see DESIGN.md)
 #endif
+#ifndef FWD_MIN_BLOCKS
+// caps the forward kernel at 56 registers (36 warps/SM), no spills; left to itself ptxas takes 60.  The bulk-copy variant
+// spills at 56 and is capped at 64 (32 warps/SM).
+#define FWD_MIN_BLOCKS (FWD_BULK ? 16 : 18)
+#endif
 #ifndef BWD_PARK
 #define BWD_PARK 16 // backward: hits parked per flush (8 or 16); 32 / BWD_PARK lanes share a hit in the flush pass.  H100 80GB
                     // HBM3, 700 W, bench step, bwd: 16 -> 13.1 ms (13.1 KB smem per CTA), 8 -> 14.0 ms (8.7 KB; 15.2-15.5 ms
@@ -57,10 +69,11 @@
                     // worst position-gradient rows out of tolerance; one Newton step (two FMAs) removes the bias.
 #endif
 
-// does the support box [px-hx,px+hx] x [py-hy,py+hy] reach the patch [x0,x0+7] x [y0,y0+3] ?
-__device__ __forceinline__ bool box_hits_patch(const float4 g0, float x0, float y0)
+// does the support box [px-hx,px+hx] x [py-hy,py+hy] reach the patch [x0,x0+7] x [y0,y0+3] ?  (x1 = x0 + 7, y1 = y0 + 3.)
+// The five comparisons have no side effects, so they are and-ed without short-circuit: one predicate chain, no branch.
+__device__ __forceinline__ bool box_hits_patch(const float4 g0, float x0, float y0, float x1, float y1)
 {
-    return (g0.z >= 0.0f) && (g0.x + g0.z >= x0) && (g0.x - g0.z <= x0 + 7.0f) && (g0.y + g0.w >= y0) && (g0.y - g0.w <= y0 + 3.0f);
+    return (g0.z >= 0.0f) & (g0.x + g0.z >= x0) & (g0.x - g0.z <= x1) & (g0.y + g0.w >= y0) & (g0.y - g0.w <= y1);
 }
 
 // power with the conic pre-scaled at staging time (A' = -A/2, B' = -B, C' = -C/2: exact operations, so the
@@ -82,8 +95,69 @@ struct __align__(16) WarpSlab {
 // ------------------------------------------------------------------------------------------------
 // F6
 // ------------------------------------------------------------------------------------------------
+// A forward pixel's running state.  A live pixel has T >= 1e-4.  A finished pixel keeps its last transmittance with the
+// sign bit set (an out-of-image pixel starts at 0): it keeps failing the T test and never accumulates, exactly like
+// upstream's `done` flag, and |T| is the transmittance to report.
+struct FwdPixel {
+    float T, C0, C1, C2, Dd, Aa;
+    uint32_t last, used; // 1-based list position of the last blended entry; entries of the chunk this pixel blended
+};
+
+// One slab hit s (three words) blended into pixel (fpx, fpy): the operation sequence of DESIGN.md section 2.  The three
+// outcomes -- skip (power > 0 or alpha < 1/255), done (T would fall below 1e-4) and blend -- are predicates, not branches:
+// 13.6 of 32 lanes blend per visit, so a branch would diverge and the warp would issue both sides anyway.  A lane that does
+// not blend keeps C0..C2, Dd, Aa, last and used bit for bit and T up to its sign: its updates are predicated off, never
+// scaled by a zero weight (c * 0 is not an exact no-op for every colour a caller may pass).
+__device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float fpy, FwdPixel &p)
+{
+    const float4 g0 = s[0], q1 = s[1], q2 = s[2];
+    const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
+    const float power = power_prescaled(q1.x, q1.y, q1.z, dx, dy);
+    const float alpha = fminf(GS_ALPHA_MAX, fmul(q1.w, gs_exp(power)));
+    const float test_T = fmul(p.T, fsub(1.0f, alpha)); // <= 0 once the pixel is done
+    const bool hit = !(power > 0.0f) & !(alpha < GS_ALPHA_MIN);
+    const bool blend = hit & !(test_T < GS_T_MIN);
+    const float w = fmul(alpha, p.T);
+    if (blend) {
+        p.C0 = ffma(q2.x, w, p.C0); p.C1 = ffma(q2.y, w, p.C1); p.C2 = ffma(q2.z, w, p.C2);
+        p.Dd = ffma(q2.w, w, p.Dd);
+        p.Aa = fadd(p.Aa, w);
+        p.last = __float_as_uint(g0.z);
+        p.used |= __float_as_uint(g0.w);
+    }
+    p.T = blend ? test_T : (hit ? -fabsf(p.T) : p.T);
+}
+
+// Blends the cnt hits staged in slab s, in order, two per iteration.
+__device__ __forceinline__ void fwd_blend_slab(const float4 *s, int cnt, float fpx, float fpy, FwdPixel &p)
+{
+    const float4 *const end2 = s + 3 * (cnt & ~1);
+#pragma unroll 1
+    for (; s != end2; s += 6) {
+        fwd_blend_hit(s, fpx, fpy, p);
+        fwd_blend_hit(s + 3, fpx, fpy, p);
+    }
+    if (cnt & 1) fwd_blend_hit(s, fpx, fpy, p);
+}
+
+// Writes the pixel's outputs (out-of-image pixels write nothing).
+__device__ __forceinline__ void fwd_store_pixel(const BlendArgs &a, int v, int px, int py, const FwdPixel &p)
+{
+    const float T_out = fabsf(p.T);
+    const size_t HW = (size_t)a.H * a.W;
+    const size_t pix = (size_t)py * a.W + px;
+    a.final_T[v * HW + pix] = T_out;
+    a.n_contrib[v * HW + pix] = p.last;
+    float *oc = a.out_color + (size_t)v * 3 * HW;
+    oc[pix] = ffma(T_out, a.bg[0], p.C0);
+    oc[HW + pix] = ffma(T_out, a.bg[1], p.C1);
+    oc[2 * HW + pix] = ffma(T_out, a.bg[2], p.C2);
+    a.out_depth[v * HW + pix] = p.Dd;
+    a.out_alpha[v * HW + pix] = p.Aa;
+}
+
 #if !FWD_BULK
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs a)
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_kernel(BlendArgs a)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
 
@@ -98,22 +172,18 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs
     const int x0 = tile_x * GS_TILE + (patch & 1) * 8, y0 = tile_y * GS_TILE + (patch >> 1) * 4;
     const int px = x0 + (lane & 7), py = y0 + (lane >> 3);
     const bool inside = px < a.W && py < a.H;
-    const float fpx = (float)px, fpy = (float)py, fx0 = (float)x0, fy0 = (float)y0;
-    WarpSlab &sl = slabs[warp];
+    const float fpx = (float)px, fpy = (float)py, fx0 = (float)x0, fy0 = (float)y0, fx1 = fx0 + 7.0f, fy1 = fy0 + 3.0f;
+    float4 *const slab = slabs[warp].rec;
 
     const uint2 range = a.ranges[(size_t)v * ntiles + tile];
     const int n_total = (int)(range.y - range.x);
     const float4 *recs4 = reinterpret_cast<const float4 *>(a.recs);
     const uint32_t *plist = a.point_list + range.x;
-    const uint32_t lt = (1u << lane) - 1u;
+    const uint32_t lt = (1u << lane) - 1u, bit = 1u << lane;
     // contributor mask of chunk c (list positions [32c, 32c+32)) of this patch: cmask[8c]
     uint32_t *const cmask = a.cmask + ((size_t)(range.x >> 5) + vt) * 8 + patch;
 
-    // T == 0 is the "done" sentinel: a finished (or out-of-image) pixel keeps failing the T test and never
-    // accumulates, exactly like upstream's `done` flag; T_out remembers the transmittance to report.
-    float T = inside ? 1.0f : 0.0f, T_out = 1.0f;
-    float C0 = 0.f, C1 = 0.f, C2 = 0.f, Dd = 0.f, Aa = 0.f;
-    uint32_t last = 0;
+    FwdPixel p = {inside ? 1.0f : 0.0f, 0.f, 0.f, 0.f, 0.f, 0.f, 0u, 0u};
 
     // software pipeline, two deep: while chunk c is blended the support boxes of chunk c+1 and the ids of chunk c+2
     // are in flight (the id -> record address dependency never sits on the critical path)
@@ -122,11 +192,12 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs
     if (lane < n_total) id_c = __ldg(plist + lane);
     if (32 + lane < n_total) id_n = __ldg(plist + 32 + lane);
     if (lane < n_total) g0_c = __ldg(recs4 + 3 * (size_t)id_c);
-    for (int base = 0; base < n_total; base += 32) {
+    uint32_t *cm = cmask;
+    for (int base = 0; base < n_total; base += 32, cm += 8) {
         // Chunks after this exit get no mask word.  The backward reads chunks up to (max n_contrib of the patch - 1) / 32
         // only, and that position was blended by a pixel of the patch before every pixel was done, so those were written.
-        if (__all_sync(FULL, T == 0.0f)) break;
-        const bool hit = box_hits_patch(g0_c, fx0, fy0);
+        if (__all_sync(FULL, !(p.T > 0.0f))) break;
+        const bool hit = box_hits_patch(g0_c, fx0, fy0, fx1, fy1);
         const uint32_t b = __ballot_sync(FULL, hit);
         float4 g1, g2;
         if (hit) {
@@ -138,60 +209,23 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs
         g0_c = make_float4(0.f, 0.f, -1.f, -1.f);
         if (base + 32 + lane < n_total) g0_c = __ldg(recs4 + 3 * (size_t)id_c);
         if (base + 64 + lane < n_total) id_n = __ldg(plist + base + 64 + lane);
-        if (b == 0u) {
-            if (lane == 0) cmask[(size_t)(base >> 5) * 8] = 0u;
-            continue;
-        }
-        if (hit) {
-            const int slot = __popc(b & lt);
-            sl.rec[3 * slot] = make_float4(g0_h.x, g0_h.y, __uint_as_float((uint32_t)(base + lane + 1)), __uint_as_float(1u << lane));
-            sl.rec[3 * slot + 1] = make_float4(fmul(-0.5f, g1.x), -g1.y, fmul(-0.5f, g1.z), g1.w);
-            sl.rec[3 * slot + 2] = g2;
-        }
-        __syncwarp();
-        const int cnt = __popc(b);
-        uint32_t used = 0; // entries of the chunk this pixel blended
-        for (int i = 0; i < cnt; i++) {
-            const float4 g0 = sl.rec[3 * i], q1 = sl.rec[3 * i + 1];
-            const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
-            const float power = power_prescaled(q1.x, q1.y, q1.z, dx, dy);
-            if (!(power > 0.0f)) {
-                const float alpha = fminf(GS_ALPHA_MAX, fmul(q1.w, gs_exp(power)));
-                if (!(alpha < GS_ALPHA_MIN)) {
-                    const float test_T = fmul(T, fsub(1.0f, alpha));
-                    if (test_T < GS_T_MIN) {
-                        if (T != 0.0f) T_out = T;
-                        T = 0.0f;
-                    } else {
-                        const float w = fmul(alpha, T);
-                        const float4 q2 = sl.rec[3 * i + 2];
-                        C0 = ffma(q2.x, w, C0); C1 = ffma(q2.y, w, C1); C2 = ffma(q2.z, w, C2);
-                        Dd = ffma(q2.w, w, Dd);
-                        Aa = fadd(Aa, w);
-                        T = test_T;
-                        last = __float_as_uint(g0.z);
-                        used |= __float_as_uint(g0.w);
-                    }
-                }
+        uint32_t m = 0u;
+        if (b != 0u) {
+            if (hit) {
+                float4 *const s = slab + 3 * __popc(b & lt);
+                s[0] = make_float4(g0_h.x, g0_h.y, __uint_as_float((uint32_t)(base + lane + 1)), __uint_as_float(bit));
+                s[1] = make_float4(fmul(-0.5f, g1.x), -g1.y, fmul(-0.5f, g1.z), g1.w);
+                s[2] = g2;
             }
+            __syncwarp();
+            p.used = 0u;
+            fwd_blend_slab(slab, __popc(b), fpx, fpy, p);
+            m = __reduce_or_sync(FULL, p.used);
+            __syncwarp();
         }
-        const uint32_t m = __reduce_or_sync(FULL, used);
-        if (lane == 0) cmask[(size_t)(base >> 5) * 8] = m;
-        __syncwarp();
+        if (lane == 0) *cm = m;
     }
-    if (inside) {
-        if (T != 0.0f) T_out = T;
-        const size_t HW = (size_t)a.H * a.W;
-        const size_t pix = (size_t)py * a.W + px;
-        a.final_T[v * HW + pix] = T_out;
-        a.n_contrib[v * HW + pix] = last;
-        float *oc = a.out_color + (size_t)v * 3 * HW;
-        oc[pix] = ffma(T_out, a.bg[0], C0);
-        oc[HW + pix] = ffma(T_out, a.bg[1], C1);
-        oc[2 * HW + pix] = ffma(T_out, a.bg[2], C2);
-        a.out_depth[v * HW + pix] = Dd;
-        a.out_alpha[v * HW + pix] = Aa;
-    }
+    if (inside) fwd_store_pixel(a, v, px, py, p);
 }
 
 #endif // !FWD_BULK
@@ -233,7 +267,7 @@ __device__ __forceinline__ void mbar_wait(unsigned long long *b, uint32_t parity
     }
 }
 
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs a)
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_kernel(BlendArgs a)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
     __shared__ BulkStage bulk[WARPS_PER_CTA];
@@ -265,9 +299,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs
     const int n_rel = (int)((range.y - range.x + 31u) >> 5);
     uint32_t carry = 0; // relative word c-1, its bits from absolute chunk c-1
 
-    float T = inside ? 1.0f : 0.0f, T_out = 1.0f;
-    float C0 = 0.f, C1 = 0.f, C2 = 0.f, Dd = 0.f, Aa = 0.f;
-    uint32_t last = 0;
+    FwdPixel p = {inside ? 1.0f : 0.0f, 0.f, 0.f, 0.f, 0.f, 0.f, 0u, 0u};
 
     if (lane == 0) { mbar_init(&bk.mbar[0], 1); mbar_init(&bk.mbar[1], 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -296,8 +328,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs
     int c = 0;
     for (; c < n_chunks; c++) {
         // as in the main variant: the relative chunks the backward reads all end before this exit
-        if (__all_sync(FULL, T == 0.0f)) break;
-        const bool hit = box_hits_patch(g0_c, fx0, fy0);
+        if (__all_sync(FULL, !(p.T > 0.0f))) break;
+        const bool hit = box_hits_patch(g0_c, fx0, fy0, fx0 + 7.0f, fy0 + 3.0f);
         const uint32_t b = __ballot_sync(FULL, hit);
         float4 g1, g2;
         if (hit) {
@@ -331,33 +363,9 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs
                 sl.rec[3 * slot + 2] = g2;
             }
             __syncwarp();
-            const int cnt = __popc(b);
-            uint32_t used = 0;
-            for (int i = 0; i < cnt; i++) {
-                const float4 g0 = sl.rec[3 * i], q1 = sl.rec[3 * i + 1];
-                const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
-                const float power = power_prescaled(q1.x, q1.y, q1.z, dx, dy);
-                if (!(power > 0.0f)) {
-                    const float alpha = fminf(GS_ALPHA_MAX, fmul(q1.w, gs_exp(power)));
-                    if (!(alpha < GS_ALPHA_MIN)) {
-                        const float test_T = fmul(T, fsub(1.0f, alpha));
-                        if (test_T < GS_T_MIN) {
-                            if (T != 0.0f) T_out = T;
-                            T = 0.0f;
-                        } else {
-                            const float w = fmul(alpha, T);
-                            const float4 q2 = sl.rec[3 * i + 2];
-                            C0 = ffma(q2.x, w, C0); C1 = ffma(q2.y, w, C1); C2 = ffma(q2.z, w, C2);
-                            Dd = ffma(q2.w, w, Dd);
-                            Aa = fadd(Aa, w);
-                            T = test_T;
-                            last = __float_as_uint(g0.z);
-                            used |= __float_as_uint(g0.w);
-                        }
-                    }
-                }
-            }
-            m = __reduce_or_sync(FULL, used);
+            p.used = 0u;
+            fwd_blend_slab(sl.rec, __popc(b), fpx, fpy, p);
+            m = __reduce_or_sync(FULL, p.used);
             __syncwarp();
         }
         // bits below r complete relative chunk c-1; bits from r up start relative chunk c
@@ -369,19 +377,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) blend_fwd_kernel(BlendArgs
     if (c >= 1 && c - 1 < n_rel && lane == 0) cmask[(size_t)(c - 1) * 8] = carry;
     // a bulk copy still in flight targets this CTA's shared memory: observe every issued stage before the warp may exit
     for (int s = waited; s < issued; s++) mbar_wait(&bk.mbar[s & 1], (uint32_t)(s >> 1) & 1u);
-    if (inside) {
-        if (T != 0.0f) T_out = T;
-        const size_t HW = (size_t)a.H * a.W;
-        const size_t pix = (size_t)py * a.W + px;
-        a.final_T[v * HW + pix] = T_out;
-        a.n_contrib[v * HW + pix] = last;
-        float *oc = a.out_color + (size_t)v * 3 * HW;
-        oc[pix] = ffma(T_out, a.bg[0], C0);
-        oc[HW + pix] = ffma(T_out, a.bg[1], C1);
-        oc[2 * HW + pix] = ffma(T_out, a.bg[2], C2);
-        a.out_depth[v * HW + pix] = Dd;
-        a.out_alpha[v * HW + pix] = Aa;
-    }
+    if (inside) fwd_store_pixel(a, v, px, py, p);
 }
 #endif // FWD_BULK
 
@@ -554,43 +550,48 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
             sl.rec[3 * s + 2] = g2;
         }
         __syncwarp();
-        const int cnt = __popc(mr);
-        for (int i = 0; i < cnt; i++) {
-            const float4 g0 = sl.rec[3 * i], q1 = sl.rec[3 * i + 1];
-            const int pos = (int)__float_as_uint(g0.z); // 0-based position in the tile list
-            const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
-            const float power = power_prescaled(q1.x, q1.y, q1.z, dx, dy);
-            const float G = gs_exp(power);
-            const float alpha = fminf(GS_ALPHA_MAX, fmul(q1.w, G));
-            const bool contrib = (pos < last) && !(power > 0.0f) && !(alpha < GS_ALPHA_MIN);
-            // (every entry the contributor mask staged has a contributing lane: no vote)
-            float q = 0.f, w = 0.f;
-            if (contrib) {
-                const float4 q2 = sl.rec[3 * i + 2];
+        // The chunk's hits in runs that end at the next flush: one counter (np, the park slot) per hit, and the slab, park
+        // and slot-table addresses advance as running pointers.
+        const float4 *s = sl.rec;
+        for (int left = __popc(mr); left > 0;) {
+            const int run = min(left, BWD_PARK - np);
+            left -= run;
+            float2 *pq = &pk.qw[np][lane];
+            for (const int stop = np + run; np < stop; np++, s += 3, pq += 33) {
+                const float4 g0 = s[0], q1 = s[1], q2 = s[2];
+                const int pos = (int)__float_as_uint(g0.z); // 0-based position in the tile list
+                const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
+                const float power = power_prescaled(q1.x, q1.y, q1.z, dx, dy);
+                const float G = gs_exp(power);
+                const float alpha = fminf(GS_ALPHA_MAX, fmul(q1.w, G));
+                const bool contrib = (pos < last) & !(power > 0.0f) & !(alpha < GS_ALPHA_MIN);
+                // (every entry the contributor mask staged has a contributing lane: no vote.)  The pixel's update is
+                // computed on every lane and selected: a lane that does not contribute keeps T, rg, last_cg and last_alpha
+                // and parks (0, 0).
                 const float cg = fmaf(q2.x, gC0, fmaf(q2.y, gC1, fmaf(q2.z, gC2, fmaf(q2.w, gD, gA))));
                 const float one_m_a = 1.0f - alpha;
-                float inv; // 1/(1-alpha), 1-alpha in [0.01, 1)
+                float inv; // 1/(1-alpha), 1-alpha in [0.01, 1) where the lane contributes
                 asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv) : "f"(one_m_a));
 #if BWD_T_DIV == 2
-                T = __fdiv_rn(T, one_m_a); // the oracle's operation, bit for bit
+                const float Tc = __fdiv_rn(T, one_m_a); // the oracle's operation, bit for bit
 #elif BWD_T_DIV == 1
                 inv = fmaf(fmaf(-one_m_a, inv, 1.0f), inv, inv); // one Newton step: removes the MUFU reciprocal's bias, which a
-                T = T * inv;                                      // list thousands of contributors deep would otherwise compound
+                const float Tc = T * inv;                         // list thousands of contributors deep would otherwise compound
 #else
-                T = T * inv;
+                const float Tc = T * inv;
 #endif
-                w = alpha * T;
-                rg = fmaf(last_alpha, last_cg - rg, rg);
-                last_cg = cg;
-                last_alpha = alpha;
-                const float dL_dalpha = fmaf(T, cg - rg, -(Kbg * inv));
-                q = G * dL_dalpha;
+                const float rgc = fmaf(last_alpha, last_cg - rg, rg);
+                const float dL_dalpha = fmaf(Tc, cg - rgc, -(Kbg * inv));
+                T = contrib ? Tc : T;
+                rg = contrib ? rgc : rg;
+                last_cg = contrib ? cg : last_cg;
+                last_alpha = contrib ? alpha : last_alpha;
+                // park (q, w); the flush forms the six moments of q over the patch (1, dx, dy, dx^2, dx*dy, dy^2; the conic /
+                // mean combination is linear and happens once per Gaussian in B2) and the four weights of w
+                *pq = contrib ? make_float2(G * dL_dalpha, alpha * Tc) : make_float2(0.f, 0.f);
+                if (lane == 0) pk.hit[np] = g0;
             }
-            // park (q, w); the flush forms the six moments of q over the patch (1, dx, dy, dx^2, dx*dy, dy^2; the conic /
-            // mean combination is linear and happens once per Gaussian in B2) and the four weights of w
-            pk.qw[np][lane] = make_float2(q, w);
-            if (lane == 0) pk.hit[np] = g0;
-            if (++np == BWD_PARK) {
+            if (np == BWD_PARK) {
                 park_flush(pk, np, lane, fx0, fy_part, sgrad);
                 np = 0;
             }
