@@ -417,6 +417,37 @@ int b200gs_densify_move(int32_t role, int32_t P, int32_t row_floats, const int32
     return B200GS_OK;
 }
 
+int b200gs_adam_packed(const b200gs_adam_cfg *cfg, float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
+                       void *stream)
+{
+    if (!cfg || !params || !grads || !exp_avg || !exp_avg_sq || cfg->P < 0) return B200GS_E_ARGS;
+    for (const void *p : {(const void *)params, (const void *)grads, (const void *)exp_avg, (const void *)exp_avg_sq})
+        if ((uintptr_t)p % 16) return B200GS_E_ARGS;
+    if (cfg->sh_coeffs < 1 || cfg->total < 0 || cfg->total % 4) return B200GS_E_RANGE;
+    AdamArgs a;
+    const int64_t P = cfg->P;
+    const int64_t off[5] = {cfg->off_xyz, cfg->off_scaling, cfg->off_rotation, cfg->off_opacity, cfg->off_sh};
+    const int64_t numel[5] = {3 * P, 3 * P, 4 * P, P, 3 * (int64_t)cfg->sh_coeffs * P};
+    const int group[5] = {ADAM_GROUP_XYZ, ADAM_GROUP_SCALING, ADAM_GROUP_ROTATION, ADAM_GROUP_OPACITY, ADAM_GROUP_F_REST};
+    int64_t end = 0;
+    for (int f = 0; f < 5; f++) {
+        if (off[f] < end || off[f] % 4) return B200GS_E_RANGE; // fields in buffer order, disjoint, 16-byte aligned
+        end = off[f] + numel[f];
+        a.off[f] = off[f]; a.numel[f] = numel[f]; a.field_group[f] = group[f];
+    }
+    if (end > cfg->total) return B200GS_E_RANGE;
+    a.sh_coeffs = cfg->sh_coeffs;
+    a.lerp_small = fabsf(cfg->one_minus_beta1) < 0.5f;
+    for (int g = 0; g < 6; g++) a.step_size[g] = cfg->step_size[g];
+    a.bias_correction2_sqrt = cfg->bias_correction2_sqrt; a.one_minus_beta1 = cfg->one_minus_beta1; a.beta2 = cfg->beta2;
+    a.one_minus_beta2 = cfg->one_minus_beta2; a.eps = cfg->eps;
+    if (cfg->total == 0) return B200GS_OK;
+    launch_adam_packed(a, cfg->total, params, grads, exp_avg, exp_avg_sq, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "adam_packed launch");
+    return B200GS_OK;
+}
+
 int b200gs_test_sort_pairs(uint32_t *keys_a, uint32_t *keys_b, uint32_t *vals_a, uint32_t *vals_b, int64_t n, int32_t nbits,
                            void *scratch, size_t scratch_bytes, int32_t *result_in_b, void *stream)
 {

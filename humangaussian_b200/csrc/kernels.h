@@ -124,3 +124,18 @@ void launch_densify_plan(const DensifyCfg &c, int P, const float *accum, const f
                          int *plan, int *counts, char *scratch, cudaStream_t st);
 void launch_densify_move(int role, int P, int rf, const int *plan, const float *src, float *dst, int n_split, int S_sel, int S_kept,
                          const float *rotation, const float *scaling, const float *noise, cudaStream_t st);
+
+// Adam over the packed buffer (optim.cu).  Groups in the reference's order (gaussian_model.py:156-163).
+enum { ADAM_GROUP_XYZ = 0, ADAM_GROUP_F_DC = 1, ADAM_GROUP_F_REST = 2, ADAM_GROUP_OPACITY = 3, ADAM_GROUP_SCALING = 4,
+       ADAM_GROUP_ROTATION = 5 };
+struct AdamArgs {
+    int64_t off[5];      // field offsets (floats) in buffer order xyz, scaling, rotation, opacity, sh; ascending, multiples of 4
+    int64_t numel[5];    // 3P, 3P, 4P, P, 3*sh_coeffs*P
+    int field_group[5];  // group of each field (the sh field's is chosen per element: f_dc or f_rest)
+    int sh_coeffs;
+    int lerp_small;      // |1-beta1| < 0.5: the branch ATen's lerp() takes
+    float step_size[6];  // -(lr_g / bias_correction1), by group
+    float bias_correction2_sqrt, one_minus_beta1, beta2, one_minus_beta2, eps;
+};
+void launch_adam_packed(const AdamArgs &a, int64_t total, float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
+                        cudaStream_t st);

@@ -15,6 +15,8 @@ bookkeeping that feeds it (threestudio/systems/GaussianDreamer.py:378-408), with
 rotation); `moments` maps the same names to (exp_avg, exp_avg_sq) or is None.  Where the reference runs ~30 PyTorch ops
 with a host sync per boolean-mask gather and concatenates every tensor twice, this plans all destinations with one
 prefix-sum pass and moves each surviving row once (csrc/densify.cu); one host read-back (the five counts) per call.
+`densify_and_prune_packed` / `prune_only_packed` run the same plan on the packed parameter buffer of an
+`optim.PackedAdam`, moving every field of it and of its two moment buffers straight into new flat buffers.
 There is no CPU path: tensors must live on a CUDA device.
 """
 from __future__ import annotations
@@ -87,8 +89,53 @@ def add_densification_stats(stats: DensifyStats, viewspace_grads: torch.Tensor, 
                                       _ptr(stats.max_radii2D), _stream(g.device)), "densify_stats")
 
 
+class _Surgery:
+    """One planned densify / prune: the plan on the device, its five counts read back once (P_new sizes every
+    destination), and the children's noise.  `move` realises the plan for one [P, ...] array into a [P_new, ...]
+    destination, which may be a view into a larger buffer (the packed form moves each field into its place in the new
+    flat buffer).  Callers run inside `torch.cuda.device(dev)`.  P >= 1."""
+
+    def __init__(self, cfg: _Cfg, stats: DensifyStats, opacity, scaling, rotation, noise, generator):
+        L = self.L = load_library()
+        dev, P = scaling.device, scaling.shape[0]
+        self.cfg, self.dev, self.P, self.rotation, self.scaling = cfg, dev, P, rotation, scaling
+        self.n_split = cfg.n_split if cfg.mode == 0 else 0
+        self.plan = torch.empty(4, P, dtype=torch.int32, device=dev)
+        counts = torch.empty(5, dtype=torch.int32, device=dev)
+        scratch = torch.empty(L.b200gs_densify_scratch_bytes(P), dtype=torch.uint8, device=dev)
+        self.st = _stream(dev)
+        _check(L.b200gs_densify_plan(P, C.byref(cfg), _ptr(stats.xyz_gradient_accum), _ptr(stats.denom), _ptr(opacity),
+                                     _ptr(scaling), _ptr(self.plan), _ptr(counts), _ptr(scratch), scratch.numel(), self.st), "densify_plan")
+        self.counts = counts.cpu()  # the one host sync of the call
+        n_keep, n_clone, S_sel, S_kept, P_new = (int(x) for x in self.counts)
+        self.P_new = P_new
+        self.ch = (C.c_int32 * 5)(n_keep, n_clone, S_sel, S_kept, P_new)
+        if cfg.mode == 0 and noise is None:
+            # torch.normal(mean=0, std=stds) == randn * stds (gaussian_model.py:369-371)
+            noise = torch.randn(self.n_split * S_sel, 3, dtype=torch.float32, device=dev, generator=generator)
+        if noise is not None:
+            noise = noise.to(device=dev, dtype=torch.float32).contiguous()
+            if noise.numel() != self.n_split * S_sel * 3:
+                raise ValueError(f"b200gs: noise must hold {self.n_split * S_sel} rows of 3 standard-normal draws")
+        self.noise = noise
+
+    def move(self, role, src: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
+        rf = src.numel() // self.P
+        if rf == 0:  # e.g. f_rest [P,0,3] at SH degree 0
+            return dst
+        _check(self.L.b200gs_densify_move(role, self.P, rf, _ptr(self.plan), self.ch, self.n_split, _ptr(src), _ptr(dst),
+                                          _ptr(self.rotation), _ptr(self.scaling), _ptr(self.noise), self.st), "densify_move")
+        return dst
+
+    def new_stats(self, stats: DensifyStats) -> DensifyStats:
+        if self.cfg.mode == 0:  # densification_postfix resets all three statistics (gaussian_model.py:358-360)
+            return DensifyStats.zeros(self.P_new, self.dev)
+        # prune_points gathers them (gaussian_model.py:310-315)
+        out = lambda t: self.move(ROLE_COPY, t, torch.empty((self.P_new,) + tuple(t.shape[1:]), dtype=torch.float32, device=self.dev))
+        return DensifyStats(out(stats.xyz_gradient_accum), out(stats.denom), out(stats.max_radii2D))
+
+
 def _run(cfg: _Cfg, params: Dict[str, torch.Tensor], moments, stats: DensifyStats, noise, generator):
-    L = load_library()
     xyz = params["xyz"]
     _need_cuda(xyz)
     dev, P = xyz.device, xyz.shape[0]
@@ -96,43 +143,18 @@ def _run(cfg: _Cfg, params: Dict[str, torch.Tensor], moments, stats: DensifyStat
     if P == 0:
         return ({k: v.clone() for k, v in src.items()}, None if moments is None else {k: (m.clone(), v.clone()) for k, (m, v) in moments.items()},
                 DensifyStats.zeros(0, dev), torch.zeros(5, dtype=torch.int32))
-    n_split = cfg.n_split if cfg.mode == 0 else 0
     with torch.cuda.device(dev):
-        plan = torch.empty(4, P, dtype=torch.int32, device=dev)
-        counts = torch.empty(5, dtype=torch.int32, device=dev)
-        scratch = torch.empty(L.b200gs_densify_scratch_bytes(P), dtype=torch.uint8, device=dev)
-        st = _stream(dev)
-        _check(L.b200gs_densify_plan(P, C.byref(cfg), _ptr(stats.xyz_gradient_accum), _ptr(stats.denom), _ptr(src["opacity"]),
-                                     _ptr(src["scaling"]), _ptr(plan), _ptr(counts), _ptr(scratch), scratch.numel(), st), "densify_plan")
-        host = counts.cpu()  # the one host sync of the call: P_new sizes every destination
-        n_keep, n_clone, S_sel, S_kept, P_new = (int(x) for x in host)
-        ch = (C.c_int32 * 5)(n_keep, n_clone, S_sel, S_kept, P_new)
-        if cfg.mode == 0 and noise is None:
-            # torch.normal(mean=0, std=stds) == randn * stds (gaussian_model.py:369-371)
-            noise = torch.randn(n_split * S_sel, 3, dtype=torch.float32, device=dev, generator=generator)
-        if noise is not None:
-            noise = noise.to(device=dev, dtype=torch.float32).contiguous()
-            if noise.numel() != n_split * S_sel * 3:
-                raise ValueError(f"b200gs: noise must hold {n_split * S_sel} rows of 3 standard-normal draws")
+        s = _Surgery(cfg, stats, src["opacity"], src["scaling"], src["rotation"], noise, generator)
 
         def move(role, t):
-            rf = t.numel() // P
-            out = torch.empty((P_new,) + tuple(t.shape[1:]), dtype=torch.float32, device=dev)
-            if rf == 0:  # e.g. f_rest [P,0,3] at SH degree 0
-                return out
-            _check(L.b200gs_densify_move(role, P, rf, _ptr(plan), ch, n_split, _ptr(t), _ptr(out), _ptr(src["rotation"]),
-                                         _ptr(src["scaling"]), None if noise is None else _ptr(noise), st), "densify_move")
-            return out
+            return s.move(role, t, torch.empty((s.P_new,) + tuple(t.shape[1:]), dtype=torch.float32, device=dev))
         roles = {"xyz": ROLE_XYZ, "scaling": ROLE_SCALING}
         new_params = {k: move(roles.get(k, ROLE_COPY), src[k]) for k in GROUPS}
         new_moments = None
         if moments is not None:
             new_moments = {k: tuple(move(ROLE_MOMENT, m.detach().to(torch.float32).contiguous()) for m in moments[k]) for k in GROUPS}
-        if cfg.mode == 0:   # densification_postfix resets all three statistics (gaussian_model.py:358-360)
-            new_stats = DensifyStats.zeros(P_new, dev)
-        else:               # prune_points gathers them (gaussian_model.py:310-315)
-            new_stats = DensifyStats(move(ROLE_COPY, stats.xyz_gradient_accum), move(ROLE_COPY, stats.denom), move(ROLE_COPY, stats.max_radii2D))
-    return new_params, new_moments, new_stats, host
+        new_stats = s.new_stats(stats)
+    return new_params, new_moments, new_stats, s.counts
 
 
 def densify_and_prune(params, moments, stats: DensifyStats, max_grad: float, min_opacity: float, extent: float,
@@ -152,6 +174,66 @@ def prune_only(params, moments, stats: DensifyStats, min_opacity: float = 0.005,
     cfg = _Cfg(1, 0, 0, 0.0, float(min_opacity), 0.0, 0.0, float(size_thresh))
     p, m, s, counts = _run(cfg, params, moments, stats, None, None)
     return (p, m, s, counts) if return_counts else (p, m, s)
+
+
+# ---- the same surgery on the packed parameter buffer, for optim.PackedAdam -----------------------------------------
+def _run_packed(cfg: _Cfg, opt: torch.optim.Optimizer, stats: DensifyStats, noise, generator) -> int:
+    """Plan once from the flat buffer's opacity / scaling fields, move every field of the parameter buffer and of both
+    Adam moment buffers straight into its place in new flat buffers (padding zero), install them into `opt`, and replace
+    the three tensors of `stats` in place.  The optimiser's step count is kept."""
+    from .rasterizer import packed_layout
+    group = opt.param_groups[0]
+    old = group["params"][0]
+    _need_cuda(old)
+    P, K, dev = int(group["P"]), int(group["sh_coeffs"]), old.device
+    if P == 0:
+        return 0
+    fields = packed_layout(P, K)[0]
+    views = lambda flat, layout: [flat.narrow(0, o, n).view(shape) for o, n, shape in layout]
+    xyz, scaling, rotation, opacity, sh = views(old.detach(), fields)
+    state = opt.state.get(old)
+    with torch.cuda.device(dev):
+        s = _Surgery(cfg, stats, opacity, scaling, rotation, noise, generator)
+        new_fields, new_total = packed_layout(s.P_new, K)
+
+        def remap(flat, roles):
+            out = torch.zeros(new_total, dtype=torch.float32, device=dev)  # alignment padding stays zero
+            for src, dst, role in zip(views(flat, fields), views(out, new_fields), roles):
+                s.move(role, src, dst)
+            return out
+        new_flat = remap(old.detach(), (ROLE_XYZ, ROLE_SCALING, ROLE_COPY, ROLE_COPY, ROLE_COPY))
+        new_moments = None
+        if state:
+            new_moments = tuple(remap(state[k], (ROLE_MOMENT,) * 5) for k in ("exp_avg", "exp_avg_sq"))
+        new_stats = s.new_stats(stats)
+    # what _prune_optimizer / cat_tensors_to_optimizer do (gaussian_model.py:284-341): new leaf, moved moments, same step
+    leaf = torch.nn.Parameter(new_flat) if isinstance(old, torch.nn.Parameter) else new_flat.requires_grad_(True)
+    group["params"][0] = leaf
+    group["P"] = s.P_new
+    opt.state.pop(old, None)
+    if new_moments is not None:
+        state["exp_avg"], state["exp_avg_sq"] = new_moments
+        opt.state[leaf] = state
+    stats.xyz_gradient_accum, stats.denom, stats.max_radii2D = new_stats.xyz_gradient_accum, new_stats.denom, new_stats.max_radii2D
+    return s.P_new
+
+
+def densify_and_prune_packed(opt: torch.optim.Optimizer, stats: DensifyStats, max_grad: float, min_opacity: float, extent: float,
+                             max_screen_size: Optional[float], percent_dense: float = 0.01, N: int = 2,
+                             noise: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None) -> int:
+    """`densify_and_prune` on the packed buffer of an `optim.PackedAdam`: same plan, same rows, same noise rows, but every
+    field of the parameter buffer and of both moment buffers is moved straight into a new flat buffer of the same layout.
+    The new buffer becomes the optimiser's parameter (`opt.packed`), `stats` is replaced in place, and the new P is
+    returned.  Equal bit for bit to densify_and_prune on the unpacked groups followed by dist.pack."""
+    cfg = _Cfg(0, int(N), 1 if max_screen_size else 0, float(max_grad), float(min_opacity), float(percent_dense * extent),
+               float(max_screen_size or 0.0), float(0.1 * extent))
+    return _run_packed(cfg, opt, stats, noise, generator)
+
+
+def prune_only_packed(opt: torch.optim.Optimizer, stats: DensifyStats, min_opacity: float = 0.005, size_thresh: float = 0.01) -> int:
+    """`prune_only` on the packed buffer of an `optim.PackedAdam` (see densify_and_prune_packed); returns the new P."""
+    cfg = _Cfg(1, 0, 0, 0.0, float(min_opacity), 0.0, 0.0, float(size_thresh))
+    return _run_packed(cfg, opt, stats, None, None)
 
 
 def moments_from_optimizer(optimizer: torch.optim.Optimizer) -> Dict[str, Tuple[torch.Tensor, torch.Tensor]]:

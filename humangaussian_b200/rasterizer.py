@@ -65,7 +65,7 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_last_cuda_error", "b200gs_abi_version", "b200gs_launch_count", "b200gs_profile_enable", "b200gs_profile_read",
            "b200gs_test_sort_pairs", "b200gs_test_sort_scratch_bytes", "b200gs_reattach", "b200gs_pack_frames_u8",
            "b200gs_knn_scratch_bytes", "b200gs_dist2_knn3", "b200gs_densify_stats", "b200gs_densify_scratch_bytes",
-           "b200gs_densify_plan", "b200gs_densify_move"]
+           "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -113,6 +113,8 @@ def load_library():
     L.b200gs_densify_plan.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
     L.b200gs_densify_move.restype = C.c_int
     L.b200gs_densify_move.argtypes = [i32, i32, i32, vp, C.POINTER(i32), i32, vp, vp, vp, vp, vp, vp]
+    L.b200gs_adam_packed.restype = C.c_int
+    L.b200gs_adam_packed.argtypes = [vp, vp, vp, vp, vp, vp]
     L.b200gs_last_cuda_error.restype = C.c_char_p
     L.b200gs_launch_count.restype = i64
     L.b200gs_profile_enable.restype = None; L.b200gs_profile_enable.argtypes = [C.c_int]

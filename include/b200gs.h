@@ -197,6 +197,30 @@ int b200gs_densify_move(int32_t role, int32_t P, int32_t row_floats, const int32
                         int32_t n_split, const float *src, float *dst, const float *rotation_raw, const float *scaling_raw,
                         const float *noise, void *stream);
 
+/* ---- Adam over the packed parameter buffer (the reference's optimiser, gaussian_model.py:156-165) ------------------
+ * One step of torch.optim.Adam (amsgrad=False, weight_decay=0, maximize=False) over the flat fp32 buffer
+ * [xyz 3P | scaling 3P | rotation 4P | opacity P | sh 3*sh_coeffs*P] that the packed forward reads and the packed backward
+ * writes the gradient of, with the reference's six parameter groups: xyz, scaling, rotation and opacity are one field each;
+ * inside the sh field [P,sh_coeffs,3] coefficient 0 is f_dc and coefficients 1.. are f_rest.  exp_avg / exp_avg_sq have the
+ * same layout.  Floats outside the five fields (alignment padding) are written as zero in params and both moments.
+ * The scalars are what torch computes on the host for step t, in double, rounded to float:
+ *   step_size[g] = -(lr_g / (1 - beta1^t)),  bias_correction2_sqrt = (1 - beta2^t)^0.5. */
+typedef struct b200gs_adam_cfg {
+    int64_t off_xyz, off_scaling, off_rotation, off_opacity, off_sh; /* field offsets in floats: ascending, multiples of 4 */
+    int32_t P;
+    int32_t sh_coeffs;           /* K >= 1 */
+    int64_t total;               /* floats in each buffer; a multiple of 4 */
+    float step_size[6];          /* by group: xyz, f_dc, f_rest, opacity, scaling, rotation */
+    float bias_correction2_sqrt;
+    float one_minus_beta1;
+    float beta2;
+    float one_minus_beta2;
+    float eps;
+} b200gs_adam_cfg;
+/* params, exp_avg, exp_avg_sq updated in place; grads read.  All four 16-byte aligned, `total` floats each. */
+int b200gs_adam_packed(const b200gs_adam_cfg *cfg, float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
+                       void *stream);
+
 /* ---- introspection of the state buffers, for parity tests (tile/sort indices must match bit-for-bit) ------- */
 typedef struct b200gs_state_view {
     const void *geom_records;     /* [V*P] x 48 B: px,py,hx,hy | conicA,conicB,conicC,opacity | r,g,b,depth */
