@@ -169,6 +169,9 @@ void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st)
     classic_bwd<<<grid, BLOCK_SIZE, 0, st>>>(a);
 }
 int blend_sgrad_is_moments() { return 0; }
+// no deterministic backward here: b200gs_backward_deterministic returns B200GS_E_UNSUPPORTED before it would launch this
+int blend_bwd_has_deterministic() { return 0; }
+void launch_blend_bwd_det(const BlendBwdArgs &, const DetFlush &, cudaStream_t) {}
 __global__ void classic_exp_kernel(const float *x, float *y, int64_t n)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

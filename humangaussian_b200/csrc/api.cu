@@ -211,16 +211,29 @@ int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *
     return B200GS_OK;
 }
 
-int b200gs_backward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
-                    const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
-                    const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                    const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth,
-                    const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                    float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
-                    size_t scratch_bytes, void *stream)
+size_t b200gs_deterministic_bytes(int64_t num_rendered, int64_t partial_capacity, int32_t P, int32_t V)
 {
-    (void)num_rendered;
+    return DetLayout(num_rendered, partial_capacity, (int64_t)(P > 0 ? P : 0) * (V > 0 ? V : 0)).total;
+}
+
+// b200gs_backward (det == false) and b200gs_backward_deterministic (det == true)
+static int backward_impl(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
+                         const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
+                         const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                         const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                         const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth,
+                         const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                         float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
+                         size_t scratch_bytes, void *stream, bool det, void *det_buf, size_t det_bytes, int64_t partial_capacity,
+                         int64_t *n_partials)
+{
+    if (det) {
+        if (!blend_bwd_has_deterministic()) return B200GS_E_UNSUPPORTED;
+        if (!n_partials || !det_buf || partial_capacity < 0) return B200GS_E_ARGS;
+        *n_partials = 0;
+        if (num_rendered < 0 || num_rendered > instance_capacity || num_rendered > B200GS_MAX_INSTANCES) return B200GS_E_ARGS;
+        if (((uintptr_t)det_buf) & 15) return B200GS_E_BUFFER;
+    }
     int rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
     if (prm->raw_params && !opacities) return B200GS_E_ARGS;
@@ -239,8 +252,11 @@ int b200gs_backward(const b200gs_params *prm, const float *means3D, const float 
     if (scratch_bytes < b200gs_backward_scratch_bytes(P, V)) return B200GS_E_BUFFER;
     if ((((uintptr_t)geom_buf) | ((uintptr_t)binning_buf) | ((uintptr_t)image_buf) | ((uintptr_t)scratch)) & 15) return B200GS_E_BUFFER;
     const char *gb = (const char *)geom_buf, *bb = (const char *)binning_buf, *ib = (const char *)image_buf;
+    const int64_t n_vp = (int64_t)P * V;
+    const DetLayout DL(num_rendered, partial_capacity, n_vp);
+    if (det && det_bytes < DL.total) return B200GS_E_BUFFER;
 
-    CK(cudaMemsetAsync(scratch, 0, (size_t)P * V * sizeof(ScreenGrad), st), "memset scratch");
+    if (!det) CK(cudaMemsetAsync(scratch, 0, (size_t)P * V * sizeof(ScreenGrad), st), "memset scratch");
     BlendBwdArgs b;
     b.H = H; b.W = W; b.grid_x = gx; b.grid_y = gy; b.V = V; b.P = P;
     b.ranges = (const uint2 *)(bb + BL.ranges); b.point_list = (const uint32_t *)(bb + BL.vals_out);
@@ -250,7 +266,43 @@ int b200gs_backward(const b200gs_params *prm, const float *means3D, const float 
     b.dL_dcolor = dL_dcolor; b.dL_ddepth = dL_ddepth; b.dL_dalpha = dL_dalpha;
     b.cmask = (const uint32_t *)(bb + BL.cmask);
     b.sgrad = scratch;
-    { StageTimer t(B200GS_STAGE_BLEND_BWD, st); launch_blend_bwd(b, st); }
+    if (!det) {
+        StageTimer t(B200GS_STAGE_BLEND_BWD, st);
+        launch_blend_bwd(b, st);
+    } else {
+        // pre-pass -> (the one host wait: the partial count) -> B1 with per-partial stores -> fixed-order reduce.  The wait
+        // sits after the scan so that a call whose partials do not fit returns before B1 runs; every access of the pre-pass
+        // stays inside buffers sized by num_rendered and P*V alone.
+        StageTimer t(B200GS_STAGE_BLEND_BWD, st);
+        char *db = (char *)det_buf;
+        DetPlanArgs pa;
+        pa.H = H; pa.W = W; pa.grid_x = gx; pa.grid_y = gy; pa.D = num_rendered;
+        pa.tile_order = b.tile_order; pa.ranges = b.ranges; pa.point_list = b.point_list; pa.cmask = b.cmask; pa.n_contrib = b.n_contrib;
+        pa.rects = (const uint2 *)(gb + GL.rects);
+        pa.order = (const uint32_t *)(bb + BL.order_in); // the depth order (four ping-pong passes end where they began)
+        pa.offsets = (const uint32_t *)(gb + GL.offsets); pa.tiles_touched = (const uint32_t *)(gb + GL.tiles_touched);
+        pa.start = (uint32_t *)(db + DL.start); pa.pm = (uint8_t *)(db + DL.pm); pa.base = (uint32_t *)(db + DL.base);
+        pa.jpos = (uint32_t *)(db + DL.jpos);
+        uint64_t H_partials = 0;
+        if (num_rendered > 0) {
+            int nl = 0;
+            if (launch_det_plan(pa, n_vp, gx * gy * V, DL, db, st, &nl)) return cuda_fail(cudaGetLastError(), "deterministic plan");
+            g_launches += nl;
+            HostSlot *hs = host_slot();
+            if (!hs) return cuda_fail(cudaGetLastError(), "pinned count slot");
+            CK(cudaMemcpyAsync(hs->total, db + DL.total_slot, 8, cudaMemcpyDeviceToHost, st), "D2H partial count");
+            CK(cudaEventRecord(hs->ev, st), "event after partial count");
+            CK(cudaEventSynchronize(hs->ev), "wait for the partial count");
+            H_partials = *hs->total;
+        }
+        *n_partials = (int64_t)H_partials;
+        if (H_partials > 0xffffffffull) return B200GS_E_RANGE; // 32-bit slots; 160 GB of partials would not fit a device anyway
+        if ((int64_t)H_partials > partial_capacity) return B200GS_E_BIN_TOO_SMALL;
+        float *partials = (float *)(db + DL.partials);
+        if (H_partials > 0) launch_blend_bwd_det(b, DetFlush{pa.pm, pa.base, partials}, st);
+        launch_det_reduce(pa, n_vp, partials, scratch, st);
+        g_launches += (H_partials > 0) + 1;
+    }
 
     PreBwdArgs a;
     a.P = P; a.V = V; a.deg = shs ? prm->sh_degree : 0; a.M = prm->sh_coeffs; a.H = H; a.W = W; a.mod = prm->scale_modifier;
@@ -265,9 +317,40 @@ int b200gs_backward(const b200gs_params *prm, const float *means3D, const float 
     a.dL_dmeans3D = dL_dmeans3D; a.dL_dmeans2D = dL_dmeans2D; a.dL_dsh = dL_dsh; a.dL_dcolors = dL_dcolors;
     a.dL_dopacity = dL_dopacity; a.dL_dscales = dL_dscales; a.dL_drots = dL_drots; a.dL_dcov3D = dL_dcov3D;
     { StageTimer t(B200GS_STAGE_PREPROCESS_BWD, st); launch_preprocess_bwd(a, st); }
-    g_launches += 2;
+    g_launches += det ? 1 : 2; // (the deterministic blend stage counted its own launches)
     CK(cudaGetLastError(), "backward launch");
     return B200GS_OK;
+}
+
+int b200gs_backward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
+                    const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
+                    const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                    const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth,
+                    const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                    float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
+                    size_t scratch_bytes, void *stream)
+{
+    return backward_impl(prm, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr);
+}
+
+int b200gs_backward_deterministic(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
+                                  const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                  const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                  const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                  const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth,
+                                  const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                                  float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
+                                  size_t scratch_bytes, void *det_buf, size_t det_bytes, int64_t partial_capacity,
+                                  int64_t *n_partials, void *stream)
+{
+    return backward_impl(prm, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials);
 }
 
 int b200gs_mark_visible(int32_t P, const float *positions, const float *viewmatrix, const float *projmatrix,

@@ -113,11 +113,28 @@ int launch_depth_order(const uint32_t *tiles_touched, uint32_t *offsets_sorted, 
     const size_t nblocks = (size_t)((n_vp + SCAN_TILE - 1) / SCAN_TILE);
     char *scr = bin_base + L.temp;
     cudaMemsetAsync(scr, 0, gs_align((nblocks + 1) * 8) + 256, st);
-    scan_tiles_kernel<<<(unsigned)nblocks, THREADS, 0, st>>>(vs, tiles_touched, offsets_sorted, n_vp, (volatile uint64_t *)(scr + 256),
-                                                            (uint32_t *)scr, (uint64_t *)(bin_base + L.total_slot));
+    lookback_scan_kernel<<<(unsigned)nblocks, THREADS, 0, st>>>(GatherLoad{vs, tiles_touched}, offsets_sorted, n_vp,
+                                                               (volatile uint64_t *)(scr + 256), (uint32_t *)scr,
+                                                               (uint64_t *)(bin_base + L.total_slot));
     *total_dev = (const uint64_t *)(bin_base + L.total_slot);
     *n_launches += 1;
     return cudaPeekAtLastError() == cudaSuccess ? 0 : -2;
+}
+
+// The deterministic backward's partial counts: x[j] = popc(pm[j]), scanned with the same look-back kernel
+struct PopcLoad {
+    const uint8_t *pm;
+    __device__ __forceinline__ uint32_t operator()(int64_t j) const { return (uint32_t)__popc((uint32_t)__ldg(pm + j)); }
+};
+size_t popc_scan_temp_bytes(int64_t n) { return 256 + gs_align((size_t)((n + SCAN_TILE - 1) / SCAN_TILE + 1) * 8); }
+int launch_popc_scan(const uint8_t *pm, uint32_t *incl, int64_t n, char *temp, uint64_t *total, cudaStream_t st)
+{
+    if (n < 1) return -1;
+    if (cudaMemsetAsync(temp, 0, popc_scan_temp_bytes(n), st) != cudaSuccess) return -1;
+    lookback_scan_kernel<<<(unsigned)((n + SCAN_TILE - 1) / SCAN_TILE), THREADS, 0, st>>>(PopcLoad{pm}, incl, n,
+                                                                                        (volatile uint64_t *)(temp + 256),
+                                                                                        (uint32_t *)temp, total);
+    return cudaPeekAtLastError() == cudaSuccess ? 0 : -1;
 }
 
 // Instance emission, warp-cooperative.  A warp owns 32 consecutive Gaussians IN DEPTH ORDER; their instances form one

@@ -32,6 +32,9 @@
 //     no BSSY/BSYNC/BRA inside the pair, about 96 per 32-entry chunk of bookkeeping.  Backward 64 registers, 13.1 KB smem,
 //     no spills; 107 per unrolled pair of hits (53.5 per hit; about 65 with a branch around the contributing-lane block
 //     and separate slot / hit counters), plus the flush.
+//   * Deterministic mode (torch.use_deterministic_algorithms): blend_bwd_det_kernel is the same body with a flush that stores
+//     each (instance, patch) partial into its own slot instead of the REDs; deterministic.cu plans the slots and adds each
+//     Gaussian's partials in a fixed order.  blend_bwd_kernel's SASS does not change.
 //   * The compile-time switches below are the A/B experiments DESIGN.md section 5 lists: the
 //     product is BWD_T_DIV=1 and BWD_PARK=16, everything else 0.
 #include "common.cuh"
@@ -416,7 +419,14 @@ __device__ __forceinline__ void red_add_v2(float *p, float a, float b)
 // constant, so the row accumulates sum q, sum q*dx, sum q*dx^2 and folds dy in once per row; dx and dy are the hit loop's
 // expressions.  The parts' sums meet in a (32 / BWD_PARK)-lane exchange, and the lanes of slot h write its record with a
 // v4 + v4 + v2 of vector REDs.
-__device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, float fx0, float fy_part, float *sgrad)
+// DET (the deterministic backward, DESIGN.md section 5): the ten sums are this (instance, patch)'s partial; they are stored
+// with plain stores into its own 40-byte slot of det.partials, slot = base[j] - popc(pm[j] >> patch) (base is the inclusive
+// scan of popc(pm)), and det_reduce_kernel adds each Gaussian's partials in a fixed order.
+// The tile's range.x and the warp's patch are re-derived here from the kernel parameters (two cached loads per flush), not
+// kept live across the hit loop: at the 64-register cap that costs the default kernel nothing and keeps this one from spilling.
+template <bool DET>
+__device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, float fx0, float fy_part, float *sgrad,
+                                           const BlendBwdArgs &a, const DetFlush &det)
 {
     __syncwarp();
     const int h = lane % BWD_PARK, part = lane / BWD_PARK;
@@ -452,7 +462,19 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
         W0 += __shfl_xor_sync(FULL, W0, o); W1 += __shfl_xor_sync(FULL, W1, o); W2 += __shfl_xor_sync(FULL, W2, o);
         W3 += __shfl_xor_sync(FULL, W3, o);
     }
-    if (h < n) {
+    if (DET) {
+        if (h < n) {
+            // partial as S0, Sx | Sy, Sxx | Sxy, Syy | w.gC0, w.gC1 | w.gC2, w.gD: 40 bytes, 8-byte aligned
+            const uint32_t range_x = __ldg(&a.ranges[__ldg(a.tile_order + blockIdx.x / CTAS_PER_TILE)].x);
+            const int patch = (blockIdx.x % CTAS_PER_TILE) * WARPS_PER_CTA + (threadIdx.x >> 5);
+            const uint32_t j = range_x + __float_as_uint(s.z);
+            const uint32_t slot = __ldg(det.base + j) - (uint32_t)__popc((uint32_t)__ldg(det.pm + j) >> patch);
+            float2 *rec = reinterpret_cast<float2 *>(det.partials + (size_t)slot * DET_PARTIAL_FLOATS);
+            if (part == 0) { rec[0] = make_float2(S0, Sx); rec[1] = make_float2(Sy, Sxx); }
+            if (part == 1) { rec[2] = make_float2(Sxy, Syy); rec[3] = make_float2(W0, W1); }
+            if (part == (PARK_LANES > 2 ? 2 : 0)) rec[4] = make_float2(W2, W3);
+        }
+    } else if (h < n) {
         // ScreenGrad as moments: S0, Sx, Sy, Sxx | Sxy, Syy, w.gC0, w.gC1 | w.gC2, w.gD
         float *rec = sgrad + (size_t)__float_as_uint(s.w) * (sizeof(ScreenGrad) / sizeof(float));
         if (part < 2) {
@@ -464,7 +486,10 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
     __syncwarp();
 }
 
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_kernel(BlendBwdArgs a)
+// The body of both B1 kernels: DET selects the flush (vector REDs into ScreenGrad, or stores of per-(instance, patch)
+// partials); everything else is the same code.
+template <bool DET>
+__device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetFlush &det)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
     __shared__ WarpPark parks[WARPS_PER_CTA];
@@ -592,19 +617,37 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
                 if (lane == 0) pk.hit[np] = g0;
             }
             if (np == BWD_PARK) {
-                park_flush(pk, np, lane, fx0, fy_part, sgrad);
+                park_flush<DET>(pk, np, lane, fx0, fy_part, sgrad, a, det);
                 np = 0;
             }
         }
         __syncwarp();
     }
-    if (np > 0) park_flush(pk, np, lane, fx0, fy_part, sgrad);
+    if (np > 0) park_flush<DET>(pk, np, lane, fx0, fy_part, sgrad, a, det);
+}
+
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_kernel(BlendBwdArgs a)
+{
+    blend_bwd_body<false>(a, DetFlush{});
+}
+
+// B1 of the deterministic backward: a.sgrad is not touched; every flushed (instance, patch) partial goes to its own slot
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_kernel(BlendBwdArgs a, DetFlush det)
+{
+    blend_bwd_body<true>(a, det);
 }
 
 void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st)
 {
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
     blend_bwd_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
+}
+
+int blend_bwd_has_deterministic() { return 1; }
+void launch_blend_bwd_det(const BlendBwdArgs &a, const DetFlush &det, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
+    blend_bwd_det_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, det);
 }
 
 // ScreenGrad holds moments of q = G*dL/dalpha here: S0, Sx, Sy, Sxx, Sxy, Syy = sum q*{1, dx, dy, dx^2, dx*dy, dy^2};

@@ -96,6 +96,43 @@ size_t test_sort32_scratch_bytes(int64_t n);
 void launch_blend_fwd(const BlendArgs &a, cudaStream_t st);
 void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st);
 int blend_sgrad_is_moments(); // which ScreenGrad format the linked blend_bwd writes
+
+// ---- deterministic backward (deterministic.cu; B1's deterministic instantiation in blend.cu) ------------------------------
+// Every (sorted instance j, patch p) that B1 flushes gets its own partial slot; the reduce adds a Gaussian's partials in
+// emission order (the tiles of its rect row-major), patches ascending, so the sums depend on the forward state only.
+#define DET_PARTIAL_FLOATS 10 // S0, Sx, Sy, Sxx, Sxy, Syy, W0..W3: 40 bytes
+struct DetFlush {
+    const uint8_t *pm;    // [D] bit p: B1 flushes a partial for (j, patch p)
+    const uint32_t *base; // [D] inclusive scan of popc(pm) (exact: the total is checked to fit 32 bits)
+    float *partials;      // [H][DET_PARTIAL_FLOATS]
+};
+// det_buf carving; pm first (b200gs.h documents that the buffer starts with it)
+struct DetLayout {
+    size_t pm, base, jpos, start, scan_temp, total_slot, partials, total;
+    __host__ DetLayout(int64_t D, int64_t partial_capacity, int64_t n_vp);
+};
+struct DetPlanArgs {
+    int H, W, grid_x, grid_y;
+    int64_t D;
+    const uint32_t *tile_order; // [V*tiles]: the plan kernel runs one CTA per (view, tile), longest list first
+    const uint2 *ranges;
+    const uint32_t *point_list, *cmask, *n_contrib;
+    const uint2 *rects;         // [V*P] tile rect of each record (preprocess)
+    const uint32_t *order, *offsets, *tiles_touched; // depth order, inclusive scan of tiles_touched in it, tiles_touched
+    uint32_t *start;            // [V*P] emission start of each record
+    uint8_t *pm;
+    uint32_t *base, *jpos;      // [D], [D]: jpos[emission index] = sorted position
+};
+// inclusive scan of popc(pm[j]) over n instances (the binning stage's look-back scan, binning.cu): incl[j] keeps the low 32
+// bits, *total the exact sum; temp (popc_scan_temp_bytes) is zeroed by the call
+size_t popc_scan_temp_bytes(int64_t n);
+int launch_popc_scan(const uint8_t *pm, uint32_t *incl, int64_t n, char *temp, uint64_t *total, cudaStream_t st);
+int blend_bwd_has_deterministic(); // 0 in the classic comparator
+void launch_blend_bwd_det(const BlendBwdArgs &a, const DetFlush &det, cudaStream_t st);
+// start scatter, plan, scan of popc(pm) -> base and the exact 64-bit partial count at *total_dev
+int launch_det_plan(const DetPlanArgs &a, int64_t n_vp, int n_tiles_all, const DetLayout &L, char *det_base, cudaStream_t st,
+                    int *n_launches);
+void launch_det_reduce(const DetPlanArgs &a, int64_t n_vp, const float *partials, void *sgrad, cudaStream_t st);
 void launch_test_exp(const float *x, float *y, int64_t n, cudaStream_t st);
 
 // animation frame path (anim.cu)

@@ -234,15 +234,22 @@ __global__ void __launch_bounds__(THREADS) scatter_kernel(const KeyT *__restrict
     }
 }
 
-// ---- inclusive scan of x[k] = tiles[order[k]] with decoupled look-back (single pass over the data) ------------
+// ---- inclusive scan of x[k] = load(k) with decoupled look-back (single pass over the data) ------------
+// Loads: the binning stage scans tiles_touched in depth order (GatherLoad); the deterministic backward scans the partial
+// counts popc(pm[j]) of the sorted instances (PopcLoad, deterministic.cu).
 constexpr int SCAN_IPT = 8;
-__global__ void __launch_bounds__(THREADS) scan_tiles_kernel(const uint32_t *__restrict__ order, const uint32_t *__restrict__ tiles,
-                                                              uint32_t *__restrict__ out, int64_t n, volatile uint64_t *status /* [nblocks], zeroed */,
-                                                              uint32_t *ticket /* zeroed */, uint64_t *total_out /* exact 64-bit sum */)
+struct GatherLoad { // x[k] = tiles[order[k]]
+    const uint32_t *order, *tiles;
+    __device__ __forceinline__ uint32_t operator()(int64_t k) const { return __ldg(tiles + __ldg(order + k)); }
+};
+template <typename Load>
+__global__ void __launch_bounds__(THREADS) lookback_scan_kernel(const Load load, uint32_t *__restrict__ out, int64_t n,
+                                                                 volatile uint64_t *status /* [nblocks], zeroed */,
+                                                                 uint32_t *ticket /* zeroed */, uint64_t *total_out /* exact 64-bit sum */)
 {
-    // status: bit 63 = prefix ready, bit 62 = aggregate ready, low 56 bits = value (the exact running sum: V*P < 2^32
-    // entries of at most 2^24 tiles each cannot reach 2^56).  out[] keeps the low 32 bits; the host rejects a batch whose
-    // exact total does not fit BEFORE anything is emitted (api.cu).
+    // status: bit 63 = prefix ready, bit 62 = aggregate ready, low 56 bits = value (the exact running sum: fewer than 2^32
+    // entries of at most 2^24 each cannot reach 2^56).  out[] keeps the low 32 bits; the callers check the exact total before
+    // anything relies on the 32-bit values (api.cu).
     constexpr int TILE = THREADS * SCAN_IPT;
     __shared__ uint32_t s_bid, s_wsum[WARPS];
     __shared__ uint64_t s_excl;
@@ -255,7 +262,7 @@ __global__ void __launch_bounds__(THREADS) scan_tiles_kernel(const uint32_t *__r
     uint32_t tsum = 0;
 #pragma unroll
     for (int i = 0; i < SCAN_IPT; i++) {
-        x[i] = (base + i < n) ? tiles[order[base + i]] : 0u;
+        x[i] = (base + i < n) ? load(base + i) : 0u;
         tsum += x[i];
     }
     uint32_t incl = tsum;

@@ -32,7 +32,7 @@ ABI_VERSION = 4
 MAX_VIEWS = 64
 MAX_INSTANCES = 0x7FFFFFFF  # (Gaussian, tile) instances per call (B200GS_MAX_INSTANCES); larger batches are split by views
 
-OK, E_ARGS, E_BIN_TOO_SMALL, E_BUFFER, E_CUDA, E_RANGE, E_INSTANCES = 0, -1, -2, -3, -4, -5, -6
+OK, E_ARGS, E_BIN_TOO_SMALL, E_BUFFER, E_CUDA, E_RANGE, E_INSTANCES, E_UNSUPPORTED = 0, -1, -2, -3, -4, -5, -6, -7
 
 
 class InstanceLimitError(RuntimeError):
@@ -65,7 +65,8 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_last_cuda_error", "b200gs_abi_version", "b200gs_launch_count", "b200gs_profile_enable", "b200gs_profile_read",
            "b200gs_test_sort_pairs", "b200gs_test_sort_scratch_bytes", "b200gs_reattach", "b200gs_pack_frames_u8",
            "b200gs_knn_scratch_bytes", "b200gs_dist2_knn3", "b200gs_densify_stats", "b200gs_densify_scratch_bytes",
-           "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed"]
+           "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed", "b200gs_deterministic_bytes",
+           "b200gs_backward_deterministic"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -90,6 +91,10 @@ def load_library():
     L.b200gs_forward.argtypes = [C.POINTER(_Params)] + [vp] * 15 + [vp, sz, vp, sz, i64, vp, sz, C.POINTER(i64), vp]
     L.b200gs_backward.restype = C.c_int
     L.b200gs_backward.argtypes = [C.POINTER(_Params)] + [vp] * 12 + [vp, vp, i64, vp, i64] + [vp] * 11 + [vp, sz, vp]
+    L.b200gs_deterministic_bytes.restype = sz; L.b200gs_deterministic_bytes.argtypes = [i64, i64, i32, i32]
+    L.b200gs_backward_deterministic.restype = C.c_int
+    L.b200gs_backward_deterministic.argtypes = ([C.POINTER(_Params)] + [vp] * 12 + [vp, vp, i64, vp, i64] + [vp] * 11 + [vp, sz] +
+                                                [vp, sz, i64, C.POINTER(i64), vp])
     L.b200gs_mark_visible.restype = C.c_int
     L.b200gs_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
     L.b200gs_describe_state.restype = C.c_int
@@ -137,12 +142,14 @@ class use_library:
         self.saved = (_lib, LIB_PATH)
         _lib, LIB_PATH = None, self.path
         _pool.clear()
+        _det_pool.clear()
         return load_library()
 
     def __exit__(self, *exc):
         global _lib, LIB_PATH
         _lib, LIB_PATH = self.saved
         _pool.clear()
+        _det_pool.clear()
         return False
 
 
@@ -168,6 +175,7 @@ def _check(rc, what):
     L = load_library()
     msg = {E_ARGS: "inconsistent arguments", E_BUFFER: "state buffer too small", E_RANGE: "size outside supported range",
            E_INSTANCES: "too many (Gaussian, tile) instances in one call",
+           E_UNSUPPORTED: "not supported by this build of the library", E_BIN_TOO_SMALL: "buffer too small after retries",
            E_CUDA: "CUDA error: " + (L.b200gs_last_cuda_error() or b"").decode()}.get(rc, f"status {rc}")
     raise RuntimeError(f"b200gs {what} failed: {msg}")
 
@@ -213,6 +221,14 @@ def last_num_rendered() -> int:
     return _last_num_rendered
 
 
+_last_num_partials = 0
+
+
+def last_num_partials() -> int:
+    """Partial count H of the most recent deterministic backward call in this process (workload statistic)."""
+    return _last_num_partials
+
+
 class _StatePool:
     """Free lists of the opaque state buffers (geom | image | binning | backward scratch), keyed by (device, stream, sizes).
     A forward checks a set out, its autograd ctx holds it until the graph is freed, then the set returns here instead of
@@ -245,11 +261,16 @@ class _StatePool:
 
 
 _pool = _StatePool()
+# the deterministic backward's work buffer (plan + partials), checked out for the duration of one backward call
+_det_pool = _StatePool()
+# partial-capacity hint of the deterministic backward per (device, P, V, H, W): the largest partial count seen (+25 %)
+_partial_hint: dict = {}
 
 
 def release_cached_buffers():
     """Drop the parked state buffers (e.g. after densification changed P)."""
     _pool.clear()
+    _det_pool.clear()
 
 
 class _Ctx:
@@ -327,10 +348,45 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     return color, radii, depth, alpha, st
 
 
+def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None):
+    """b200gs_backward_deterministic with the work buffer from _det_pool, sized by the partial-capacity hint; a call whose
+    partials do not fit is repeated with room for the count it reported (at most two retries)."""
+    P, V, H, W = st.P, st.V, st.H, st.W
+    key = (dev.index, P, V, H, W)
+    pcap = _partial_hint.get(key, max(1 << 16, 2 * st.num_rendered))
+    n_out = C.c_int64(0)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    for _ in range(3):
+        # sized for the forward's instance capacity (>= its count), so the pool key stays the same from call to call
+        pkey = (dev.index, stream, st.capacity, pcap, P, V)
+        bufs = _det_pool.take(pkey)
+        if bufs is None:
+            bufs = dict(det=torch.empty(L.b200gs_deterministic_bytes(st.capacity, pcap, P, V), dtype=torch.uint8, device=dev))
+        det = bufs["det"]
+        rc = L.b200gs_backward_deterministic(*args, _ptr(det), det.numel(), pcap, C.byref(n_out), C.c_void_p(stream))
+        if rc == OK and det_state is not None:
+            det_state["patch_masks"] = det[:st.num_rendered].clone()
+            det_state["n_partials"] = int(n_out.value)
+        _det_pool.give(pkey, bufs)  # stream-ordered: the next call on this stream runs after this one's kernels
+        if rc != E_BIN_TOO_SMALL:
+            break
+        pcap = int(n_out.value * 1.25) + 1024
+    if rc == OK:
+        _partial_hint[key] = max(int(n_out.value * 1.25) + 1024, 1 << 16, _partial_hint.get(key, 0))
+        global _last_num_partials
+        _last_num_partials = int(n_out.value)
+    return rc
+
+
 def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
-                   projmatrix, campos, g_color, g_depth, g_alpha, out=None):
+                   projmatrix, campos, g_color, g_depth, g_alpha, out=None, det_state=None):
     """`out` (optional): dict of preallocated contiguous fp32 gradient buffers by name (means3D, sh, opacity, scales,
-    rotations) -- the packed entry points them into one flat buffer so that B3 writes the all-reduce payload in place."""
+    rotations) -- the packed entry points them into one flat buffer so that B3 writes the all-reduce payload in place.
+
+    Under torch.use_deterministic_algorithms(True) the backward is the library's deterministic one: the same gradients up
+    to float rounding, bit-identical from run to run (one host wait per call, for its partial count).  `det_state`
+    (optional dict) then receives the per-instance patch masks ("patch_masks", uint8 [num_rendered]) and the partial count
+    ("n_partials")."""
     L = load_library()
     dev = means3D.device
     P, V, M = st.P, st.V, st.M
@@ -347,13 +403,16 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
     if P == 0:
         return d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov
     scratch = st.scratch
+    args = (C.byref(st.prm), _ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities), _ptr(scales), _ptr(rotations),
+            _ptr(cov3D_precomp), _ptr(bg), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), _ptr(st.radii), _ptr(st.geom),
+            _ptr(st.binning), st.capacity, _ptr(st.image), st.num_rendered, _ptr(g_color), _ptr(g_depth), _ptr(g_alpha),
+            _ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh), _ptr(d_col), _ptr(d_op), _ptr(d_sc), _ptr(d_rot), _ptr(d_cov),
+            _ptr(scratch), scratch.numel())
     with torch.cuda.device(dev):
-        rc = L.b200gs_backward(C.byref(st.prm), _ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities), _ptr(scales),
-                               _ptr(rotations), _ptr(cov3D_precomp), _ptr(bg), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
-                               _ptr(st.radii), _ptr(st.geom), _ptr(st.binning), st.capacity, _ptr(st.image), st.num_rendered,
-                               _ptr(g_color), _ptr(g_depth), _ptr(g_alpha), _ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh),
-                               _ptr(d_col), _ptr(d_op), _ptr(d_sc), _ptr(d_rot), _ptr(d_cov), _ptr(scratch), scratch.numel(),
-                               _stream(dev))
+        if torch.are_deterministic_algorithms_enabled():
+            rc = _backward_deterministic(L, st, dev, args, det_state)
+        else:
+            rc = L.b200gs_backward(*args, _stream(dev))
     _check(rc, "backward")
     return d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov
 
@@ -641,15 +700,19 @@ def forward_backward_with_state(g_color, g_depth, g_alpha, **kw):
     """forward_with_state(**kw), then the backward of that same call for the image gradients g_color [V,3,H,W],
     g_depth [V,1,H,W], g_alpha [V,1,H,W].  Returns (color, radii, depth, alpha, state, sums): `sums` [V,P,12] float32 is
     the backward blend's ScreenGrad record of every (view, Gaussian) -- record v*P + g, in the format
-    blend_sgrad_is_moments() names (csrc/common.cuh) -- copied out before the state buffers can be re-used."""
+    blend_sgrad_is_moments() names (csrc/common.cuh) -- copied out before the state buffers can be re-used.  Under
+    torch.use_deterministic_algorithms(True) the deterministic backward runs, and `state` also holds its "patch_masks"
+    (uint8 per sorted instance, bit p = a partial for patch p of the instance's tile) and "n_partials"."""
     color, radii, depth, alpha, state, st = forward_with_state(**kw)
     dev = kw["means3D"].device
     V, P = st.V, st.P
     t = lambda k: _f32c(kw.get(k), dev)
     g = [_f32c(x, dev).reshape(V, c, st.H, st.W) for x, c in ((g_color, 3), (g_depth, 1), (g_alpha, 1))]
+    det_state = {}
     _backward_impl(st, t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"),
                    t("cov3D_precomp"), _f32c(kw["bg"], dev), t("viewmatrix").reshape(V, 4, 4), t("projmatrix").reshape(V, 4, 4),
-                   t("campos").reshape(V, 3), *g)
+                   t("campos").reshape(V, 3), *g, det_state=det_state)
+    state.update(det_state)
     nbytes = V * P * 48
     sums = st.scratch[:nbytes].view(torch.float32).reshape(V, P, 12).clone()
     return color, radii, depth, alpha, state, sums

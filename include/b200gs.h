@@ -19,7 +19,8 @@
  *     except b200gs_forward which reads the instance count back once per call (upstream blocks on it in the middle of
  *     every view's forward).  For batches of up to 4 M (view, Gaussian) pairs every kernel of the forward is enqueued
  *     FIRST (sized for instance_capacity, the count read on the device) and the host then waits on an event recorded
- *     right after the scan -- the GPU never idles behind the host; larger batches wait once in place;
+ *     right after the scan -- the GPU never idles behind the host; larger batches wait once in place.
+ *     b200gs_backward_deterministic also waits once, for its partial count;
  *   - return value 0 = success, negative = b200gs_status; nothing throws across the ABI; process state is limited to an
  *     error string, a launch counter, the optional stage profiler and one pinned count word + event per (thread, device);
  *   - matrices are the reference's row-vector-convention 4x4 tensors read as 16 contiguous floats
@@ -45,8 +46,9 @@ typedef enum b200gs_status {
     B200GS_E_BUFFER = -3,        /* a state buffer is smaller than b200gs_*_bytes() asks for */
     B200GS_E_CUDA = -4,          /* a CUDA call failed; see b200gs_last_cuda_error() */
     B200GS_E_RANGE = -5,         /* sizes outside supported range (sh_degree > 3, n_views > B200GS_MAX_VIEWS, P*V >= 2^32, > 65535 tiles per axis) */
-    B200GS_E_INSTANCES = -6      /* the batch has more than B200GS_MAX_INSTANCES (Gaussian, tile) instances; *num_rendered holds the exact
+    B200GS_E_INSTANCES = -6,     /* the batch has more than B200GS_MAX_INSTANCES (Gaussian, tile) instances; *num_rendered holds the exact
                                     64-bit count; nothing was emitted: render fewer views per call (the host mirror halves the batch) */
+    B200GS_E_UNSUPPORTED = -7    /* this build of the library does not implement the call (the classic comparator's deterministic backward) */
 } b200gs_status;
 #define B200GS_MAX_INSTANCES 0x7fffffffLL
 
@@ -127,6 +129,35 @@ int b200gs_backward(const b200gs_params *prm,
                     float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
                     float *dL_dscales, float *dL_drots, float *dL_dcov3D,
                     void *scratch, size_t scratch_bytes, void *stream);
+
+/*
+ * Deterministic backward: the same arguments, outputs and gradients as b200gs_backward, bit-reproducible from the forward
+ * state.  b200gs_backward adds each (tile, 8x4 patch) partial sum of the backward blend into its Gaussian's record with float
+ * atomics, in an order that depends on scheduling; this call stores every partial into its own slot of det_buf and then adds
+ * each (view, Gaussian)'s partials in a fixed order: its tiles in emission order (its screen rect row-major), within a tile its
+ * patches ascending, sequential fp32 adds.  Two calls on the same forward state write identical bytes.
+ *   det_buf: b200gs_deterministic_bytes(num_rendered, partial_capacity, P, n_views) bytes, 16-byte aligned.  Its first
+ *     num_rendered bytes hold, after the call, the patch mask of every sorted instance (bit p: the instance has a partial for
+ *     patch p of its tile).  num_rendered must be the matching forward's count.
+ *   partial_capacity: partials det_buf was sized for; *n_partials (host, int64[1]) receives the exact number H the call
+ *     needs.  If H > partial_capacity the call returns B200GS_E_BIN_TOO_SMALL before any gradient is written (grow, call
+ *     again; every access stayed inside the buffers); H >= 2^32 returns B200GS_E_RANGE.
+ * Unlike b200gs_backward this call waits on the host once: for H, read back after the plan pre-pass and before the blend.
+ * The classic comparator build returns B200GS_E_UNSUPPORTED.
+ */
+size_t b200gs_deterministic_bytes(int64_t num_rendered, int64_t partial_capacity, int32_t P, int32_t n_views);
+int b200gs_backward_deterministic(const b200gs_params *prm,
+                                  const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                                  const float *scales, const float *rotations, const float *cov3D_precomp,
+                                  const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                  const int32_t *radii,
+                                  const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                  const void *image_buf, int64_t num_rendered,
+                                  const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                  float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+                                  float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                  void *scratch, size_t scratch_bytes,
+                                  void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *stream);
 
 /* Frustum test only (upstream markVisible): present[i] = 1 if p_view.z > 0.2 for view 0.  positions [P,3]. */
 int b200gs_mark_visible(int32_t P, const float *positions, const float *viewmatrix, const float *projmatrix,
