@@ -1,6 +1,7 @@
 // api.cu -- the C-ABI of libb200gs (include/b200gs.h): argument validation, state-buffer carving,
 // kernel sequencing.  No torch types, no global state except an error string and a launch counter.
 #include <atomic>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 
@@ -99,14 +100,27 @@ static int check_common(const b200gs_params *p, const float *shs, const float *c
     return B200GS_OK;
 }
 
-int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
-                   const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
-                   const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                   float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf, size_t geom_bytes,
-                   void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf, size_t image_bytes,
-                   int64_t *num_rendered, void *stream)
+// b200gs_render_opts: NULL = the defaults; a struct too short to hold the fields this library reads is an argument error
+static int read_opts(const b200gs_render_opts *o, bool *aa)
 {
-    int rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
+    *aa = false;
+    if (!o) return B200GS_OK;
+    if (o->struct_bytes < (int32_t)(offsetof(b200gs_render_opts, antialiasing) + sizeof(o->antialiasing))) return B200GS_E_ARGS;
+    *aa = o->antialiasing != 0;
+    return B200GS_OK;
+}
+
+int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
+                        const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
+                        const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+                        const float *campos, float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf,
+                        size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf,
+                        size_t image_bytes, int64_t *num_rendered, void *stream)
+{
+    bool aa = false;
+    int rc = read_opts(opts, &aa);
+    if (rc) return rc;
+    rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
     if (!means3D || !opacities || !bg || !viewmatrix || !projmatrix || !campos || !out_color || !out_depth || !out_alpha ||
         !radii || !geom_buf || !binning_buf || !image_buf || !num_rendered)
@@ -141,7 +155,7 @@ int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *
         a.radii = radii; a.recs = (GeomRec *)(gb + GL.recs); a.tiles_touched = (uint32_t *)(gb + GL.tiles_touched);
         a.rects = (uint2 *)(gb + GL.rects); a.clamped = (uint8_t *)(gb + GL.clamped);
         a.dkeys = (uint32_t *)(bb + BL.dkeys_in); a.order_in = (uint32_t *)(bb + BL.order_in);
-        { StageTimer t(B200GS_STAGE_PREPROCESS, st); launch_preprocess_fwd(a, V, st); }
+        { StageTimer t(B200GS_STAGE_PREPROCESS, st); launch_preprocess_fwd(a, V, aa, st); }
         g_launches += 1;
         uint32_t *offsets = (uint32_t *)(gb + GL.offsets); // inclusive scan of tiles_touched in DEPTH order
         const int64_t n_vp = (int64_t)P * V;
@@ -211,13 +225,25 @@ int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *
     return B200GS_OK;
 }
 
+int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
+                   const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
+                   const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                   float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf, size_t geom_bytes,
+                   void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf, size_t image_bytes,
+                   int64_t *num_rendered, void *stream)
+{
+    return b200gs_forward_opts(prm, nullptr, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
+                               projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf,
+                               binning_bytes, instance_capacity, image_buf, image_bytes, num_rendered, stream);
+}
+
 size_t b200gs_deterministic_bytes(int64_t num_rendered, int64_t partial_capacity, int32_t P, int32_t V)
 {
     return DetLayout(num_rendered, partial_capacity, (int64_t)(P > 0 ? P : 0) * (V > 0 ? V : 0)).total;
 }
 
 // b200gs_backward (det == false) and b200gs_backward_deterministic (det == true)
-static int backward_impl(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
+static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs, const float *colors_precomp,
                          const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
                          const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
                          const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
@@ -227,6 +253,8 @@ static int backward_impl(const b200gs_params *prm, const float *means3D, const f
                          size_t scratch_bytes, void *stream, bool det, void *det_buf, size_t det_bytes, int64_t partial_capacity,
                          int64_t *n_partials)
 {
+    bool aa = false;
+    if (read_opts(opts, &aa)) return B200GS_E_ARGS;
     if (det) {
         if (!blend_bwd_has_deterministic()) return B200GS_E_UNSUPPORTED;
         if (!n_partials || !det_buf || partial_capacity < 0) return B200GS_E_ARGS;
@@ -236,7 +264,7 @@ static int backward_impl(const b200gs_params *prm, const float *means3D, const f
     }
     int rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
-    if (prm->raw_params && !opacities) return B200GS_E_ARGS;
+    if ((prm->raw_params || aa) && !opacities) return B200GS_E_ARGS;
     if (!means3D || !bg || !viewmatrix || !projmatrix || !campos || !radii || !geom_buf || !binning_buf || !image_buf ||
         !dL_dmeans3D || !dL_dmeans2D || !dL_dopacity || !scratch)
         return B200GS_E_ARGS;
@@ -316,10 +344,25 @@ static int backward_impl(const b200gs_params *prm, const float *means3D, const f
     a.recs = (const GeomRec *)(gb + GL.recs); a.moments = blend_sgrad_is_moments();
     a.dL_dmeans3D = dL_dmeans3D; a.dL_dmeans2D = dL_dmeans2D; a.dL_dsh = dL_dsh; a.dL_dcolors = dL_dcolors;
     a.dL_dopacity = dL_dopacity; a.dL_dscales = dL_dscales; a.dL_drots = dL_drots; a.dL_dcov3D = dL_dcov3D;
-    { StageTimer t(B200GS_STAGE_PREPROCESS_BWD, st); launch_preprocess_bwd(a, st); }
+    { StageTimer t(B200GS_STAGE_PREPROCESS_BWD, st); launch_preprocess_bwd(a, aa, st); }
     g_launches += det ? 1 : 2; // (the deterministic blend stage counted its own launches)
     CK(cudaGetLastError(), "backward launch");
     return B200GS_OK;
+}
+
+int b200gs_backward_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
+                         const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
+                         const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+                         const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf,
+                         int64_t instance_capacity, const void *image_buf, int64_t num_rendered, const float *dL_dcolor,
+                         const float *dL_ddepth, const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
+                         float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
+                         size_t scratch_bytes, void *stream)
+{
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr);
 }
 
 int b200gs_backward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
@@ -331,10 +374,26 @@ int b200gs_backward(const b200gs_params *prm, const float *means3D, const float 
                     float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
                     size_t scratch_bytes, void *stream)
 {
-    return backward_impl(prm, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+    return backward_impl(prm, nullptr, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                          campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
                          scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr);
+}
+
+int b200gs_backward_deterministic_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D,
+                                       const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
+                                       const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix,
+                                       const float *projmatrix, const float *campos, const int32_t *radii, const void *geom_buf,
+                                       const void *binning_buf, int64_t instance_capacity, const void *image_buf,
+                                       int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                       float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+                                       float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch, size_t scratch_bytes,
+                                       void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *stream)
+{
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials);
 }
 
 int b200gs_backward_deterministic(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
@@ -347,7 +406,7 @@ int b200gs_backward_deterministic(const b200gs_params *prm, const float *means3D
                                   size_t scratch_bytes, void *det_buf, size_t det_bytes, int64_t partial_capacity,
                                   int64_t *n_partials, void *stream)
 {
-    return backward_impl(prm, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+    return backward_impl(prm, nullptr, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                          campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
                          scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials);

@@ -65,8 +65,9 @@ struct BlendBwdArgs {
     void *sgrad;                                    // [V*P] accumulators (format: blend_sgrad_is_moments()), zeroed by the caller
 };
 
-void launch_preprocess_fwd(const PreArgs &a, int V, cudaStream_t st);
-void launch_preprocess_bwd(const PreBwdArgs &a, cudaStream_t st);
+// aa: the antialiasing filter (record opacity op * rho; DESIGN.md section 2)
+void launch_preprocess_fwd(const PreArgs &a, int V, bool aa, cudaStream_t st);
+void launch_preprocess_bwd(const PreBwdArgs &a, bool aa, cudaStream_t st);
 void launch_mark_visible(int P, const float *pos, const float *V, uint8_t *present, cudaStream_t st);
 
 // binning: depth pre-sort of the V*P Gaussians, scan in depth order, tile-key emission, stable tile sort, ranges

@@ -91,11 +91,13 @@ __device__ __forceinline__ float gs_normalize4(float *q)
 // row pitch allows), builds the 3D covariance once, then loops over the V views of the batch writing one
 // 48-byte record per view.  Per step this reads P*(44+12K) bytes instead of V times that.
 // DEG = -1: colours are given (colors_precomp), no SH.
+// AA: the antialiasing filter (DESIGN.md section 2): the record's opacity is op * rho, rho = sqrt(det0 / det), det0 the
+// determinant of the 2D covariance before the +0.3 px^2 dilation; the support box is bounded with that opacity too.
 // ------------------------------------------------------------------------------------------------
 #ifndef PFWD_MIN_BLOCKS
 #define PFWD_MIN_BLOCKS 3 // 80 registers; H100 (400 W): 2 / 4 blocks make this kernel 33 % / 26 % slower
 #endif
-template <int DEG>
+template <int DEG, bool AA>
 __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(PreArgs a, int nviews)
 {
     constexpr int NB = DEG < 0 ? 1 : (DEG + 1) * (DEG + 1);
@@ -196,9 +198,11 @@ __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(Pr
                 N0[k] = gs_dot3(M0[0], M0[1], M0[2], S[0][k], S[1][k], S[2][k]);
                 N1[k] = gs_dot3(M1[0], M1[1], M1[2], S[0][k], S[1][k], S[2][k]);
             }
-            const float ca = fadd(gs_dot3(N0[0], N0[1], N0[2], M0[0], M0[1], M0[2]), GS_DILATE);
+            const float ca0 = gs_dot3(N0[0], N0[1], N0[2], M0[0], M0[1], M0[2]);
+            const float ca = fadd(ca0, GS_DILATE);
             const float cb = gs_dot3(N0[0], N0[1], N0[2], M1[0], M1[1], M1[2]);
-            const float cc = fadd(gs_dot3(N1[0], N1[1], N1[2], M1[0], M1[1], M1[2]), GS_DILATE);
+            const float cc0 = gs_dot3(N1[0], N1[1], N1[2], M1[0], M1[1], M1[2]);
+            const float cc = fadd(cc0, GS_DILATE);
             const float det = ffma(ca, cc, -fmul(cb, cb));
             if (det == 0.0f) break;
             const float det_inv = fdiv(1.0f, det);
@@ -241,17 +245,23 @@ __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(Pr
             } else {
                 rgb[0] = shc[0]; rgb[1] = shc[1]; rgb[2] = shc[2];
             }
+            float oe = op; // the record's opacity
+            if (AA) {
+                // floor rho >= 0.005: a degenerate footprint (det0 <= 0) lands on it
+                const float det0 = ffma(ca0, cc0, -fmul(cb, cb));
+                oe = fmul(op, fsqrt(fmaxf(2.5e-5f, fdiv(det0, det))));
+            }
             radius = rad;
             tiles = (uint32_t)area;
             rect_pack = make_uint2((uint32_t)x0 | ((uint32_t)y0 << 16), (uint32_t)x1 | ((uint32_t)y1 << 16));
             rec.px = pxs; rec.py = pys;
-            rec.A = conA; rec.B = conB; rec.C = conC; rec.o = op;
+            rec.A = conA; rec.B = conB; rec.C = conC; rec.o = oe;
             rec.r = rgb[0]; rec.g = rgb[1]; rec.b = rgb[2]; rec.depth = tz;
             // Conservative half extents of {alpha >= 1/255}: power >= -tau, tau = ln(255*o).  Product-only
             // acceleration data (never changes a result: a pixel outside [px+-hx] x [py+-hy] has
             // alpha < 1/255 with margin far above the float error of gs_power/gs_exp; see DESIGN.md).
             {
-                const float k255 = 255.0f * op;
+                const float k255 = 255.0f * oe;
                 const float aniso = (ca * cc) * det_inv; // 1/(1-rho^2): amplifies rounding error of power
                 if (!(k255 > 1.0f)) {
                     rec.hx = rec.hy = -1.0f; // can never reach 1/255
@@ -278,14 +288,20 @@ __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(Pr
     }
 }
 
-void launch_preprocess_fwd(const PreArgs &a, int V, cudaStream_t st)
+template <bool AA>
+static void launch_preprocess_fwd_t(const PreArgs &a, int V, cudaStream_t st)
 {
     const dim3 grid((a.P + 255) / 256);
-    if (!a.shs) preprocess_fwd_kernel<-1><<<grid, 256, 0, st>>>(a, V);
-    else if (a.deg == 0) preprocess_fwd_kernel<0><<<grid, 256, 0, st>>>(a, V);
-    else if (a.deg == 1) preprocess_fwd_kernel<1><<<grid, 256, 0, st>>>(a, V);
-    else if (a.deg == 2) preprocess_fwd_kernel<2><<<grid, 256, 0, st>>>(a, V);
-    else preprocess_fwd_kernel<3><<<grid, 256, 0, st>>>(a, V);
+    if (!a.shs) preprocess_fwd_kernel<-1, AA><<<grid, 256, 0, st>>>(a, V);
+    else if (a.deg == 0) preprocess_fwd_kernel<0, AA><<<grid, 256, 0, st>>>(a, V);
+    else if (a.deg == 1) preprocess_fwd_kernel<1, AA><<<grid, 256, 0, st>>>(a, V);
+    else if (a.deg == 2) preprocess_fwd_kernel<2, AA><<<grid, 256, 0, st>>>(a, V);
+    else preprocess_fwd_kernel<3, AA><<<grid, 256, 0, st>>>(a, V);
+}
+void launch_preprocess_fwd(const PreArgs &a, int V, bool aa, cudaStream_t st)
+{
+    if (aa) launch_preprocess_fwd_t<true>(a, V, st);
+    else launch_preprocess_fwd_t<false>(a, V, st);
 }
 
 __global__ void mark_visible_kernel(int P, const float *pos, const float *V, uint8_t *present)
@@ -303,11 +319,12 @@ void launch_mark_visible(int P, const float *pos, const float *V, uint8_t *prese
 // ------------------------------------------------------------------------------------------------
 // B2 + B3: one thread per Gaussian, loops over the views of the batch and SUMS parameter gradients
 // (deterministic: no atomics at the parameter level).  Plain float arithmetic (tolerance-compared).
+// AA: the forward's record opacity was op * rho (F1): dL/dop = rho * S0, and dL/drho = op * S0 joins the cov2D gradient.
 // ------------------------------------------------------------------------------------------------
 #ifndef PBWD_MIN_BLOCKS
 #define PBWD_MIN_BLOCKS 4 // 128 registers; 5 / 6 blocks (96 / 80 registers) spill the 48 SH accumulators
 #endif
-template <int DEG>
+template <int DEG, bool AA>
 __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(PreBwdArgs a)
 {
     constexpr int nb = DEG < 0 ? 1 : (DEG + 1) * (DEG + 1);
@@ -400,7 +417,7 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
         const float gcol[3] = {g1.z, g1.w, g2.x};
         const float gdepth = g2.y;
         m2d[0] = gdx; m2d[1] = gdy; m2d[2] = 0.f;
-        dop += gO;
+        if (!AA) dop += gO;
 
         const float *V = a.view + 16 * v, *PV = a.proj + 16 * v;
         const float tx = gs_affine(V[0], V[4], V[8], V[12], px, py, pz);
@@ -429,16 +446,38 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
             N0[k] = M0[0] * S[0][k] + M0[1] * S[1][k] + M0[2] * S[2][k];
             N1[k] = M1[0] * S[0][k] + M1[1] * S[1][k] + M1[2] * S[2][k];
         }
-        const float ca = N0[0] * M0[0] + N0[1] * M0[1] + N0[2] * M0[2] + GS_DILATE;
+        const float ca0 = N0[0] * M0[0] + N0[1] * M0[1] + N0[2] * M0[2];
+        const float ca = ca0 + GS_DILATE;
         const float cb = N0[0] * M1[0] + N0[1] * M1[1] + N0[2] * M1[2];
-        const float cc = N1[0] * M1[0] + N1[1] * M1[1] + N1[2] * M1[2] + GS_DILATE;
+        const float cc0 = N1[0] * M1[0] + N1[1] * M1[1] + N1[2] * M1[2];
+        const float cc = cc0 + GS_DILATE;
         const float denom = ca * cc - cb * cb;
         const float d2inv = 1.0f / (denom * denom + 0.0000001f);
+        float ra = 0.f, rb = 0.f, rc = 0.f; // AA: dL/drho * drho/d(a, b, c)
+        if (AA) {
+            // rho = sqrt(det0 / det), det = det0 + d (ca0 + cc0 + d), d = 0.3: the derivatives in a cancellation-free form
+            //   drho/da = d (cc0 cc + b^2) / (2 rho det^2),  drho/dc = d (ca0 ca + b^2) / (2 rho det^2),
+            //   drho/db = -d b (ca + cc0) / (rho det^2);  zero where the floor holds
+            const float ratio = (ca0 * cc0 - cb * cb) / denom;
+            const float rho = sqrtf(fmaxf(2.5e-5f, ratio));
+            dop += rho * gO;
+            if (ratio > 2.5e-5f) {
+                // the opacity before the filter (after the sigmoid for raw parameters), re-read per view (an L1 hit) rather
+                // than kept live across the view loop
+                const float opr = __ldg(a.opac + i);
+                const float op = a.raw ? gs_sigmoid(opr) : opr;
+                const float k = GS_DILATE * op * gO / (rho * denom * denom);
+                ra = 0.5f * k * (cc0 * cc + cb * cb);
+                rc = 0.5f * k * (ca0 * ca + cb * cb);
+                rb = -k * cb * (ca + cc0);
+            }
+        }
         if (d2inv != 0.f) {
             // (denom - a*c) == -b*b and (denom + 2*b*b) == a*c + b*b, written without the cancellation
-            const float da = d2inv * (-cc * cc * dA + 2.f * cb * cc * dBh - cb * cb * dC);
-            const float dc = d2inv * (-ca * ca * dC + 2.f * ca * cb * dBh - cb * cb * dA);
-            const float db = d2inv * 2.f * (cb * cc * dA - (ca * cc + cb * cb) * dBh + ca * cb * dC);
+            float da = d2inv * (-cc * cc * dA + 2.f * cb * cc * dBh - cb * cb * dC);
+            float dc = d2inv * (-ca * ca * dC + 2.f * ca * cb * dBh - cb * cb * dA);
+            float db = d2inv * 2.f * (cb * cc * dA - (ca * cc + cb * cb) * dBh + ca * cb * dC);
+            if (AA) { da += ra; db += rb; dc += rc; }
             dcov[0] += M0[0] * M0[0] * da + M0[0] * M1[0] * db + M1[0] * M1[0] * dc;
             dcov[3] += M0[1] * M0[1] * da + M0[1] * M1[1] * db + M1[1] * M1[1] * dc;
             dcov[5] += M0[2] * M0[2] * da + M0[2] * M1[2] * db + M1[2] * M1[2] * dc;
@@ -591,12 +630,18 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
     }
 }
 
-void launch_preprocess_bwd(const PreBwdArgs &a, cudaStream_t st)
+template <bool AA>
+static void launch_preprocess_bwd_t(const PreBwdArgs &a, cudaStream_t st)
 {
     const int grid = (a.P + 127) / 128;
-    if (!a.shs) preprocess_bwd_kernel<-1><<<grid, 128, 0, st>>>(a);
-    else if (a.deg == 0) preprocess_bwd_kernel<0><<<grid, 128, 0, st>>>(a);
-    else if (a.deg == 1) preprocess_bwd_kernel<1><<<grid, 128, 0, st>>>(a);
-    else if (a.deg == 2) preprocess_bwd_kernel<2><<<grid, 128, 0, st>>>(a);
-    else preprocess_bwd_kernel<3><<<grid, 128, 0, st>>>(a);
+    if (!a.shs) preprocess_bwd_kernel<-1, AA><<<grid, 128, 0, st>>>(a);
+    else if (a.deg == 0) preprocess_bwd_kernel<0, AA><<<grid, 128, 0, st>>>(a);
+    else if (a.deg == 1) preprocess_bwd_kernel<1, AA><<<grid, 128, 0, st>>>(a);
+    else if (a.deg == 2) preprocess_bwd_kernel<2, AA><<<grid, 128, 0, st>>>(a);
+    else preprocess_bwd_kernel<3, AA><<<grid, 128, 0, st>>>(a);
+}
+void launch_preprocess_bwd(const PreBwdArgs &a, bool aa, cudaStream_t st)
+{
+    if (aa) launch_preprocess_bwd_t<true>(a, st);
+    else launch_preprocess_bwd_t<false>(a, st);
 }

@@ -53,6 +53,15 @@ class _Params(C.Structure):
                 ("raw_params", C.c_int32)]
 
 
+class _RenderOpts(C.Structure):
+    """b200gs_render_opts (include/b200gs.h): options of the *_opts entry points"""
+    _fields_ = [("struct_bytes", C.c_int32), ("antialiasing", C.c_int32)]
+
+
+def _render_opts(antialiasing: bool):
+    return _RenderOpts(C.sizeof(_RenderOpts), int(bool(antialiasing)))
+
+
 class _StateView(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("geom_records", "tiles_touched", "offsets", "clamped", "sorted_tile_keys",
                                           "depth_order", "point_list", "ranges", "final_T", "n_contrib",
@@ -66,7 +75,8 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_test_sort_pairs", "b200gs_test_sort_scratch_bytes", "b200gs_reattach", "b200gs_pack_frames_u8",
            "b200gs_knn_scratch_bytes", "b200gs_dist2_knn3", "b200gs_densify_stats", "b200gs_densify_scratch_bytes",
            "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed", "b200gs_deterministic_bytes",
-           "b200gs_backward_deterministic"]
+           "b200gs_backward_deterministic", "b200gs_forward_opts", "b200gs_backward_opts",
+           "b200gs_backward_deterministic_opts"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -95,6 +105,14 @@ def load_library():
     L.b200gs_backward_deterministic.restype = C.c_int
     L.b200gs_backward_deterministic.argtypes = ([C.POINTER(_Params)] + [vp] * 12 + [vp, vp, i64, vp, i64] + [vp] * 11 + [vp, sz] +
                                                 [vp, sz, i64, C.POINTER(i64), vp])
+    # the *_opts forms: the same argument lists with the options pointer after prm
+    L.b200gs_forward_opts.restype = C.c_int
+    L.b200gs_forward_opts.argtypes = [L.b200gs_forward.argtypes[0], vp] + L.b200gs_forward.argtypes[1:]
+    L.b200gs_backward_opts.restype = C.c_int
+    L.b200gs_backward_opts.argtypes = [L.b200gs_backward.argtypes[0], vp] + L.b200gs_backward.argtypes[1:]
+    L.b200gs_backward_deterministic_opts.restype = C.c_int
+    L.b200gs_backward_deterministic_opts.argtypes = ([L.b200gs_backward_deterministic.argtypes[0], vp] +
+                                                     L.b200gs_backward_deterministic.argtypes[1:])
     L.b200gs_mark_visible.restype = C.c_int
     L.b200gs_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
     L.b200gs_describe_state.restype = C.c_int
@@ -276,7 +294,7 @@ def release_cached_buffers():
 class _Ctx:
     """What one forward keeps for its backward (upstream keeps geomBuffer/binningBuffer/imgBuffer the same way)."""
     __slots__ = ("prm", "tanx", "tany", "geom", "binning", "image", "scratch", "capacity", "num_rendered", "radii", "V", "P", "H",
-                 "W", "M", "__weakref__")
+                 "W", "M", "opts", "__weakref__")
 
 
 def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=False, per_view_means=False, raw=False):
@@ -288,9 +306,11 @@ def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=F
 
 
 def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                  campos, tanfovx, tanfovy, H, W, sh_degree, scale_modifier, prefiltered=False, debug=False, raw=False):
+                  campos, tanfovx, tanfovy, H, W, sh_degree, scale_modifier, prefiltered=False, debug=False, raw=False,
+                  antialiasing=False):
     """All tensors float32 contiguous on one CUDA device.  viewmatrix/projmatrix [V,4,4], campos [V,3].
-    raw: opacities / scales / rotations are GaussianModel's raw parameters (activations fused into the kernels)."""
+    raw: opacities / scales / rotations are GaussianModel's raw parameters (activations fused into the kernels).
+    antialiasing: the screen-space mip filter (b200gs_render_opts); the state remembers it for the backward."""
     L = load_library()
     dev = means3D.device
     if dev.type != "cuda":
@@ -316,6 +336,9 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     cap = _cap_hint.get(key, max(1 << 16, 4 * P * V))
     n_out = C.c_int64(0)
     stream = torch.cuda.current_stream(dev).cuda_stream
+    opts = _render_opts(True) if antialiasing else None
+    # with the defaults the plain entry point runs (b200gs_forward == b200gs_forward_opts with NULL options)
+    fwd = (lambda *a: L.b200gs_forward_opts(a[0], C.byref(opts), *a[1:])) if opts is not None else L.b200gs_forward
     with torch.cuda.device(dev):
         for _ in range(3):
             pkey = (key, stream, cap)
@@ -325,7 +348,7 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
                             binning=torch.empty(L.b200gs_binning_bytes(cap, H, W, P, V), **u8),
                             scratch=torch.empty(max(L.b200gs_backward_scratch_bytes(P, V), 16), **u8))
             geom, image, binning = bufs["geom"], bufs["image"], bufs["binning"]
-            rc = L.b200gs_forward(C.byref(prm), _ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities), _ptr(scales),
+            rc = fwd(C.byref(prm), _ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities), _ptr(scales),
                                   _ptr(rotations), _ptr(cov3D_precomp), _ptr(bg), _ptr(viewmatrix), _ptr(projmatrix),
                                   _ptr(campos), _ptr(color), _ptr(depth), _ptr(alpha), _ptr(radii), _ptr(geom), geom.numel(),
                                   _ptr(binning), binning.numel(), cap, _ptr(image), image.numel(), C.byref(n_out), C.c_void_p(stream))
@@ -344,6 +367,7 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     st.prm, st.tanx, st.tany = prm, tx, ty
     st.geom, st.binning, st.image, st.scratch, st.capacity, st.num_rendered = geom, binning, image, bufs["scratch"], cap, int(n_out.value)
     st.radii, st.V, st.P, st.H, st.W, st.M = radii, V, P, H, W, M
+    st.opts = opts
     weakref.finalize(st, _pool.give, pkey, bufs)  # when the autograd graph drops the state, the buffers are parked for re-use
     return color, radii, depth, alpha, st
 
@@ -363,7 +387,11 @@ def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None):
         if bufs is None:
             bufs = dict(det=torch.empty(L.b200gs_deterministic_bytes(st.capacity, pcap, P, V), dtype=torch.uint8, device=dev))
         det = bufs["det"]
-        rc = L.b200gs_backward_deterministic(*args, _ptr(det), det.numel(), pcap, C.byref(n_out), C.c_void_p(stream))
+        if st.opts is not None:
+            rc = L.b200gs_backward_deterministic_opts(args[0], C.byref(st.opts), *args[1:], _ptr(det), det.numel(), pcap,
+                                                      C.byref(n_out), C.c_void_p(stream))
+        else:
+            rc = L.b200gs_backward_deterministic(*args, _ptr(det), det.numel(), pcap, C.byref(n_out), C.c_void_p(stream))
         if rc == OK and det_state is not None:
             det_state["patch_masks"] = det[:st.num_rendered].clone()
             det_state["n_partials"] = int(n_out.value)
@@ -411,6 +439,8 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
     with torch.cuda.device(dev):
         if torch.are_deterministic_algorithms_enabled():
             rc = _backward_deterministic(L, st, dev, args, det_state)
+        elif st.opts is not None:  # the backward gets the options its forward got
+            rc = L.b200gs_backward_opts(args[0], C.byref(st.opts), *args[1:], _stream(dev))
         else:
             rc = L.b200gs_backward(*args, _stream(dev))
     _check(rc, "backward")
@@ -436,10 +466,11 @@ class _RasterizeViews(torch.autograd.Function):
     def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, squeeze):
         bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, prefiltered, debug = cams[:12]
         raw = bool(cams[12]) if len(cams) > 12 else False
+        aa = bool(cams[13]) if len(cams) > 13 else False
         dev = means3D.device
         args = [_f32c(t, dev) for t in (means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)]
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
-        color, radii, depth, alpha, st = _forward_impl(*args, *camt, tanx, tany, H, W, deg, mod, prefiltered, debug, raw)
+        color, radii, depth, alpha, st = _forward_impl(*args, *camt, tanx, tany, H, W, deg, mod, prefiltered, debug, raw, aa)
         ctx.st, ctx.squeeze = st, squeeze
         _save(ctx, args + camt)
         ctx.in_shapes = [None if t is None else t.shape for t in (means3D, means2D, shs, colors_precomp, opacities, scales,
@@ -480,20 +511,26 @@ class GaussianRasterizationSettings(NamedTuple):
     debug: bool
 
 
-def _cams_from_settings(s: GaussianRasterizationSettings):
+def _cams_from_settings(s: GaussianRasterizationSettings, antialiasing=False):
     return (s.bg, s.viewmatrix.reshape(1, 4, 4), s.projmatrix.reshape(1, 4, 4), s.campos.reshape(1, 3), [s.tanfovx], [s.tanfovy],
-            int(s.image_height), int(s.image_width), int(s.sh_degree), float(s.scale_modifier), s.prefiltered, s.debug)
+            int(s.image_height), int(s.image_width), int(s.sh_degree), float(s.scale_modifier), s.prefiltered, s.debug, False,
+            bool(antialiasing))
 
 
-def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+                        antialiasing=False):
     return _RasterizeViews.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                 _cams_from_settings(raster_settings), True)
+                                 _cams_from_settings(raster_settings, antialiasing), True)
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings):
+    """antialiasing: the screen-space mip filter (DESIGN.md section 2).  None takes `raster_settings.antialiasing` when the
+    settings tuple has that field (upstream's 13-field settings do), else off."""
+
+    def __init__(self, raster_settings, antialiasing=None):
         super().__init__()
         self.raster_settings = raster_settings
+        self.antialiasing = bool(getattr(raster_settings, "antialiasing", False) if antialiasing is None else antialiasing)
 
     def markVisible(self, positions):
         L = load_library()
@@ -514,13 +551,16 @@ class GaussianRasterizer(nn.Module):
                 ((scales is not None or rotations is not None) and cov3D_precomp is not None):
             raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   self.raster_settings)
+                                   self.raster_settings, self.antialiasing)
 
 
 def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, tanfovx, tanfovy, image_height, image_width,
                     bg, sh_degree=0, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
-                    means2D=None, scale_modifier=1.0, raw=False):
+                    means2D=None, scale_modifier=1.0, raw=False, antialiasing=False):
     """Render V cameras of one Gaussian set in ONE call (one preprocess/sort/blend launch set, one host sync).
+
+    antialiasing=True: the screen-space mip filter -- each Gaussian's opacity is scaled by sqrt(det(S) / det(S + 0.3 I)) of
+    its projected covariance S, so its footprint keeps its integrated weight at any pixel scale (DESIGN.md section 2).
 
     raw=True: `opacities`, `scales`, `rotations` are GaussianModel's RAW parameters (`_opacity`, `_scaling`, `_rotation`,
     gaussian_model.py:44-59); sigmoid / exp / F.normalize run inside the preprocess kernel and their Jacobians inside the
@@ -538,13 +578,14 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                                 tanfovx=tanfovx[i:i + MAX_VIEWS], tanfovy=tanfovy[i:i + MAX_VIEWS], image_height=image_height,
                                 image_width=image_width, bg=bg, sh_degree=sh_degree, shs=shs, colors_precomp=colors_precomp,
                                 scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
-                                means2D=None if means2D is None else means2D[i:i + MAX_VIEWS], scale_modifier=scale_modifier, raw=raw)
+                                means2D=None if means2D is None else means2D[i:i + MAX_VIEWS], scale_modifier=scale_modifier, raw=raw,
+                                antialiasing=antialiasing)
                 for i in range(0, V, MAX_VIEWS)]
         return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
     if means2D is None:
         means2D = torch.zeros(V, means3D.shape[-2], 3, dtype=torch.float32, device=means3D.device)
     cams = (bg, viewmatrices, projmatrices, camposs, list(tanfovx), list(tanfovy), int(image_height), int(image_width),
-            int(sh_degree), float(scale_modifier), False, False, bool(raw))
+            int(sh_degree), float(scale_modifier), False, False, bool(raw), bool(antialiasing))
     try:
         return _RasterizeViews.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, False)
     except InstanceLimitError:
@@ -556,7 +597,8 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                             projmatrices=projmatrices[sl], camposs=camposs[sl], tanfovx=list(tanfovx)[sl], tanfovy=list(tanfovy)[sl],
                             image_height=image_height, image_width=image_width, bg=bg, sh_degree=sh_degree, shs=shs,
                             colors_precomp=colors_precomp, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
-                            means2D=means2D[sl], scale_modifier=scale_modifier, raw=raw) for sl in (slice(0, h), slice(h, V))]
+                            means2D=means2D[sl], scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing)
+            for sl in (slice(0, h), slice(h, V))]
     return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
 
 
@@ -587,11 +629,12 @@ def _split_packed(flat: torch.Tensor, P: int, M: int):
 class _RasterizePacked(torch.autograd.Function):
     @staticmethod
     def forward(ctx, packed, means2D, P, M, cams):
-        bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, raw = cams
+        bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, raw, aa = cams
         dev = packed.device
         xyz, sc, rot, op, sh = _split_packed(packed.detach(), P, M)
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
-        color, radii, depth, alpha, st = _forward_impl(xyz, sh, None, op, sc, rot, None, *camt, tanx, tany, H, W, deg, mod, raw=raw)
+        color, radii, depth, alpha, st = _forward_impl(xyz, sh, None, op, sc, rot, None, *camt, tanx, tany, H, W, deg, mod, raw=raw,
+                                                       antialiasing=aa)
         ctx.st, ctx.P, ctx.M = st, P, M
         ctx.save_for_backward(packed, *camt)
         ctx.mark_non_differentiable(radii)
@@ -612,14 +655,14 @@ class _RasterizePacked(torch.autograd.Function):
 
 
 def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, viewmatrices, projmatrices, camposs, tanfovx, tanfovy,
-                           image_height, image_width, bg, sh_degree=0, means2D=None, scale_modifier=1.0, raw=False):
+                           image_height, image_width, bg, sh_degree=0, means2D=None, scale_modifier=1.0, raw=False, antialiasing=False):
     """`rasterize_views` over ONE flat fp32 buffer [xyz 3P | scales 3P | rotations 4P | opacities P | shs 3*K*P], each
     field starting on a 16-byte boundary (`packed_layout`; what `dist.pack` produces, broadcast once per parameter
     version).  raw=False: post-activation values, as the rasteriser's classic inputs.  raw=True: the buffer holds the
     optimiser's RAW parameters (log-scales, un-normalised quaternions, opacity logits; SH = cat(f_dc, f_rest)); the
     activations of gaussian_model.py:95-118 and their Jacobians run inside the kernels, so `packed.grad` is the gradient
     of the raw parameters and a training step needs no activation kernels, no pack copy and no autograd nodes besides
-    this one.  The backward
+    this one.  antialiasing: as `rasterize_views`.  The backward
     kernels write the parameter gradients straight into one buffer of the same layout, which becomes `packed.grad`
     as is: no per-tensor gradient accumulation, and on several GPUs that buffer is the all-reduce payload in place.
     V <= MAX_VIEWS.  Returns color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W]."""
@@ -633,7 +676,7 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
     if means2D is None:
         means2D = torch.zeros(V, P, 3, dtype=torch.float32, device=packed.device)
     cams = (bg, viewmatrices, projmatrices, camposs, list(tanfovx), list(tanfovy), int(image_height), int(image_width),
-            int(sh_degree), float(scale_modifier), bool(raw))
+            int(sh_degree), float(scale_modifier), bool(raw), bool(antialiasing))
     try:
         return _RasterizePacked.apply(packed, means2D, int(P), int(sh_coeffs), cams)
     except InstanceLimitError:
@@ -643,7 +686,7 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
     outs = [rasterize_views_packed(packed, P, sh_coeffs, viewmatrices=viewmatrices[sl], projmatrices=projmatrices[sl], camposs=camposs[sl],
                                    tanfovx=list(tanfovx)[sl], tanfovy=list(tanfovy)[sl], image_height=image_height,
                                    image_width=image_width, bg=bg, sh_degree=sh_degree, means2D=means2D[sl],
-                                   scale_modifier=scale_modifier, raw=raw) for sl in (slice(0, h), slice(h, V))]
+                                   scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing) for sl in (slice(0, h), slice(h, V))]
     return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
 
 
@@ -662,7 +705,7 @@ def forward_with_state(**kw):
         t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"), t("cov3D_precomp"),
         _f32c(kw["bg"], dev), _f32c(vm, dev).reshape(V, 4, 4), _f32c(pm, dev).reshape(V, 4, 4), _f32c(cp, dev).reshape(V, 3),
         tanx, tany, int(kw["image_height"]), int(kw["image_width"]), int(kw.get("sh_degree", 0)),
-        float(kw.get("scale_modifier", 1.0)))
+        float(kw.get("scale_modifier", 1.0)), antialiasing=bool(kw.get("antialiasing", False)))
     sv = _StateView()
     _check(L.b200gs_describe_state(C.byref(st.prm), _ptr(st.geom), _ptr(st.binning), st.capacity, _ptr(st.image), C.byref(sv)),
            "describe_state")

@@ -23,6 +23,7 @@ class PipelineParams:
     convert_SHs_python = False
     compute_cov3D_python = False
     debug = False
+    antialiasing = False  # the screen-space mip filter (rasterizer.rasterize_views); the name upstream 3DGS gives it
 
 
 def _raw_tensors(pc):
@@ -39,7 +40,8 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
     """fused_activations=True (optional fast path, SURVEY.md 8f-1): instead of calling the getters (sigmoid / exp /
     F.normalize: three kernels + autograd nodes per view, gaussian_model.py:95-118) the raw parameter tensors go straight
     to the rasteriser, which applies the activations and their Jacobians inside its kernels.  Same dict, same gradients
-    (they arrive at the raw tensors directly)."""
+    (they arrive at the raw tensors directly).  `pipe.antialiasing` (absent = False) turns on the screen-space mip filter."""
+    aa = bool(getattr(pipe, "antialiasing", False))
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
     try:
@@ -52,7 +54,7 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
         bg=bg_color, scale_modifier=scaling_modifier, viewmatrix=viewpoint_camera.world_view_transform,
         projmatrix=viewpoint_camera.full_proj_transform, sh_degree=pc.active_sh_degree,
         campos=viewpoint_camera.camera_center, prefiltered=False, debug=False)
-    rasterizer = GaussianRasterizer(raster_settings=settings)
+    rasterizer = GaussianRasterizer(raster_settings=settings, antialiasing=aa)
     shs = colors = None
     if override_color is None:
         shs = pc.get_features
@@ -65,7 +67,7 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
             means3D=xyz, opacities=op, viewmatrices=viewpoint_camera.world_view_transform[None], projmatrices=viewpoint_camera.full_proj_transform[None],
             camposs=viewpoint_camera.camera_center[None], tanfovx=[settings.tanfovx], tanfovy=[settings.tanfovy], image_height=settings.image_height,
             image_width=settings.image_width, bg=bg_color, sh_degree=pc.active_sh_degree, shs=shs, colors_precomp=colors, scales=sc, rotations=rot,
-            means2D=screenspace_points[None], scale_modifier=scaling_modifier, raw=True)
+            means2D=screenspace_points[None], scale_modifier=scaling_modifier, raw=True, antialiasing=aa)
         image, radii, depth, alpha = image[0], radii[0], depth[0], alpha[0]
         return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
                 "depth_3dgs": depth, "alpha_3dgs": alpha}
@@ -99,11 +101,12 @@ class _StackSinks(torch.autograd.Function):
         return (None, *g.unbind(0))
 
 
-def render_views(cameras, pc, bg_color, scaling_modifier=1.0):
+def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False):
     """All cameras share image size.  Returns the dict of `render` with a leading view axis:
     render [V,3,H,W], depth_3dgs/alpha_3dgs [V,1,H,W], radii [V,P], viewspace_points [V,P,3] (its .grad is [V,P,3]),
     plus viewspace_point_list: V leaf tensors [P,3] whose .grad backward fills -- what the reference's
-    `self.viewspace_point_list` holds (GaussianDreamer.py:242-250) and on_before_optimizer_step sums (:385-387)."""
+    `self.viewspace_point_list` holds (GaussianDreamer.py:242-250) and on_before_optimizer_step sums (:385-387).
+    antialiasing: the screen-space mip filter, as `rasterizer.rasterize_views`."""
     xyz = pc.get_xyz
     V = len(cameras)
     vm, pm, cp, tanx, tany = stack_cameras(cameras, xyz.device)
@@ -118,6 +121,6 @@ def render_views(cameras, pc, bg_color, scaling_modifier=1.0):
         means3D=xyz, opacities=pc.get_opacity, viewmatrices=vm, projmatrices=pm, camposs=cp, tanfovx=tanx, tanfovy=tany,
         image_height=int(cameras[0].image_height), image_width=int(cameras[0].image_width), bg=bg_color,
         sh_degree=pc.active_sh_degree, shs=pc.get_features, scales=pc.get_scaling, rotations=pc.get_rotation,
-        means2D=screenspace_points, scale_modifier=scaling_modifier)
+        means2D=screenspace_points, scale_modifier=scaling_modifier, antialiasing=antialiasing)
     return {"render": image, "viewspace_points": screenspace_points, "viewspace_point_list": sinks, "visibility_filter": radii > 0,
             "radii": radii, "depth_3dgs": depth, "alpha_3dgs": alpha}

@@ -159,6 +159,52 @@ int b200gs_backward_deterministic(const b200gs_params *prm,
                                   void *scratch, size_t scratch_bytes,
                                   void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *stream);
 
+/* ---- render options (additive to ABI 4) -----------------------------------------------------------------------------
+ * The *_opts entry points take the argument list of their plain counterpart with `opts` after `prm`.  opts == NULL means the
+ * defaults, which is exactly what b200gs_forward / b200gs_backward / b200gs_backward_deterministic do.  struct_bytes =
+ * sizeof(b200gs_render_opts) of the caller's header; a value too small to hold the fields the library reads returns
+ * B200GS_E_ARGS.  A backward call MUST get the same options as the forward call whose state buffers it reads.
+ *   antialiasing: 0 = off.  Non-zero = the screen-space mip filter: the covariance keeps its +0.3 px^2 dilation and the
+ *     opacity is multiplied by rho = sqrt(det(S) / det(S + 0.3 I)), S the projected 2D covariance, floored at rho = 0.005,
+ *     so that a Gaussian's integrated footprint does not depend on the pixel scale it is drawn at.  The backward then needs
+ *     opacities (as for raw_params); dL_dopacity is w.r.t. the opacity before the filter. */
+typedef struct b200gs_render_opts {
+    int32_t struct_bytes;   /* sizeof(b200gs_render_opts) */
+    int32_t antialiasing;   /* 0 | 1 */
+} b200gs_render_opts;
+int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                        const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                        const float *scales, const float *rotations, const float *cov3D_precomp,
+                        const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                        float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
+                        void *geom_buf, size_t geom_bytes,
+                        void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
+                        void *image_buf, size_t image_bytes,
+                        int64_t *num_rendered, void *stream);
+int b200gs_backward_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                         const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                         const float *scales, const float *rotations, const float *cov3D_precomp,
+                         const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                         const int32_t *radii,
+                         const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                         const void *image_buf, int64_t num_rendered,
+                         const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                         float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+                         float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                         void *scratch, size_t scratch_bytes, void *stream);
+int b200gs_backward_deterministic_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                                       const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                                       const float *scales, const float *rotations, const float *cov3D_precomp,
+                                       const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                       const int32_t *radii,
+                                       const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                       const void *image_buf, int64_t num_rendered,
+                                       const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                       float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+                                       float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                       void *scratch, size_t scratch_bytes,
+                                       void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *stream);
+
 /* Frustum test only (upstream markVisible): present[i] = 1 if p_view.z > 0.2 for view 0.  positions [P,3]. */
 int b200gs_mark_visible(int32_t P, const float *positions, const float *viewmatrix, const float *projmatrix,
                         uint8_t *present, void *stream);
