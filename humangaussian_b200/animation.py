@@ -57,11 +57,12 @@ def pack_frames_u8(color: torch.Tensor) -> torch.Tensor:
 
 @torch.no_grad()
 def render_frames(pc, xyz_frames: torch.Tensor, cameras, bg_color: torch.Tensor, scaling_modifier: float = 1.0,
-                  chunk: int = MAX_VIEWS, antialiasing: bool = False) -> torch.Tensor:
+                  chunk: int = MAX_VIEWS, antialiasing: bool = False, filter_3d: torch.Tensor = None) -> torch.Tensor:
     """Forward-only render of F frames with per-frame Gaussian centres xyz_frames [F,P,3]; everything else (scales,
     rotations, opacities, SH) is shared, exactly what animation.py changes between frames (only `_xyz`, :403).
     Returns uint8 frames [F,H,W,3] (the buffer animation.py appends to its video).  antialiasing: the screen-space mip
-    filter (rasterizer.rasterize_views)."""
+    filter (rasterizer.rasterize_views).  filter_3d: the 3D smoothing filter's [P] variances; the filter is per Gaussian, so
+    one set (computed in the canonical pose, filter3d.compute_filter_3d) serves every frame."""
     F = xyz_frames.shape[0]
     dev = xyz_frames.device
     vm, pm, cp, tanx, tany = stack_cameras(cameras, dev)
@@ -73,6 +74,6 @@ def render_frames(pc, xyz_frames: torch.Tensor, cameras, bg_color: torch.Tensor,
         color = rasterize_views(means3D=xyz_frames[f0:f1], opacities=op, viewmatrices=vm[f0:f1], projmatrices=pm[f0:f1],
                                 camposs=cp[f0:f1], tanfovx=tanx[f0:f1], tanfovy=tany[f0:f1], image_height=H, image_width=W,
                                 bg=bg_color, sh_degree=pc.active_sh_degree, shs=sh, scales=sc, rotations=rot,
-                                scale_modifier=scaling_modifier, antialiasing=antialiasing)[0]
+                                scale_modifier=scaling_modifier, antialiasing=antialiasing, filter_3d=filter_3d)[0]
         outs.append(pack_frames_u8(color))
     return torch.cat(outs, 0)

@@ -100,13 +100,18 @@ static int check_common(const b200gs_params *p, const float *shs, const float *c
     return B200GS_OK;
 }
 
-// b200gs_render_opts: NULL = the defaults; a struct too short to hold the fields this library reads is an argument error
-static int read_opts(const b200gs_render_opts *o, bool *aa)
+// b200gs_render_opts: NULL = the defaults; a struct too short to hold the fields this library reads is an argument error.
+// struct_bytes = 8 is the header before filter3d_var (no 3D filter); a size that cuts that pointer is an argument error.
+static int read_opts(const b200gs_render_opts *o, bool *aa, const float **f3d)
 {
     *aa = false;
+    *f3d = nullptr;
     if (!o) return B200GS_OK;
-    if (o->struct_bytes < (int32_t)(offsetof(b200gs_render_opts, antialiasing) + sizeof(o->antialiasing))) return B200GS_E_ARGS;
+    const int32_t n0 = (int32_t)(offsetof(b200gs_render_opts, antialiasing) + sizeof(o->antialiasing));
+    const int32_t n1 = (int32_t)(offsetof(b200gs_render_opts, filter3d_var) + sizeof(o->filter3d_var));
+    if (o->struct_bytes < n0 || (o->struct_bytes > n0 && o->struct_bytes < n1)) return B200GS_E_ARGS;
     *aa = o->antialiasing != 0;
+    if (o->struct_bytes >= n1) *f3d = o->filter3d_var;
     return B200GS_OK;
 }
 
@@ -118,10 +123,12 @@ int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts
                         size_t image_bytes, int64_t *num_rendered, void *stream)
 {
     bool aa = false;
-    int rc = read_opts(opts, &aa);
+    const float *f3d = nullptr;
+    int rc = read_opts(opts, &aa, &f3d);
     if (rc) return rc;
     rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
+    if (f3d && cov3D_precomp) return B200GS_E_ARGS; // the 3D filter widens scales; a precomputed covariance has none
     if (!means3D || !opacities || !bg || !viewmatrix || !projmatrix || !campos || !out_color || !out_depth || !out_alpha ||
         !radii || !geom_buf || !binning_buf || !image_buf || !num_rendered)
         return B200GS_E_ARGS;
@@ -155,7 +162,7 @@ int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts
         a.radii = radii; a.recs = (GeomRec *)(gb + GL.recs); a.tiles_touched = (uint32_t *)(gb + GL.tiles_touched);
         a.rects = (uint2 *)(gb + GL.rects); a.clamped = (uint8_t *)(gb + GL.clamped);
         a.dkeys = (uint32_t *)(bb + BL.dkeys_in); a.order_in = (uint32_t *)(bb + BL.order_in);
-        { StageTimer t(B200GS_STAGE_PREPROCESS, st); launch_preprocess_fwd(a, V, aa, st); }
+        { StageTimer t(B200GS_STAGE_PREPROCESS, st); launch_preprocess_fwd(a, V, aa, f3d, st); }
         g_launches += 1;
         uint32_t *offsets = (uint32_t *)(gb + GL.offsets); // inclusive scan of tiles_touched in DEPTH order
         const int64_t n_vp = (int64_t)P * V;
@@ -254,7 +261,9 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
                          int64_t *n_partials)
 {
     bool aa = false;
-    if (read_opts(opts, &aa)) return B200GS_E_ARGS;
+    const float *f3d = nullptr;
+    if (read_opts(opts, &aa, &f3d)) return B200GS_E_ARGS;
+    if (f3d && cov3D_precomp) return B200GS_E_ARGS;
     if (det) {
         if (!blend_bwd_has_deterministic()) return B200GS_E_UNSUPPORTED;
         if (!n_partials || !det_buf || partial_capacity < 0) return B200GS_E_ARGS;
@@ -264,7 +273,7 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     }
     int rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
-    if ((prm->raw_params || aa) && !opacities) return B200GS_E_ARGS;
+    if ((prm->raw_params || aa || f3d) && !opacities) return B200GS_E_ARGS;
     if (!means3D || !bg || !viewmatrix || !projmatrix || !campos || !radii || !geom_buf || !binning_buf || !image_buf ||
         !dL_dmeans3D || !dL_dmeans2D || !dL_dopacity || !scratch)
         return B200GS_E_ARGS;
@@ -344,7 +353,8 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     a.recs = (const GeomRec *)(gb + GL.recs); a.moments = blend_sgrad_is_moments();
     a.dL_dmeans3D = dL_dmeans3D; a.dL_dmeans2D = dL_dmeans2D; a.dL_dsh = dL_dsh; a.dL_dcolors = dL_dcolors;
     a.dL_dopacity = dL_dopacity; a.dL_dscales = dL_dscales; a.dL_drots = dL_drots; a.dL_dcov3D = dL_dcov3D;
-    { StageTimer t(B200GS_STAGE_PREPROCESS_BWD, st); launch_preprocess_bwd(a, aa, st); }
+    a.f3d_var = f3d;
+    { StageTimer t(B200GS_STAGE_PREPROCESS_BWD, st); launch_preprocess_bwd(a, aa, f3d != nullptr, st); }
     g_launches += det ? 1 : 2; // (the deterministic blend stage counted its own launches)
     CK(cudaGetLastError(), "backward launch");
     return B200GS_OK;
@@ -410,6 +420,23 @@ int b200gs_backward_deterministic(const b200gs_params *prm, const float *means3D
                          campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
                          scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials);
+}
+
+int b200gs_sampling_rate(int32_t P, int32_t n_views, const float *means3D, const float *viewmatrix, const float *tanfovx,
+                         const float *tanfovy, int32_t image_height, int32_t image_width, float *max_rate, void *stream)
+{
+    if (P < 0 || n_views < 1 || image_height < 1 || image_width < 1 || !tanfovx || !tanfovy) return B200GS_E_ARGS;
+    if (n_views > B200GS_MAX_VIEWS) return B200GS_E_RANGE;
+    if (P == 0) return B200GS_OK;
+    if (!means3D || !viewmatrix || !max_rate) return B200GS_E_ARGS;
+    RateArgs a;
+    a.P = P; a.nviews = n_views; a.H = image_height; a.W = image_width;
+    a.means = means3D; a.view = viewmatrix; a.max_rate = max_rate;
+    for (int v = 0; v < n_views; v++) { a.tanfovx[v] = tanfovx[v]; a.tanfovy[v] = tanfovy[v]; }
+    launch_sampling_rate(a, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "sampling_rate launch");
+    return B200GS_OK;
 }
 
 int b200gs_mark_visible(int32_t P, const float *positions, const float *viewmatrix, const float *projmatrix,

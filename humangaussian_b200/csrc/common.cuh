@@ -58,6 +58,8 @@ __device__ __forceinline__ float gs_affine(float m0, float m1, float m2, float m
     a = ffma(m2, z, a);
     return fadd(a, m3);
 }
+// focal length in pixels of an image extent (W or H) under tan(fov/2): F1's fx / fy, shared with the 3D filter's rates
+__device__ __forceinline__ float gs_focal(int extent, float tanfov) { return fdiv((float)extent, fmul(2.0f, tanfov)); }
 __device__ __forceinline__ float gs_dot3(float a0, float a1, float a2, float b0, float b1, float b2)
 {
     float a = fmul(a0, b0);

@@ -36,6 +36,7 @@ struct PreBwdArgs {
     const GeomRec *recs;     // [V*P] forward records (conic, opacity) -- used when sgrad holds moments
     int moments;             // 0: classic float (dx,dy,dA,dBh,dC,dO,dr,dg,db,dd); 1: float moments (S0,Sx,Sy,Sxx,Sxy,Syy,cr,cg,cb,cd)
     float *dL_dmeans3D, *dL_dmeans2D, *dL_dsh, *dL_dcolors, *dL_dopacity, *dL_dscales, *dL_drots, *dL_dcov3D;
+    const float *f3d_var;    // [P] 3D filter variances, read by the F3D instantiations (last: the others' layout stays)
 };
 
 struct BlendArgs {
@@ -65,9 +66,18 @@ struct BlendBwdArgs {
     void *sgrad;                                    // [V*P] accumulators (format: blend_sgrad_is_moments()), zeroed by the caller
 };
 
-// aa: the antialiasing filter (record opacity op * rho; DESIGN.md section 2)
-void launch_preprocess_fwd(const PreArgs &a, int V, bool aa, cudaStream_t st);
-void launch_preprocess_bwd(const PreBwdArgs &a, bool aa, cudaStream_t st);
+// aa: the antialiasing filter (record opacity op * rho; DESIGN.md section 2).  f3d / f3d_var (NULL = off): the 3D smoothing
+// filter (scales widened by the [P] variances, opacity compensated; DESIGN.md section 2)
+void launch_preprocess_fwd(const PreArgs &a, int V, bool aa, const float *f3d_var, cudaStream_t st);
+void launch_preprocess_bwd(const PreBwdArgs &a, bool aa, bool f3d, cudaStream_t st);
+// per-Gaussian maximal sampling rate over n_views <= GS_MAX_VIEWS cameras, folded into max_rate by max (filter3d.cu)
+struct RateArgs {
+    int P, nviews, H, W;
+    const float *means, *view; // [P,3], [nviews,16]
+    float tanfovx[GS_MAX_VIEWS], tanfovy[GS_MAX_VIEWS];
+    float *max_rate;           // [P] in/out
+};
+void launch_sampling_rate(const RateArgs &a, cudaStream_t st);
 void launch_mark_visible(int P, const float *pos, const float *V, uint8_t *present, cudaStream_t st);
 
 // binning: depth pre-sort of the V*P Gaussians, scan in depth order, tile-key emission, stable tile sort, ranges

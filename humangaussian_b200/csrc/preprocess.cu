@@ -75,6 +75,21 @@ __device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, flo
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(hi, max(lo, v)); }
 
+// The 3D smoothing filter (DESIGN.md section 2) on one Gaussian's activated scales s (before scale_modifier) and variance
+// v: t_i = s_i^2 + v, s'_i = sqrt(t_i), r_i = s_i^2 / t_i (1 where t_i = 0); returns coef = sqrt(r_0 r_1 r_2), the factor
+// that keeps o * sqrt(det Sigma) when the opacity becomes o' = o * coef.  IEEE float32, no contraction.
+__device__ __forceinline__ float gs_filter3d(float *s, float v, float *t, float *r)
+{
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const float s2 = fmul(s[k], s[k]);
+        t[k] = fadd(s2, v);
+        r[k] = t[k] > 0.0f ? fdiv(s2, t[k]) : 1.0f;
+        s[k] = fsqrt(t[k]);
+    }
+    return fsqrt(fmul(fmul(r[0], r[1]), r[2]));
+}
+
 // torch.sigmoid / F.normalize(dim=1) as torch's CUDA kernels evaluate them in float32
 __device__ __forceinline__ float gs_sigmoid(float x) { return fdiv(1.0f, fadd(1.0f, expf(-x))); }
 __device__ __forceinline__ float gs_normalize4(float *q)
@@ -93,12 +108,14 @@ __device__ __forceinline__ float gs_normalize4(float *q)
 // DEG = -1: colours are given (colors_precomp), no SH.
 // AA: the antialiasing filter (DESIGN.md section 2): the record's opacity is op * rho, rho = sqrt(det0 / det), det0 the
 // determinant of the 2D covariance before the +0.3 px^2 dilation; the support box is bounded with that opacity too.
+// F3D: the 3D smoothing filter, once per Gaussian before the view loop: the activated scales become s' (gs_filter3d) and the
+// opacity o * coef; everything after (scale_modifier, the covariance, AA's rho, the support box) sees s' and o * coef.
 // ------------------------------------------------------------------------------------------------
 #ifndef PFWD_MIN_BLOCKS
 #define PFWD_MIN_BLOCKS 3 // 80 registers; H100 (400 W): 2 / 4 blocks make this kernel 33 % / 26 % slower
 #endif
-template <int DEG, bool AA>
-__global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(PreArgs a, int nviews)
+template <int DEG, bool AA, bool F3D>
+__global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(PreArgs a, int nviews, const float *f3d_var)
 {
     constexpr int NB = DEG < 0 ? 1 : (DEG + 1) * (DEG + 1);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -127,6 +144,10 @@ __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(Pr
         if (a.raw) {
             s3[0] = expf(s3[0]); s3[1] = expf(s3[1]); s3[2] = expf(s3[2]);
             gs_normalize4(q);
+        }
+        if (F3D) {
+            float t[3], r[3];
+            op = fmul(op, gs_filter3d(s3, __ldg(f3d_var + i), t, r));
         }
         build_cov3d(s3, a.mod, q, c6);
     }
@@ -178,7 +199,7 @@ __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(Pr
             const float ndcx = fmul(hx, pw), ndcy = fmul(hy, pw);
 
             const float tanx = a.tanfovx[v], tany = a.tanfovy[v];
-            const float fx = fdiv((float)a.W, fmul(2.0f, tanx)), fy = fdiv((float)a.H, fmul(2.0f, tany));
+            const float fx = gs_focal(a.W, tanx), fy = gs_focal(a.H, tany);
             const float limx = fmul(1.3f, tanx), limy = fmul(1.3f, tany);
             const float txtz = fdiv(tx, tz), tytz = fdiv(ty, tz);
             const float cx = fmul(fminf(limx, fmaxf(-limx, txtz)), tz);
@@ -288,20 +309,25 @@ __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(Pr
     }
 }
 
-template <bool AA>
-static void launch_preprocess_fwd_t(const PreArgs &a, int V, cudaStream_t st)
+template <bool AA, bool F3D>
+static void launch_preprocess_fwd_t(const PreArgs &a, int V, const float *f3d_var, cudaStream_t st)
 {
     const dim3 grid((a.P + 255) / 256);
-    if (!a.shs) preprocess_fwd_kernel<-1, AA><<<grid, 256, 0, st>>>(a, V);
-    else if (a.deg == 0) preprocess_fwd_kernel<0, AA><<<grid, 256, 0, st>>>(a, V);
-    else if (a.deg == 1) preprocess_fwd_kernel<1, AA><<<grid, 256, 0, st>>>(a, V);
-    else if (a.deg == 2) preprocess_fwd_kernel<2, AA><<<grid, 256, 0, st>>>(a, V);
-    else preprocess_fwd_kernel<3, AA><<<grid, 256, 0, st>>>(a, V);
+    if (!a.shs) preprocess_fwd_kernel<-1, AA, F3D><<<grid, 256, 0, st>>>(a, V, f3d_var);
+    else if (a.deg == 0) preprocess_fwd_kernel<0, AA, F3D><<<grid, 256, 0, st>>>(a, V, f3d_var);
+    else if (a.deg == 1) preprocess_fwd_kernel<1, AA, F3D><<<grid, 256, 0, st>>>(a, V, f3d_var);
+    else if (a.deg == 2) preprocess_fwd_kernel<2, AA, F3D><<<grid, 256, 0, st>>>(a, V, f3d_var);
+    else preprocess_fwd_kernel<3, AA, F3D><<<grid, 256, 0, st>>>(a, V, f3d_var);
 }
-void launch_preprocess_fwd(const PreArgs &a, int V, bool aa, cudaStream_t st)
+void launch_preprocess_fwd(const PreArgs &a, int V, bool aa, const float *f3d_var, cudaStream_t st)
 {
-    if (aa) launch_preprocess_fwd_t<true>(a, V, st);
-    else launch_preprocess_fwd_t<false>(a, V, st);
+    if (f3d_var) {
+        if (aa) launch_preprocess_fwd_t<true, true>(a, V, f3d_var, st);
+        else launch_preprocess_fwd_t<false, true>(a, V, f3d_var, st);
+    } else {
+        if (aa) launch_preprocess_fwd_t<true, false>(a, V, f3d_var, st);
+        else launch_preprocess_fwd_t<false, false>(a, V, f3d_var, st);
+    }
 }
 
 __global__ void mark_visible_kernel(int P, const float *pos, const float *V, uint8_t *present)
@@ -320,11 +346,15 @@ void launch_mark_visible(int P, const float *pos, const float *V, uint8_t *prese
 // B2 + B3: one thread per Gaussian, loops over the views of the batch and SUMS parameter gradients
 // (deterministic: no atomics at the parameter level).  Plain float arithmetic (tolerance-compared).
 // AA: the forward's record opacity was op * rho (F1): dL/dop = rho * S0, and dL/drho = op * S0 joins the cov2D gradient.
+// F3D: the view loop yields the gradients w.r.t. the filtered s' and o' = o * coef; after it, once per Gaussian,
+//   dL/do = coef * g_o',  dL/ds_i = g_s'_i * s_i / s'_i + o * g_o' * sqrt(r_j r_k) * v / (t_i s'_i)
+// (the second factor is dcoef/ds_i in a form without cancellation, finite at s_i = 0).  The filter's quantities are
+// recomputed there from the inputs rather than held across the loop; with AA, coef stays live for the per-view o'.
 // ------------------------------------------------------------------------------------------------
 #ifndef PBWD_MIN_BLOCKS
 #define PBWD_MIN_BLOCKS 4 // 128 registers; 5 / 6 blocks (96 / 80 registers) spill the 48 SH accumulators
 #endif
-template <int DEG, bool AA>
+template <int DEG, bool AA, bool F3D>
 __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(PreBwdArgs a)
 {
     constexpr int nb = DEG < 0 ? 1 : (DEG + 1) * (DEG + 1);
@@ -334,6 +364,7 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
 
     float c6[6];
     float R[3][3], s[3] = {0, 0, 0}, q[4] = {0, 0, 0, 0}, qnorm = 1.0f;
+    float coef = 1.0f; // F3D: o' = o * coef
     if (a.cov_pre) {
         for (int k = 0; k < 6; k++) c6[k] = a.cov_pre[6 * (size_t)i + k];
     } else {
@@ -342,6 +373,10 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
         if (a.raw) { // the same activations F1 applied
             s3[0] = expf(s3[0]); s3[1] = expf(s3[1]); s3[2] = expf(s3[2]);
             qnorm = gs_normalize4(q);
+        }
+        if (F3D) { // the same filter F1 applied: s3 becomes s'
+            float t[3], r[3];
+            coef = gs_filter3d(s3, a.f3d_var[i], t, r);
         }
         build_cov3d(s3, a.mod, q, c6);
         const float r = q[0], x = q[1], y = q[2], z = q[3];
@@ -465,7 +500,8 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
                 // the opacity before the filter (after the sigmoid for raw parameters), re-read per view (an L1 hit) rather
                 // than kept live across the view loop
                 const float opr = __ldg(a.opac + i);
-                const float op = a.raw ? gs_sigmoid(opr) : opr;
+                float op = a.raw ? gs_sigmoid(opr) : opr;
+                if (F3D) op *= coef; // the opacity rho multiplied in F1 is o'
                 const float k = GS_DILATE * op * gO / (rho * denom * denom);
                 ra = 0.5f * k * (cc0 * cc + cb * cb);
                 rc = 0.5f * k * (ca0 * ca + cb * cb);
@@ -576,6 +612,27 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
         float *o = a.dL_dmeans3D + 3 * ((a.means_view_stride ? (size_t)(a.V - 1) * a.P : 0) + (size_t)i);
         o[0] = dmean[0]; o[1] = dmean[1]; o[2] = dmean[2];
     }
+    // F3D: dL/ds_i = f3s[i] * dL/ds'_i + f3q[i]; so = the activated scales before the filter (the exp Jacobian's factor)
+    float f3s[3] = {1.f, 1.f, 1.f}, f3q[3] = {0.f, 0.f, 0.f}, so[3] = {0.f, 0.f, 0.f};
+    if (F3D && !a.cov_pre) {
+        const float v = a.f3d_var[i];
+        float t[3], r[3], sp[3];
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            so[k] = a.scales[3 * (size_t)i + k];
+            if (a.raw) so[k] = expf(so[k]);
+            sp[k] = so[k];
+        }
+        const float cf = gs_filter3d(sp, v, t, r);
+        const float opa = a.raw ? gs_sigmoid(a.opac[i]) : a.opac[i];
+        const float og = opa * dop; // o * g_o'
+        dop *= cf;
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            f3s[k] = t[k] > 0.f ? so[k] / sp[k] : 1.f;
+            if (v > 0.f) f3q[k] = og * sqrtf(r[(k + 1) % 3] * r[(k + 2) % 3]) * v / (t[k] * sp[k]);
+        }
+    }
     if (a.raw) { // d sigmoid(x)/dx = o (1 - o)
         const float o = gs_sigmoid(a.opac[i]);
         dop *= o * (1.0f - o);
@@ -606,8 +663,14 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
             for (int k = 0; k < 3; k++) dLm[r2][k] = 2.f * (dS[r2][0] * L[0][k] + dS[r2][1] * L[1][k] + dS[r2][2] * L[2][k]);
 #pragma unroll
         for (int k = 0; k < 3; k++) {
-            // raw: d exp(x)/dx = exp(x) = s[k] / mod
-            a.dL_dscales[3 * (size_t)i + k] = (a.raw ? s[k] : a.mod) * (R[0][k] * dLm[0][k] + R[1][k] * dLm[1][k] + R[2][k] * dLm[2][k]);
+            if (F3D) { // through the filter (f3s = 1, f3q = 0 where v = 0), then exp's Jacobian so[k]
+                float g = f3s[k] * (a.mod * (R[0][k] * dLm[0][k] + R[1][k] * dLm[1][k] + R[2][k] * dLm[2][k]));
+                if (f3q[k] != 0.f) g += f3q[k];
+                a.dL_dscales[3 * (size_t)i + k] = a.raw ? g * so[k] : g;
+            } else {
+                // raw: d exp(x)/dx = exp(x) = s[k] / mod
+                a.dL_dscales[3 * (size_t)i + k] = (a.raw ? s[k] : a.mod) * (R[0][k] * dLm[0][k] + R[1][k] * dLm[1][k] + R[2][k] * dLm[2][k]);
+            }
 #pragma unroll
             for (int r2 = 0; r2 < 3; r2++) dR[r2][k] = dLm[r2][k] * s[k];
         }
@@ -630,18 +693,23 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
     }
 }
 
-template <bool AA>
+template <bool AA, bool F3D>
 static void launch_preprocess_bwd_t(const PreBwdArgs &a, cudaStream_t st)
 {
     const int grid = (a.P + 127) / 128;
-    if (!a.shs) preprocess_bwd_kernel<-1, AA><<<grid, 128, 0, st>>>(a);
-    else if (a.deg == 0) preprocess_bwd_kernel<0, AA><<<grid, 128, 0, st>>>(a);
-    else if (a.deg == 1) preprocess_bwd_kernel<1, AA><<<grid, 128, 0, st>>>(a);
-    else if (a.deg == 2) preprocess_bwd_kernel<2, AA><<<grid, 128, 0, st>>>(a);
-    else preprocess_bwd_kernel<3, AA><<<grid, 128, 0, st>>>(a);
+    if (!a.shs) preprocess_bwd_kernel<-1, AA, F3D><<<grid, 128, 0, st>>>(a);
+    else if (a.deg == 0) preprocess_bwd_kernel<0, AA, F3D><<<grid, 128, 0, st>>>(a);
+    else if (a.deg == 1) preprocess_bwd_kernel<1, AA, F3D><<<grid, 128, 0, st>>>(a);
+    else if (a.deg == 2) preprocess_bwd_kernel<2, AA, F3D><<<grid, 128, 0, st>>>(a);
+    else preprocess_bwd_kernel<3, AA, F3D><<<grid, 128, 0, st>>>(a);
 }
-void launch_preprocess_bwd(const PreBwdArgs &a, bool aa, cudaStream_t st)
+void launch_preprocess_bwd(const PreBwdArgs &a, bool aa, bool f3d, cudaStream_t st)
 {
-    if (aa) launch_preprocess_bwd_t<true>(a, st);
-    else launch_preprocess_bwd_t<false>(a, st);
+    if (f3d) {
+        if (aa) launch_preprocess_bwd_t<true, true>(a, st);
+        else launch_preprocess_bwd_t<false, true>(a, st);
+    } else {
+        if (aa) launch_preprocess_bwd_t<true, false>(a, st);
+        else launch_preprocess_bwd_t<false, false>(a, st);
+    }
 }

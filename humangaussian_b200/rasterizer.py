@@ -55,11 +55,26 @@ class _Params(C.Structure):
 
 class _RenderOpts(C.Structure):
     """b200gs_render_opts (include/b200gs.h): options of the *_opts entry points"""
-    _fields_ = [("struct_bytes", C.c_int32), ("antialiasing", C.c_int32)]
+    _fields_ = [("struct_bytes", C.c_int32), ("antialiasing", C.c_int32), ("filter3d_var", C.c_void_p)]
 
 
-def _render_opts(antialiasing: bool):
-    return _RenderOpts(C.sizeof(_RenderOpts), int(bool(antialiasing)))
+def _render_opts(antialiasing: bool, filter_3d: Optional[torch.Tensor] = None):
+    return _RenderOpts(C.sizeof(_RenderOpts), int(bool(antialiasing)), None if filter_3d is None else filter_3d.data_ptr())
+
+
+def _check_filter_3d(filter_3d, P, device, cov3D_precomp=None):
+    """The 3D smoothing filter's variances: a [P] fp32 tensor on the Gaussians' device, or None.  The values are the
+    caller's contract (finite, >= 0; filter3d.compute_filter_3d meets it); checking them would cost a host sync."""
+    if filter_3d is None:
+        return None
+    if cov3D_precomp is not None:
+        raise ValueError("b200gs: the 3D filter widens scales; it cannot be used with cov3D_precomp")
+    if not isinstance(filter_3d, torch.Tensor) or filter_3d.dtype != torch.float32 or filter_3d.device != device or \
+            filter_3d.dim() != 1 or filter_3d.shape[0] != P:
+        raise ValueError(f"b200gs: filter_3d must be a [{P}] float32 tensor on {device} (recompute it after densify / prune); got "
+                         f"{tuple(filter_3d.shape) if isinstance(filter_3d, torch.Tensor) else type(filter_3d).__name__}"
+                         f"{'' if not isinstance(filter_3d, torch.Tensor) else f' {filter_3d.dtype} on {filter_3d.device}'}")
+    return filter_3d.detach().contiguous()
 
 
 class _StateView(C.Structure):
@@ -76,7 +91,7 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_knn_scratch_bytes", "b200gs_dist2_knn3", "b200gs_densify_stats", "b200gs_densify_scratch_bytes",
            "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed", "b200gs_deterministic_bytes",
            "b200gs_backward_deterministic", "b200gs_forward_opts", "b200gs_backward_opts",
-           "b200gs_backward_deterministic_opts"]
+           "b200gs_backward_deterministic_opts", "b200gs_sampling_rate"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -113,6 +128,8 @@ def load_library():
     L.b200gs_backward_deterministic_opts.restype = C.c_int
     L.b200gs_backward_deterministic_opts.argtypes = ([L.b200gs_backward_deterministic.argtypes[0], vp] +
                                                      L.b200gs_backward_deterministic.argtypes[1:])
+    L.b200gs_sampling_rate.restype = C.c_int
+    L.b200gs_sampling_rate.argtypes = [i32, i32, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float), i32, i32, vp, vp]
     L.b200gs_mark_visible.restype = C.c_int
     L.b200gs_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
     L.b200gs_describe_state.restype = C.c_int
@@ -294,7 +311,7 @@ def release_cached_buffers():
 class _Ctx:
     """What one forward keeps for its backward (upstream keeps geomBuffer/binningBuffer/imgBuffer the same way)."""
     __slots__ = ("prm", "tanx", "tany", "geom", "binning", "image", "scratch", "capacity", "num_rendered", "radii", "V", "P", "H",
-                 "W", "M", "opts", "__weakref__")
+                 "W", "M", "opts", "f3d", "__weakref__")
 
 
 def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=False, per_view_means=False, raw=False):
@@ -307,10 +324,11 @@ def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=F
 
 def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                   campos, tanfovx, tanfovy, H, W, sh_degree, scale_modifier, prefiltered=False, debug=False, raw=False,
-                  antialiasing=False):
+                  antialiasing=False, filter_3d=None):
     """All tensors float32 contiguous on one CUDA device.  viewmatrix/projmatrix [V,4,4], campos [V,3].
     raw: opacities / scales / rotations are GaussianModel's raw parameters (activations fused into the kernels).
-    antialiasing: the screen-space mip filter (b200gs_render_opts); the state remembers it for the backward."""
+    antialiasing: the screen-space mip filter; filter_3d: the 3D smoothing filter's [P] variances (b200gs_render_opts).
+    The state remembers both for the backward."""
     L = load_library()
     dev = means3D.device
     if dev.type != "cuda":
@@ -326,6 +344,7 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
             ((scales is not None or rotations is not None) and cov3D_precomp is not None):
         raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
     M = 0 if shs is None else shs.shape[1]
+    filter_3d = _check_filter_3d(filter_3d, P, dev, cov3D_precomp)
     prm, tx, ty = _make_params(P, V, sh_degree, M, H, W, scale_modifier, tanfovx, tanfovy, prefiltered, debug, per_view_means, raw)
     u8 = dict(dtype=torch.uint8, device=dev)
     color = torch.empty(V, 3, H, W, dtype=torch.float32, device=dev)
@@ -336,7 +355,7 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     cap = _cap_hint.get(key, max(1 << 16, 4 * P * V))
     n_out = C.c_int64(0)
     stream = torch.cuda.current_stream(dev).cuda_stream
-    opts = _render_opts(True) if antialiasing else None
+    opts = _render_opts(antialiasing, filter_3d) if (antialiasing or filter_3d is not None) else None
     # with the defaults the plain entry point runs (b200gs_forward == b200gs_forward_opts with NULL options)
     fwd = (lambda *a: L.b200gs_forward_opts(a[0], C.byref(opts), *a[1:])) if opts is not None else L.b200gs_forward
     with torch.cuda.device(dev):
@@ -367,7 +386,7 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     st.prm, st.tanx, st.tany = prm, tx, ty
     st.geom, st.binning, st.image, st.scratch, st.capacity, st.num_rendered = geom, binning, image, bufs["scratch"], cap, int(n_out.value)
     st.radii, st.V, st.P, st.H, st.W, st.M = radii, V, P, H, W, M
-    st.opts = opts
+    st.opts, st.f3d = opts, filter_3d  # the backward reads the same variances (st keeps them alive)
     weakref.finalize(st, _pool.give, pkey, bufs)  # when the autograd graph drops the state, the buffers are parked for re-use
     return color, radii, depth, alpha, st
 
@@ -467,10 +486,11 @@ class _RasterizeViews(torch.autograd.Function):
         bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, prefiltered, debug = cams[:12]
         raw = bool(cams[12]) if len(cams) > 12 else False
         aa = bool(cams[13]) if len(cams) > 13 else False
+        f3d = cams[14] if len(cams) > 14 else None
         dev = means3D.device
         args = [_f32c(t, dev) for t in (means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)]
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
-        color, radii, depth, alpha, st = _forward_impl(*args, *camt, tanx, tany, H, W, deg, mod, prefiltered, debug, raw, aa)
+        color, radii, depth, alpha, st = _forward_impl(*args, *camt, tanx, tany, H, W, deg, mod, prefiltered, debug, raw, aa, f3d)
         ctx.st, ctx.squeeze = st, squeeze
         _save(ctx, args + camt)
         ctx.in_shapes = [None if t is None else t.shape for t in (means3D, means2D, shs, colors_precomp, opacities, scales,
@@ -556,8 +576,12 @@ class GaussianRasterizer(nn.Module):
 
 def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, tanfovx, tanfovy, image_height, image_width,
                     bg, sh_degree=0, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
-                    means2D=None, scale_modifier=1.0, raw=False, antialiasing=False):
+                    means2D=None, scale_modifier=1.0, raw=False, antialiasing=False, filter_3d=None):
     """Render V cameras of one Gaussian set in ONE call (one preprocess/sort/blend launch set, one host sync).
+
+    filter_3d: [P] fp32 variances of the 3D smoothing filter (`filter3d.compute_filter_3d`), or None: each Gaussian's
+    activated scales become sqrt(s^2 + v) and its opacity is scaled to keep its integrated 3D weight, inside the kernels
+    (DESIGN.md section 2).  Gradients stay w.r.t. the unfiltered parameters; v gets none.  Not with cov3D_precomp.
 
     antialiasing=True: the screen-space mip filter -- each Gaussian's opacity is scaled by sqrt(det(S) / det(S + 0.3 I)) of
     its projected covariance S, so its footprint keeps its integrated weight at any pixel scale (DESIGN.md section 2).
@@ -579,13 +603,14 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                                 image_width=image_width, bg=bg, sh_degree=sh_degree, shs=shs, colors_precomp=colors_precomp,
                                 scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
                                 means2D=None if means2D is None else means2D[i:i + MAX_VIEWS], scale_modifier=scale_modifier, raw=raw,
-                                antialiasing=antialiasing)
+                                antialiasing=antialiasing, filter_3d=filter_3d)
                 for i in range(0, V, MAX_VIEWS)]
         return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
+    _check_filter_3d(filter_3d, means3D.shape[-2], means3D.device, cov3D_precomp)
     if means2D is None:
         means2D = torch.zeros(V, means3D.shape[-2], 3, dtype=torch.float32, device=means3D.device)
     cams = (bg, viewmatrices, projmatrices, camposs, list(tanfovx), list(tanfovy), int(image_height), int(image_width),
-            int(sh_degree), float(scale_modifier), False, False, bool(raw), bool(antialiasing))
+            int(sh_degree), float(scale_modifier), False, False, bool(raw), bool(antialiasing), filter_3d)
     try:
         return _RasterizeViews.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, False)
     except InstanceLimitError:
@@ -597,7 +622,8 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                             projmatrices=projmatrices[sl], camposs=camposs[sl], tanfovx=list(tanfovx)[sl], tanfovy=list(tanfovy)[sl],
                             image_height=image_height, image_width=image_width, bg=bg, sh_degree=sh_degree, shs=shs,
                             colors_precomp=colors_precomp, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
-                            means2D=means2D[sl], scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing)
+                            means2D=means2D[sl], scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing,
+                            filter_3d=filter_3d)
             for sl in (slice(0, h), slice(h, V))]
     return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
 
@@ -629,12 +655,12 @@ def _split_packed(flat: torch.Tensor, P: int, M: int):
 class _RasterizePacked(torch.autograd.Function):
     @staticmethod
     def forward(ctx, packed, means2D, P, M, cams):
-        bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, raw, aa = cams
+        bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, raw, aa, f3d = cams
         dev = packed.device
         xyz, sc, rot, op, sh = _split_packed(packed.detach(), P, M)
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
         color, radii, depth, alpha, st = _forward_impl(xyz, sh, None, op, sc, rot, None, *camt, tanx, tany, H, W, deg, mod, raw=raw,
-                                                       antialiasing=aa)
+                                                       antialiasing=aa, filter_3d=f3d)
         ctx.st, ctx.P, ctx.M = st, P, M
         ctx.save_for_backward(packed, *camt)
         ctx.mark_non_differentiable(radii)
@@ -655,14 +681,15 @@ class _RasterizePacked(torch.autograd.Function):
 
 
 def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, viewmatrices, projmatrices, camposs, tanfovx, tanfovy,
-                           image_height, image_width, bg, sh_degree=0, means2D=None, scale_modifier=1.0, raw=False, antialiasing=False):
+                           image_height, image_width, bg, sh_degree=0, means2D=None, scale_modifier=1.0, raw=False, antialiasing=False,
+                           filter_3d=None):
     """`rasterize_views` over ONE flat fp32 buffer [xyz 3P | scales 3P | rotations 4P | opacities P | shs 3*K*P], each
     field starting on a 16-byte boundary (`packed_layout`; what `dist.pack` produces, broadcast once per parameter
     version).  raw=False: post-activation values, as the rasteriser's classic inputs.  raw=True: the buffer holds the
     optimiser's RAW parameters (log-scales, un-normalised quaternions, opacity logits; SH = cat(f_dc, f_rest)); the
     activations of gaussian_model.py:95-118 and their Jacobians run inside the kernels, so `packed.grad` is the gradient
     of the raw parameters and a training step needs no activation kernels, no pack copy and no autograd nodes besides
-    this one.  antialiasing: as `rasterize_views`.  The backward
+    this one.  antialiasing, filter_3d: as `rasterize_views`.  The backward
     kernels write the parameter gradients straight into one buffer of the same layout, which becomes `packed.grad`
     as is: no per-tensor gradient accumulation, and on several GPUs that buffer is the all-reduce payload in place.
     V <= MAX_VIEWS.  Returns color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W]."""
@@ -673,10 +700,11 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
     V = viewmatrices.shape[0]
     if V > MAX_VIEWS:
         raise ValueError(f"b200gs: at most {MAX_VIEWS} views per packed call")
+    _check_filter_3d(filter_3d, P, packed.device)
     if means2D is None:
         means2D = torch.zeros(V, P, 3, dtype=torch.float32, device=packed.device)
     cams = (bg, viewmatrices, projmatrices, camposs, list(tanfovx), list(tanfovy), int(image_height), int(image_width),
-            int(sh_degree), float(scale_modifier), bool(raw), bool(antialiasing))
+            int(sh_degree), float(scale_modifier), bool(raw), bool(antialiasing), filter_3d)
     try:
         return _RasterizePacked.apply(packed, means2D, int(P), int(sh_coeffs), cams)
     except InstanceLimitError:
@@ -686,7 +714,8 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
     outs = [rasterize_views_packed(packed, P, sh_coeffs, viewmatrices=viewmatrices[sl], projmatrices=projmatrices[sl], camposs=camposs[sl],
                                    tanfovx=list(tanfovx)[sl], tanfovy=list(tanfovy)[sl], image_height=image_height,
                                    image_width=image_width, bg=bg, sh_degree=sh_degree, means2D=means2D[sl],
-                                   scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing) for sl in (slice(0, h), slice(h, V))]
+                                   scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing, filter_3d=filter_3d)
+            for sl in (slice(0, h), slice(h, V))]
     return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
 
 
@@ -705,7 +734,7 @@ def forward_with_state(**kw):
         t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"), t("cov3D_precomp"),
         _f32c(kw["bg"], dev), _f32c(vm, dev).reshape(V, 4, 4), _f32c(pm, dev).reshape(V, 4, 4), _f32c(cp, dev).reshape(V, 3),
         tanx, tany, int(kw["image_height"]), int(kw["image_width"]), int(kw.get("sh_degree", 0)),
-        float(kw.get("scale_modifier", 1.0)), antialiasing=bool(kw.get("antialiasing", False)))
+        float(kw.get("scale_modifier", 1.0)), antialiasing=bool(kw.get("antialiasing", False)), filter_3d=kw.get("filter_3d"))
     sv = _StateView()
     _check(L.b200gs_describe_state(C.byref(st.prm), _ptr(st.geom), _ptr(st.binning), st.capacity, _ptr(st.image), C.byref(sv)),
            "describe_state")
@@ -759,6 +788,28 @@ def forward_backward_with_state(g_color, g_depth, g_alpha, **kw):
     nbytes = V * P * 48
     sums = st.scratch[:nbytes].view(torch.float32).reshape(V, P, 12).clone()
     return color, radii, depth, alpha, state, sums
+
+
+def sampling_rate(means3D: torch.Tensor, viewmatrices: torch.Tensor, tanfovx, tanfovy, image_height: int, image_width: int,
+                  max_rate: torch.Tensor) -> torch.Tensor:
+    """b200gs_sampling_rate: fold up to MAX_VIEWS cameras into max_rate [P] (in place, by max) and return it.
+    means3D [P,3]; viewmatrices [V,4,4]; tanfovx / tanfovy sequences of V floats."""
+    L = load_library()
+    dev = means3D.device
+    if dev.type != "cuda":
+        raise RuntimeError("b200gs: tensors must live on a CUDA device (there is no CPU path)")
+    V = viewmatrices.shape[0]
+    if V > MAX_VIEWS:
+        raise ValueError(f"b200gs: at most {MAX_VIEWS} cameras per sampling_rate call")
+    if max_rate.dtype != torch.float32 or max_rate.device != dev or not max_rate.is_contiguous() or max_rate.shape != (means3D.shape[0],):
+        raise ValueError("b200gs: max_rate must be a contiguous [P] float32 tensor on the means' device")
+    pts, vm = _f32c(means3D), _f32c(viewmatrices, dev)
+    tx = (C.c_float * V)(*[float(t) for t in tanfovx])
+    ty = (C.c_float * V)(*[float(t) for t in tanfovy])
+    with torch.cuda.device(dev):
+        _check(L.b200gs_sampling_rate(pts.shape[0], V, _ptr(pts), _ptr(vm), tx, ty, int(image_height), int(image_width),
+                                      _ptr(max_rate), _stream(dev)), "sampling_rate")
+    return max_rate
 
 
 def device_sort_pairs(keys: torch.Tensor, vals: torch.Tensor, nbits: int):

@@ -36,11 +36,13 @@ def _raw_tensors(pc):
     return None
 
 
-def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, fused_activations=False):
+def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, fused_activations=False, filter_3d=None):
     """fused_activations=True (optional fast path, SURVEY.md 8f-1): instead of calling the getters (sigmoid / exp /
     F.normalize: three kernels + autograd nodes per view, gaussian_model.py:95-118) the raw parameter tensors go straight
     to the rasteriser, which applies the activations and their Jacobians inside its kernels.  Same dict, same gradients
-    (they arrive at the raw tensors directly).  `pipe.antialiasing` (absent = False) turns on the screen-space mip filter."""
+    (they arrive at the raw tensors directly).  `pipe.antialiasing` (absent = False) turns on the screen-space mip filter.
+    filter_3d ([P] variances from filter3d.compute_filter_3d, or None): the 3D smoothing filter; the call then goes through
+    rasterize_views (GaussianRasterizer keeps upstream's surface, which has no such input)."""
     aa = bool(getattr(pipe, "antialiasing", False))
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
@@ -61,13 +63,24 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
     else:
         colors = override_color
     raw = _raw_tensors(pc) if fused_activations else None
+    if raw is None and filter_3d is not None:
+        image, radii, depth, alpha = rasterize_views(
+            means3D=xyz, opacities=pc.get_opacity, viewmatrices=viewpoint_camera.world_view_transform[None],
+            projmatrices=viewpoint_camera.full_proj_transform[None], camposs=viewpoint_camera.camera_center[None],
+            tanfovx=[settings.tanfovx], tanfovy=[settings.tanfovy], image_height=settings.image_height, image_width=settings.image_width,
+            bg=bg_color, sh_degree=pc.active_sh_degree, shs=shs, colors_precomp=colors, scales=pc.get_scaling,
+            rotations=pc.get_rotation, means2D=screenspace_points[None], scale_modifier=scaling_modifier, antialiasing=aa,
+            filter_3d=filter_3d)
+        image, radii, depth, alpha = image[0], radii[0], depth[0], alpha[0]
+        return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
+                "depth_3dgs": depth, "alpha_3dgs": alpha}
     if raw is not None:
         op, sc, rot = raw[0], raw[1], raw[2]
         image, radii, depth, alpha = rasterize_views(
             means3D=xyz, opacities=op, viewmatrices=viewpoint_camera.world_view_transform[None], projmatrices=viewpoint_camera.full_proj_transform[None],
             camposs=viewpoint_camera.camera_center[None], tanfovx=[settings.tanfovx], tanfovy=[settings.tanfovy], image_height=settings.image_height,
             image_width=settings.image_width, bg=bg_color, sh_degree=pc.active_sh_degree, shs=shs, colors_precomp=colors, scales=sc, rotations=rot,
-            means2D=screenspace_points[None], scale_modifier=scaling_modifier, raw=True, antialiasing=aa)
+            means2D=screenspace_points[None], scale_modifier=scaling_modifier, raw=True, antialiasing=aa, filter_3d=filter_3d)
         image, radii, depth, alpha = image[0], radii[0], depth[0], alpha[0]
         return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
                 "depth_3dgs": depth, "alpha_3dgs": alpha}
@@ -101,12 +114,12 @@ class _StackSinks(torch.autograd.Function):
         return (None, *g.unbind(0))
 
 
-def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False):
+def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False, filter_3d=None):
     """All cameras share image size.  Returns the dict of `render` with a leading view axis:
     render [V,3,H,W], depth_3dgs/alpha_3dgs [V,1,H,W], radii [V,P], viewspace_points [V,P,3] (its .grad is [V,P,3]),
     plus viewspace_point_list: V leaf tensors [P,3] whose .grad backward fills -- what the reference's
     `self.viewspace_point_list` holds (GaussianDreamer.py:242-250) and on_before_optimizer_step sums (:385-387).
-    antialiasing: the screen-space mip filter, as `rasterizer.rasterize_views`."""
+    antialiasing, filter_3d: the screen-space mip filter and the 3D smoothing filter, as `rasterizer.rasterize_views`."""
     xyz = pc.get_xyz
     V = len(cameras)
     vm, pm, cp, tanx, tany = stack_cameras(cameras, xyz.device)
@@ -121,6 +134,6 @@ def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False
         means3D=xyz, opacities=pc.get_opacity, viewmatrices=vm, projmatrices=pm, camposs=cp, tanfovx=tanx, tanfovy=tany,
         image_height=int(cameras[0].image_height), image_width=int(cameras[0].image_width), bg=bg_color,
         sh_degree=pc.active_sh_degree, shs=pc.get_features, scales=pc.get_scaling, rotations=pc.get_rotation,
-        means2D=screenspace_points, scale_modifier=scaling_modifier, antialiasing=antialiasing)
+        means2D=screenspace_points, scale_modifier=scaling_modifier, antialiasing=antialiasing, filter_3d=filter_3d)
     return {"render": image, "viewspace_points": screenspace_points, "viewspace_point_list": sinks, "visibility_filter": radii > 0,
             "radii": radii, "depth_3dgs": depth, "alpha_3dgs": alpha}

@@ -167,10 +167,18 @@ int b200gs_backward_deterministic(const b200gs_params *prm,
  *   antialiasing: 0 = off.  Non-zero = the screen-space mip filter: the covariance keeps its +0.3 px^2 dilation and the
  *     opacity is multiplied by rho = sqrt(det(S) / det(S + 0.3 I)), S the projected 2D covariance, floored at rho = 0.005,
  *     so that a Gaussian's integrated footprint does not depend on the pixel scale it is drawn at.  The backward then needs
- *     opacities (as for raw_params); dL_dopacity is w.r.t. the opacity before the filter. */
+ *     opacities (as for raw_params); dL_dopacity is w.r.t. the opacity before the filter.
+ *   filter3d_var: NULL = off.  Otherwise [P] device fp32 variances v >= 0 (finite; world length^2, e.g. from
+ *     b200gs_sampling_rate): the 3D smoothing filter.  Per Gaussian, before scale_modifier, the activated scales become
+ *     s'_i = sqrt(s_i^2 + v) and the opacity o * sqrt(prod_i s_i^2 / (s_i^2 + v)), so that its integrated 3D weight is kept;
+ *     the backward's dL_dscales / dL_dopacity are w.r.t. the unfiltered parameters, and v gets no gradient.  With
+ *     cov3D_precomp it is B200GS_E_ARGS; the backward needs opacities.  Only shape is checked, not the values (no sync).
+ *   struct_bytes: 8 (a header before filter3d_var) reads antialiasing only; >= 16 reads both; any other value is
+ *     B200GS_E_ARGS. */
 typedef struct b200gs_render_opts {
     int32_t struct_bytes;   /* sizeof(b200gs_render_opts) */
     int32_t antialiasing;   /* 0 | 1 */
+    const float *filter3d_var; /* [P] or NULL */
 } b200gs_render_opts;
 int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
                         const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
@@ -204,6 +212,16 @@ int b200gs_backward_deterministic_opts(const b200gs_params *prm, const b200gs_re
                                        float *dL_dscales, float *dL_drots, float *dL_dcov3D,
                                        void *scratch, size_t scratch_bytes,
                                        void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *stream);
+
+/* ---- 3D smoothing filter: per-Gaussian maximal sampling rate over a camera set (Mip-Splatting's 3D filter) ------------
+ * For each of the n_views cameras (viewmatrix [n_views,16] device, tanfovx / tanfovy host [n_views], shared H x W), with
+ * (tx, ty, tz) the preprocess's view-space position and fx = W / (2 tanfovx), fy = H / (2 tanfovy): Gaussian k is in view
+ * iff tz > 0.2, |tx / tz * fx| <= 0.65 W and |ty / tz * fy| <= 0.65 H (the image plus a 15 % margin per side; a NaN
+ * position is out).  Then max_rate[k] = max(max_rate[k], max(fx, fy) / tz) (in/out, device [P]).  The fold is a max, so
+ * any camera set passed in chunks of at most B200GS_MAX_VIEWS, in any order, gives the same bits.  The filter variance is
+ * then c / max_rate^2 (DESIGN.md section 2; humangaussian_b200.filter3d).  n_views > B200GS_MAX_VIEWS: B200GS_E_RANGE. */
+int b200gs_sampling_rate(int32_t P, int32_t n_views, const float *means3D, const float *viewmatrix, const float *tanfovx,
+                         const float *tanfovy, int32_t image_height, int32_t image_width, float *max_rate, void *stream);
 
 /* Frustum test only (upstream markVisible): present[i] = 1 if p_view.z > 0.2 for view 0.  positions [P,3]. */
 int b200gs_mark_visible(int32_t P, const float *positions, const float *viewmatrix, const float *projmatrix,
