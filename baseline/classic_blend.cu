@@ -172,6 +172,10 @@ int blend_sgrad_is_moments() { return 0; }
 // no deterministic backward here: b200gs_backward_deterministic returns B200GS_E_UNSUPPORTED before it would launch this
 int blend_bwd_has_deterministic() { return 0; }
 void launch_blend_bwd_det(const BlendBwdArgs &, const DetFlush &, cudaStream_t) {}
+// nor the absolute screen-space gradients: the absgrad entry points return B200GS_E_UNSUPPORTED before these would run
+int blend_bwd_has_absgrad() { return 0; }
+void launch_blend_bwd_abs(const BlendBwdArgs &, const DetFlush *, cudaStream_t) {}
+void launch_absgrad_out(int64_t, int, int, const int32_t *, const GeomRec *, const void *, float *, cudaStream_t) {}
 __global__ void classic_exp_kernel(const float *x, float *y, int64_t n)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

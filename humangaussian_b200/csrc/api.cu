@@ -249,7 +249,8 @@ size_t b200gs_deterministic_bytes(int64_t num_rendered, int64_t partial_capacity
     return DetLayout(num_rendered, partial_capacity, (int64_t)(P > 0 ? P : 0) * (V > 0 ? V : 0)).total;
 }
 
-// b200gs_backward (det == false) and b200gs_backward_deterministic (det == true)
+// b200gs_backward (det == false) and b200gs_backward_deterministic (det == true); dL_dmeans2D_abs != NULL: the absgrad forms
+// (abs_partials: the deterministic one's [partial_capacity] float2 array)
 static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs, const float *colors_precomp,
                          const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
                          const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
@@ -258,18 +259,25 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
                          const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
                          float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
                          size_t scratch_bytes, void *stream, bool det, void *det_buf, size_t det_bytes, int64_t partial_capacity,
-                         int64_t *n_partials)
+                         int64_t *n_partials, bool absgrad = false, float *dL_dmeans2D_abs = nullptr, void *abs_partials = nullptr,
+                         size_t abs_partials_bytes = 0)
 {
     bool aa = false;
     const float *f3d = nullptr;
+    if (absgrad && !blend_bwd_has_absgrad()) return B200GS_E_UNSUPPORTED;
     if (read_opts(opts, &aa, &f3d)) return B200GS_E_ARGS;
     if (f3d && cov3D_precomp) return B200GS_E_ARGS;
+    if (absgrad && !dL_dmeans2D_abs) return B200GS_E_ARGS;
     if (det) {
         if (!blend_bwd_has_deterministic()) return B200GS_E_UNSUPPORTED;
         if (!n_partials || !det_buf || partial_capacity < 0) return B200GS_E_ARGS;
         *n_partials = 0;
         if (num_rendered < 0 || num_rendered > instance_capacity || num_rendered > B200GS_MAX_INSTANCES) return B200GS_E_ARGS;
         if (((uintptr_t)det_buf) & 15) return B200GS_E_BUFFER;
+        if (absgrad) {
+            if (!abs_partials) return B200GS_E_ARGS;
+            if ((((uintptr_t)abs_partials) & 7) || abs_partials_bytes < (size_t)partial_capacity * sizeof(float2)) return B200GS_E_BUFFER;
+        }
     }
     int rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
@@ -305,7 +313,8 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     b.sgrad = scratch;
     if (!det) {
         StageTimer t(B200GS_STAGE_BLEND_BWD, st);
-        launch_blend_bwd(b, st);
+        if (absgrad) launch_blend_bwd_abs(b, nullptr, st);
+        else launch_blend_bwd(b, st);
     } else {
         // pre-pass -> (the one host wait: the partial count) -> B1 with per-partial stores -> fixed-order reduce.  The wait
         // sits after the scan so that a call whose partials do not fit returns before B1 runs; every access of the pre-pass
@@ -336,9 +345,19 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
         if (H_partials > 0xffffffffull) return B200GS_E_RANGE; // 32-bit slots; 160 GB of partials would not fit a device anyway
         if ((int64_t)H_partials > partial_capacity) return B200GS_E_BIN_TOO_SMALL;
         float *partials = (float *)(db + DL.partials);
-        if (H_partials > 0) launch_blend_bwd_det(b, DetFlush{pa.pm, pa.base, partials}, st);
-        launch_det_reduce(pa, n_vp, partials, scratch, st);
+        float2 *abs_p = absgrad ? (float2 *)abs_partials : nullptr;
+        const DetFlush flush{pa.pm, pa.base, partials, abs_p};
+        if (H_partials > 0) {
+            if (absgrad) launch_blend_bwd_abs(b, &flush, st);
+            else launch_blend_bwd_det(b, flush, st);
+        }
+        launch_det_reduce(pa, n_vp, partials, abs_p, scratch, st);
         g_launches += (H_partials > 0) + 1;
+    }
+    if (absgrad) {
+        StageTimer t(B200GS_STAGE_BLEND_BWD, st);
+        launch_absgrad_out(n_vp, H, W, radii, b.recs, scratch, dL_dmeans2D_abs, st);
+        g_launches += 1;
     }
 
     PreBwdArgs a;
@@ -420,6 +439,41 @@ int b200gs_backward_deterministic(const b200gs_params *prm, const float *means3D
                          campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
                          scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials);
+}
+
+int b200gs_backward_absgrad_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
+                                 const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
+                                 const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+                                 const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf,
+                                 int64_t instance_capacity, const void *image_buf, int64_t num_rendered, const float *dL_dcolor,
+                                 const float *dL_ddepth, const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
+                                 float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                 float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream)
+{
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr, true, dL_dmeans2D_abs);
+}
+
+int b200gs_backward_deterministic_absgrad_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D,
+                                               const float *shs, const float *colors_precomp, const float *opacities,
+                                               const float *scales, const float *rotations, const float *cov3D_precomp,
+                                               const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                               const int32_t *radii, const void *geom_buf, const void *binning_buf,
+                                               int64_t instance_capacity, const void *image_buf, int64_t num_rendered,
+                                               const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                               float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                                               float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                               float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *det_buf,
+                                               size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *abs_partials,
+                                               size_t abs_partials_bytes, void *stream)
+{
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials, true, dL_dmeans2D_abs,
+                         abs_partials, abs_partials_bytes);
 }
 
 int b200gs_sampling_rate(int32_t P, int32_t n_views, const float *means3D, const float *viewmatrix, const float *tanfovx,

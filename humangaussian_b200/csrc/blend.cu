@@ -35,6 +35,10 @@
 //   * Deterministic mode (torch.use_deterministic_algorithms): blend_bwd_det_kernel is the same body with a flush that stores
 //     each (instance, patch) partial into its own slot instead of the REDs; deterministic.cu plans the slots and adds each
 //     Gaussian's partials in a fixed order.  blend_bwd_kernel's SASS does not change.
+//   * Absolute screen-space gradients (densification statistic, DESIGN.md section 2): blend_bwd_abs_kernel and
+//     blend_bwd_det_abs_kernel are the same bodies with a flush that also sums |q (A dx + B dy)| and |q (B dx + C dy)| into
+//     ScreenGrad's padding (or a float2 per partial); absgrad_out_kernel scales them to dL_dmeans2D_abs.  The default
+//     kernels' SASS does not change.
 //   * The compile-time switches below are the A/B experiments DESIGN.md section 5 lists: the
 //     product is BWD_T_DIV=1 and BWD_PARK=16, everything else 0.
 #include "common.cuh"
@@ -424,20 +428,33 @@ __device__ __forceinline__ void red_add_v2(float *p, float a, float b)
 // scan of popc(pm)), and det_reduce_kernel adds each Gaussian's partials in a fixed order.
 // The tile's range.x and the warp's patch are re-derived here from the kernel parameters (two cached loads per flush), not
 // kept live across the hit loop: at the 64-register cap that costs the default kernel nothing and keeps this one from spilling.
-template <bool DET>
+// ABS (absolute screen-space gradients, DESIGN.md section 2): the flush also forms Ax = sum |q (A dx + B dy)| and
+// Ay = sum |q (B dx + C dy)| over the slot's pixels, with the record's conic (word 1, still in L1 from the hit loop's staging
+// load); B dy and C dy are folded once per row.  They go to ScreenGrad's padding (the third RED becomes a v4), or in
+// deterministic mode to the partial's own float2 of det.abs_partials.  The ten sums are formed exactly as without ABS.
+template <bool DET, bool ABS>
 __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, float fx0, float fy_part, float *sgrad,
                                            const BlendBwdArgs &a, const DetFlush &det)
 {
     __syncwarp();
     const int h = lane % BWD_PARK, part = lane / BWD_PARK;
     const float4 s = pk.hit[h];
+    float4 conic = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (ABS && h < n) conic = __ldg(reinterpret_cast<const float4 *>(a.recs) + 3 * (size_t)__float_as_uint(s.w) + 1);
     float dxk[8];
 #pragma unroll
     for (int k = 0; k < 8; k++) dxk[k] = fsub(s.x, fadd(fx0, (float)k));
     float S0 = 0.f, Sx = 0.f, Sy = 0.f, Sxx = 0.f, Sxy = 0.f, Syy = 0.f, W0 = 0.f, W1 = 0.f, W2 = 0.f, W3 = 0.f;
+    float Ax = 0.f, Ay = 0.f;
 #pragma unroll
     for (int r = 0; r < BWD_PARK / 8; r++) {
         const int p0 = BWD_PARK * part + 8 * r; // first pixel of the row
+        float Bdy = 0.f, Cdy = 0.f;
+        if (ABS) {
+            const float dy = fsub(s.y, fadd(fy_part, (float)r));
+            Bdy = conic.y * dy;
+            Cdy = conic.z * dy;
+        }
         float R0 = 0.f, Rx = 0.f, Rxx = 0.f;
 #pragma unroll
         for (int k = 0; k < 8; k++) {
@@ -448,6 +465,10 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
             Rx += qx;
             Rxx = fmaf(qx, dxk[k], Rxx);
             W0 = fmaf(v.y, g.x, W0); W1 = fmaf(v.y, g.y, W1); W2 = fmaf(v.y, g.z, W2); W3 = fmaf(v.y, g.w, W3);
+            if (ABS) {
+                Ax += fabsf(v.x * fmaf(conic.x, dxk[k], Bdy));
+                Ay += fabsf(v.x * fmaf(conic.y, dxk[k], Cdy));
+            }
         }
         const float dy = fsub(s.y, fadd(fy_part, (float)r));
         const float qy = R0 * dy;
@@ -461,6 +482,7 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
         Sxx += __shfl_xor_sync(FULL, Sxx, o); Sxy += __shfl_xor_sync(FULL, Sxy, o); Syy += __shfl_xor_sync(FULL, Syy, o);
         W0 += __shfl_xor_sync(FULL, W0, o); W1 += __shfl_xor_sync(FULL, W1, o); W2 += __shfl_xor_sync(FULL, W2, o);
         W3 += __shfl_xor_sync(FULL, W3, o);
+        if (ABS) { Ax += __shfl_xor_sync(FULL, Ax, o); Ay += __shfl_xor_sync(FULL, Ay, o); }
     }
     if (DET) {
         if (h < n) {
@@ -472,23 +494,29 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
             float2 *rec = reinterpret_cast<float2 *>(det.partials + (size_t)slot * DET_PARTIAL_FLOATS);
             if (part == 0) { rec[0] = make_float2(S0, Sx); rec[1] = make_float2(Sy, Sxx); }
             if (part == 1) { rec[2] = make_float2(Sxy, Syy); rec[3] = make_float2(W0, W1); }
-            if (part == (PARK_LANES > 2 ? 2 : 0)) rec[4] = make_float2(W2, W3);
+            if (part == (PARK_LANES > 2 ? 2 : 0)) {
+                rec[4] = make_float2(W2, W3);
+                if (ABS) det.abs_partials[slot] = make_float2(Ax, Ay);
+            }
         }
     } else if (h < n) {
-        // ScreenGrad as moments: S0, Sx, Sy, Sxx | Sxy, Syy, w.gC0, w.gC1 | w.gC2, w.gD
+        // ScreenGrad as moments: S0, Sx, Sy, Sxx | Sxy, Syy, w.gC0, w.gC1 | w.gC2, w.gD (| Ax, Ay in the padding with ABS)
         float *rec = sgrad + (size_t)__float_as_uint(s.w) * (sizeof(ScreenGrad) / sizeof(float));
         if (part < 2) {
             const bool hi = part == 1;
             red_add_v4(rec + (hi ? 4 : 0), hi ? Sxy : S0, hi ? Syy : Sx, hi ? W0 : Sy, hi ? W1 : Sxx);
         }
-        if (part == (PARK_LANES > 2 ? 2 : 0)) red_add_v2(rec + 8, W2, W3);
+        if (part == (PARK_LANES > 2 ? 2 : 0)) {
+            if (ABS) red_add_v4(rec + 8, W2, W3, Ax, Ay);
+            else red_add_v2(rec + 8, W2, W3);
+        }
     }
     __syncwarp();
 }
 
-// The body of both B1 kernels: DET selects the flush (vector REDs into ScreenGrad, or stores of per-(instance, patch)
-// partials); everything else is the same code.
-template <bool DET>
+// The body of the B1 kernels: DET selects the flush (vector REDs into ScreenGrad, or stores of per-(instance, patch)
+// partials), ABS adds the absolute sums to it; everything else is the same code.
+template <bool DET, bool ABS>
 __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetFlush &det)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
@@ -617,24 +645,36 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
                 if (lane == 0) pk.hit[np] = g0;
             }
             if (np == BWD_PARK) {
-                park_flush<DET>(pk, np, lane, fx0, fy_part, sgrad, a, det);
+                park_flush<DET, ABS>(pk, np, lane, fx0, fy_part, sgrad, a, det);
                 np = 0;
             }
         }
         __syncwarp();
     }
-    if (np > 0) park_flush<DET>(pk, np, lane, fx0, fy_part, sgrad, a, det);
+    if (np > 0) park_flush<DET, ABS>(pk, np, lane, fx0, fy_part, sgrad, a, det);
 }
 
 __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_kernel(BlendBwdArgs a)
 {
-    blend_bwd_body<false>(a, DetFlush{});
+    blend_bwd_body<false, false>(a, DetFlush{});
 }
 
 // B1 of the deterministic backward: a.sgrad is not touched; every flushed (instance, patch) partial goes to its own slot
 __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_kernel(BlendBwdArgs a, DetFlush det)
 {
-    blend_bwd_body<true>(a, det);
+    blend_bwd_body<true, false>(a, det);
+}
+
+// B1 with the absolute screen-space sums (Ax, Ay in ScreenGrad's padding)
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_abs_kernel(BlendBwdArgs a)
+{
+    blend_bwd_body<false, true>(a, DetFlush{});
+}
+
+// deterministic B1 with the absolute sums: (Ax, Ay) of partial `slot` go to det.abs_partials[slot]
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_abs_kernel(BlendBwdArgs a, DetFlush det)
+{
+    blend_bwd_body<true, true>(a, det);
 }
 
 void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st)
@@ -648,6 +688,37 @@ void launch_blend_bwd_det(const BlendBwdArgs &a, const DetFlush &det, cudaStream
 {
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
     blend_bwd_det_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, det);
+}
+
+int blend_bwd_has_absgrad() { return 1; }
+void launch_blend_bwd_abs(const BlendBwdArgs &a, const DetFlush *det, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
+    if (det) blend_bwd_det_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det);
+    else blend_bwd_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
+}
+
+// dL_dmeans2D_abs of every (view, Gaussian): the padding sums (Ax, Ay) times o * W/2 and o * H/2, o the record's opacity --
+// the factors B2 applies to the signed moments (preprocess.cu), both positive.  Zero where radii == 0.
+__global__ void __launch_bounds__(256) absgrad_out_kernel(int64_t n_vp, int H, int W, const int32_t *__restrict__ radii,
+                                                          const GeomRec *__restrict__ recs, const ScreenGrad *__restrict__ sgrad,
+                                                          float *__restrict__ out)
+{
+    const int64_t vp = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (vp >= n_vp) return;
+    float gx = 0.f, gy = 0.f;
+    if (radii[vp] > 0) {
+        const float o = recs[vp].o;
+        const float2 s = *reinterpret_cast<const float2 *>(&sgrad[vp].pad0);
+        gx = o * s.x * (0.5f * (float)W);
+        gy = o * s.y * (0.5f * (float)H);
+    }
+    out[3 * vp] = gx; out[3 * vp + 1] = gy; out[3 * vp + 2] = 0.f;
+}
+void launch_absgrad_out(int64_t n_vp, int H, int W, const int32_t *radii, const GeomRec *recs, const void *sgrad, float *out,
+                        cudaStream_t st)
+{
+    absgrad_out_kernel<<<(unsigned)((n_vp + 255) / 256), 256, 0, st>>>(n_vp, H, W, radii, recs, (const ScreenGrad *)sgrad, out);
 }
 
 // ScreenGrad holds moments of q = G*dL/dalpha here: S0, Sx, Sy, Sxx, Sxy, Syy = sum q*{1, dx, dy, dx^2, dx*dy, dy^2};

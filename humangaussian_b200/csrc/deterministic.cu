@@ -9,7 +9,8 @@
 //                               jpos[start[vp] + (ty - y0) * w + (tx - x0)] = j
 //             lookback_scan     base = inclusive scan of popc(pm), exact 64-bit total H (radix.cuh, via binning.cu)
 //   reduce:   det_reduce_kernel one thread per (view, Gaussian): walks its emission range, writes the whole ScreenGrad
-//                               record (padding zero), so the default path's scratch memset is not needed
+//                               record (padding zero, or the absolute sums (Ax, Ay) with absgrad), so the default path's
+//                               scratch memset is not needed
 #include "common.cuh"
 #include "kernels.h"
 
@@ -84,8 +85,10 @@ __global__ void __launch_bounds__(256) det_plan_kernel(const DetPlanArgs a)
 
 // One thread per (view, Gaussian), taken in depth order k: vp = order[k] owns the emission indices
 // [offsets[k] - tiles_touched[vp], offsets[k]).
+// ABS: also adds the partials' (Ax, Ay) from abs_partials, same order, into the record's padding.
+template <bool ABS>
 __global__ void __launch_bounds__(256) det_reduce_kernel(const DetPlanArgs a, int64_t n_vp, const float *__restrict__ partials,
-                                                          float *__restrict__ sgrad)
+                                                          float *__restrict__ sgrad, const float2 *__restrict__ abs_partials)
 {
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_vp) return;
@@ -94,6 +97,7 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const DetPlanArgs a, in
     float s[DET_PARTIAL_FLOATS];
 #pragma unroll
     for (int i = 0; i < DET_PARTIAL_FLOATS; i++) s[i] = 0.0f;
+    float ax = 0.0f, ay = 0.0f;
     for (uint32_t e = e0; e != e0 + n; e++) {
         const uint32_t j = __ldg(a.jpos + e);
         const uint32_t np = (uint32_t)__popc((uint32_t)__ldg(a.pm + j));
@@ -106,12 +110,17 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const DetPlanArgs a, in
                 s[2 * i] = fadd(s[2 * i], x.x);
                 s[2 * i + 1] = fadd(s[2 * i + 1], x.y);
             }
+            if (ABS) {
+                const float2 x = __ldg(abs_partials + q);
+                ax = fadd(ax, x.x);
+                ay = fadd(ay, x.y);
+            }
         }
     }
     float4 *dst = reinterpret_cast<float4 *>(sgrad + (size_t)vp * (sizeof(ScreenGrad) / sizeof(float)));
     dst[0] = make_float4(s[0], s[1], s[2], s[3]);
     dst[1] = make_float4(s[4], s[5], s[6], s[7]);
-    dst[2] = make_float4(s[8], s[9], 0.0f, 0.0f);
+    dst[2] = make_float4(s[8], s[9], ax, ay);
 }
 
 int launch_det_plan(const DetPlanArgs &a, int64_t n_vp, int n_tiles_all, const DetLayout &L, char *det_base, cudaStream_t st,
@@ -123,7 +132,10 @@ int launch_det_plan(const DetPlanArgs &a, int64_t n_vp, int n_tiles_all, const D
     return launch_popc_scan(a.pm, a.base, a.D, det_base + L.scan_temp, (uint64_t *)(det_base + L.total_slot), st);
 }
 
-void launch_det_reduce(const DetPlanArgs &a, int64_t n_vp, const float *partials, void *sgrad, cudaStream_t st)
+void launch_det_reduce(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
+                       cudaStream_t st)
 {
-    det_reduce_kernel<<<(unsigned)((n_vp + 255) / 256), 256, 0, st>>>(a, n_vp, partials, (float *)sgrad);
+    const unsigned grid = (unsigned)((n_vp + 255) / 256);
+    if (abs_partials) det_reduce_kernel<true><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, abs_partials);
+    else det_reduce_kernel<false><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, nullptr);
 }

@@ -116,6 +116,7 @@ struct DetFlush {
     const uint8_t *pm;    // [D] bit p: B1 flushes a partial for (j, patch p)
     const uint32_t *base; // [D] inclusive scan of popc(pm) (exact: the total is checked to fit 32 bits)
     float *partials;      // [H][DET_PARTIAL_FLOATS]
+    float2 *abs_partials; // [H] (Ax, Ay) of each partial: written by the absgrad instantiation only
 };
 // det_buf carving; pm first (b200gs.h documents that the buffer starts with it)
 struct DetLayout {
@@ -143,7 +144,15 @@ void launch_blend_bwd_det(const BlendBwdArgs &a, const DetFlush &det, cudaStream
 // start scatter, plan, scan of popc(pm) -> base and the exact 64-bit partial count at *total_dev
 int launch_det_plan(const DetPlanArgs &a, int64_t n_vp, int n_tiles_all, const DetLayout &L, char *det_base, cudaStream_t st,
                     int *n_launches);
-void launch_det_reduce(const DetPlanArgs &a, int64_t n_vp, const float *partials, void *sgrad, cudaStream_t st);
+// abs_partials (NULL: none): their (Ax, Ay) are added in the same order into ScreenGrad's padding, which is zero without them
+void launch_det_reduce(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
+                       cudaStream_t st);
+// absolute screen-space gradients (DESIGN.md section 2): B1 with Ax, Ay in ScreenGrad's padding -- atomic (det NULL) or
+// deterministic -- and the pass that writes dL_dmeans2D_abs [V,P,3] from them.  0 in the classic comparator.
+int blend_bwd_has_absgrad();
+void launch_blend_bwd_abs(const BlendBwdArgs &a, const DetFlush *det, cudaStream_t st);
+void launch_absgrad_out(int64_t n_vp, int H, int W, const int32_t *radii, const GeomRec *recs, const void *sgrad, float *out,
+                        cudaStream_t st);
 void launch_test_exp(const float *x, float *y, int64_t n, cudaStream_t st);
 
 // animation frame path (anim.cu)

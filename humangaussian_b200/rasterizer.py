@@ -91,7 +91,8 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_knn_scratch_bytes", "b200gs_dist2_knn3", "b200gs_densify_stats", "b200gs_densify_scratch_bytes",
            "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed", "b200gs_deterministic_bytes",
            "b200gs_backward_deterministic", "b200gs_forward_opts", "b200gs_backward_opts",
-           "b200gs_backward_deterministic_opts", "b200gs_sampling_rate"]
+           "b200gs_backward_deterministic_opts", "b200gs_sampling_rate", "b200gs_backward_absgrad_opts",
+           "b200gs_backward_deterministic_absgrad_opts"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -128,6 +129,13 @@ def load_library():
     L.b200gs_backward_deterministic_opts.restype = C.c_int
     L.b200gs_backward_deterministic_opts.argtypes = ([L.b200gs_backward_deterministic.argtypes[0], vp] +
                                                      L.b200gs_backward_deterministic.argtypes[1:])
+    # the absgrad forms: the *_opts argument lists with dL_dmeans2D_abs after dL_dcov3D (and abs_partials after n_partials)
+    bo = L.b200gs_backward_opts.argtypes
+    L.b200gs_backward_absgrad_opts.restype = C.c_int
+    L.b200gs_backward_absgrad_opts.argtypes = bo[:30] + [vp] + bo[30:]
+    bdo = L.b200gs_backward_deterministic_opts.argtypes
+    L.b200gs_backward_deterministic_absgrad_opts.restype = C.c_int
+    L.b200gs_backward_deterministic_absgrad_opts.argtypes = bdo[:30] + [vp] + bdo[30:36] + [vp, sz] + bdo[36:]
     L.b200gs_sampling_rate.restype = C.c_int
     L.b200gs_sampling_rate.argtypes = [i32, i32, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float), i32, i32, vp, vp]
     L.b200gs_mark_visible.restype = C.c_int
@@ -391,9 +399,10 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     return color, radii, depth, alpha, st
 
 
-def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None):
+def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_abs=None):
     """b200gs_backward_deterministic with the work buffer from _det_pool, sized by the partial-capacity hint; a call whose
-    partials do not fit is repeated with room for the count it reported (at most two retries)."""
+    partials do not fit is repeated with room for the count it reported (at most two retries).  d_means2D_abs: the absgrad
+    form, with its float2-per-partial array pooled beside the work buffer."""
     P, V, H, W = st.P, st.V, st.H, st.W
     key = (dev.index, P, V, H, W)
     pcap = _partial_hint.get(key, max(1 << 16, 2 * st.num_rendered))
@@ -401,12 +410,20 @@ def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None):
     stream = torch.cuda.current_stream(dev).cuda_stream
     for _ in range(3):
         # sized for the forward's instance capacity (>= its count), so the pool key stays the same from call to call
-        pkey = (dev.index, stream, st.capacity, pcap, P, V)
+        pkey = (dev.index, stream, st.capacity, pcap, P, V, d_means2D_abs is not None)
         bufs = _det_pool.take(pkey)
         if bufs is None:
             bufs = dict(det=torch.empty(L.b200gs_deterministic_bytes(st.capacity, pcap, P, V), dtype=torch.uint8, device=dev))
+            if d_means2D_abs is not None:
+                bufs["abs"] = torch.empty(max(8 * pcap, 16), dtype=torch.uint8, device=dev)
         det = bufs["det"]
-        if st.opts is not None:
+        if d_means2D_abs is not None:
+            ab = bufs["abs"]
+            opts = C.byref(st.opts) if st.opts is not None else None
+            rc = L.b200gs_backward_deterministic_absgrad_opts(args[0], opts, *args[1:29], _ptr(d_means2D_abs), *args[29:], _ptr(det),
+                                                              det.numel(), pcap, C.byref(n_out), _ptr(ab), ab.numel(),
+                                                              C.c_void_p(stream))
+        elif st.opts is not None:
             rc = L.b200gs_backward_deterministic_opts(args[0], C.byref(st.opts), *args[1:], _ptr(det), det.numel(), pcap,
                                                       C.byref(n_out), C.c_void_p(stream))
         else:
@@ -426,9 +443,12 @@ def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None):
 
 
 def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
-                   projmatrix, campos, g_color, g_depth, g_alpha, out=None, det_state=None):
+                   projmatrix, campos, g_color, g_depth, g_alpha, out=None, det_state=None, absgrad=False):
     """`out` (optional): dict of preallocated contiguous fp32 gradient buffers by name (means3D, sh, opacity, scales,
     rotations) -- the packed entry points them into one flat buffer so that B3 writes the all-reduce payload in place.
+
+    absgrad=True: the absgrad entry points run, and a ninth value is returned: dL_dmeans2D_abs [V,P,3], the per-pixel terms
+    of dL_dmeans2D summed in absolute value (include/b200gs.h).  Every other gradient is what absgrad=False gives.
 
     Under torch.use_deterministic_algorithms(True) the backward is the library's deterministic one: the same gradients up
     to float rounding, bit-identical from run to run (one host wait per call, for its partial count).  `det_state`
@@ -447,8 +467,10 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
     d_sc = (out.get("scales") if "scales" in out else torch.empty(P, 3, **f)) if scales is not None else None
     d_rot = (out.get("rotations") if "rotations" in out else torch.empty(P, 4, **f)) if rotations is not None else None
     d_cov = torch.empty(P, 6, **f) if cov3D_precomp is not None else None
+    d_abs = torch.empty(V, P, 3, **f) if absgrad else None
+    grads = (d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov) + ((d_abs,) if absgrad else ())
     if P == 0:
-        return d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov
+        return grads
     scratch = st.scratch
     args = (C.byref(st.prm), _ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities), _ptr(scales), _ptr(rotations),
             _ptr(cov3D_precomp), _ptr(bg), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), _ptr(st.radii), _ptr(st.geom),
@@ -457,13 +479,16 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
             _ptr(scratch), scratch.numel())
     with torch.cuda.device(dev):
         if torch.are_deterministic_algorithms_enabled():
-            rc = _backward_deterministic(L, st, dev, args, det_state)
+            rc = _backward_deterministic(L, st, dev, args, det_state, d_abs)
+        elif absgrad:
+            rc = L.b200gs_backward_absgrad_opts(args[0], C.byref(st.opts) if st.opts is not None else None, *args[1:29], _ptr(d_abs),
+                                                *args[29:], _stream(dev))
         elif st.opts is not None:  # the backward gets the options its forward got
             rc = L.b200gs_backward_opts(args[0], C.byref(st.opts), *args[1:], _stream(dev))
         else:
             rc = L.b200gs_backward(*args, _stream(dev))
     _check(rc, "backward")
-    return d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov
+    return grads
 
 
 def _save(ctx, tensors):
@@ -482,7 +507,8 @@ class _RasterizeViews(torch.autograd.Function):
     """V >= 1 views of one Gaussian set.  means2D is [V,P,3] (or [P,3] when V == 1 and squeeze=True)."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, squeeze):
+    def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, squeeze,
+                means2D_abs=None):
         bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, prefiltered, debug = cams[:12]
         raw = bool(cams[12]) if len(cams) > 12 else False
         aa = bool(cams[13]) if len(cams) > 13 else False
@@ -491,7 +517,7 @@ class _RasterizeViews(torch.autograd.Function):
         args = [_f32c(t, dev) for t in (means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)]
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
         color, radii, depth, alpha, st = _forward_impl(*args, *camt, tanx, tany, H, W, deg, mod, prefiltered, debug, raw, aa, f3d)
-        ctx.st, ctx.squeeze = st, squeeze
+        ctx.st, ctx.squeeze, ctx.absgrad = st, squeeze, means2D_abs is not None
         _save(ctx, args + camt)
         ctx.in_shapes = [None if t is None else t.shape for t in (means3D, means2D, shs, colors_precomp, opacities, scales,
                                                                   rotations, cov3D_precomp)]
@@ -506,14 +532,15 @@ class _RasterizeViews(torch.autograd.Function):
         means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix, campos = _saved(ctx)
         dev = means3D.device
         g = [None if t is None else _f32c(t, dev) for t in (g_color, g_depth, g_alpha)]
-        d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov = _backward_impl(
-            st, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix, campos, *g)
+        d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov, *d_abs = _backward_impl(
+            st, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix, campos, *g,
+            absgrad=ctx.absgrad)
         if ctx.squeeze:
             d_means2D = d_means2D[0]
         # gradients take the shape the caller passed (e.g. opacities [P] or [P,1])
         grads = [g if (g is None or shp is None) else g.reshape(shp)
                  for g, shp in zip((d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov), ctx.in_shapes)]
-        return (*grads, None, None)
+        return (*grads, None, None, d_abs[0] if d_abs else None)
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -576,8 +603,14 @@ class GaussianRasterizer(nn.Module):
 
 def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, tanfovx, tanfovy, image_height, image_width,
                     bg, sh_degree=0, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
-                    means2D=None, scale_modifier=1.0, raw=False, antialiasing=False, filter_3d=None):
+                    means2D=None, scale_modifier=1.0, raw=False, antialiasing=False, filter_3d=None, means2D_abs=None):
     """Render V cameras of one Gaussian set in ONE call (one preprocess/sort/blend launch set, one host sync).
+
+    means2D_abs: None, or a [V,P,3] fp32 gradient sink like means2D (zeros, requires_grad): the backward then fills its
+    .grad with the absolute screen-space gradient -- per (view, Gaussian) the per-pixel terms of means2D's gradient summed
+    in absolute value per component (x, y; z = 0), which does not cancel where a Gaussian's pixels pull it in opposite
+    directions (DESIGN.md section 2).  Feed it to densify.add_densification_stats in place of means2D.grad.  Every other
+    output and gradient is unchanged.
 
     filter_3d: [P] fp32 variances of the 3D smoothing filter (`filter3d.compute_filter_3d`), or None: each Gaussian's
     activated scales become sqrt(s^2 + v) and its opacity is scaled to keep its integrated 3D weight, inside the kernels
@@ -603,7 +636,8 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                                 image_width=image_width, bg=bg, sh_degree=sh_degree, shs=shs, colors_precomp=colors_precomp,
                                 scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
                                 means2D=None if means2D is None else means2D[i:i + MAX_VIEWS], scale_modifier=scale_modifier, raw=raw,
-                                antialiasing=antialiasing, filter_3d=filter_3d)
+                                antialiasing=antialiasing, filter_3d=filter_3d,
+                                means2D_abs=None if means2D_abs is None else means2D_abs[i:i + MAX_VIEWS])
                 for i in range(0, V, MAX_VIEWS)]
         return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
     _check_filter_3d(filter_3d, means3D.shape[-2], means3D.device, cov3D_precomp)
@@ -612,7 +646,8 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
     cams = (bg, viewmatrices, projmatrices, camposs, list(tanfovx), list(tanfovy), int(image_height), int(image_width),
             int(sh_degree), float(scale_modifier), False, False, bool(raw), bool(antialiasing), filter_3d)
     try:
-        return _RasterizeViews.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, False)
+        return _RasterizeViews.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, False,
+                                     means2D_abs)
     except InstanceLimitError:
         if V == 1:
             raise
@@ -623,7 +658,7 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                             image_height=image_height, image_width=image_width, bg=bg, sh_degree=sh_degree, shs=shs,
                             colors_precomp=colors_precomp, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
                             means2D=means2D[sl], scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing,
-                            filter_3d=filter_3d)
+                            filter_3d=filter_3d, means2D_abs=None if means2D_abs is None else means2D_abs[sl])
             for sl in (slice(0, h), slice(h, V))]
     return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
 
@@ -654,14 +689,14 @@ def _split_packed(flat: torch.Tensor, P: int, M: int):
 
 class _RasterizePacked(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, packed, means2D, P, M, cams):
+    def forward(ctx, packed, means2D, P, M, cams, means2D_abs=None):
         bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, raw, aa, f3d = cams
         dev = packed.device
         xyz, sc, rot, op, sh = _split_packed(packed.detach(), P, M)
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
         color, radii, depth, alpha, st = _forward_impl(xyz, sh, None, op, sc, rot, None, *camt, tanx, tany, H, W, deg, mod, raw=raw,
                                                        antialiasing=aa, filter_3d=f3d)
-        ctx.st, ctx.P, ctx.M = st, P, M
+        ctx.st, ctx.P, ctx.M, ctx.absgrad = st, P, M, means2D_abs is not None
         ctx.save_for_backward(packed, *camt)
         ctx.mark_non_differentiable(radii)
         return color, radii, depth, alpha
@@ -675,21 +710,22 @@ class _RasterizePacked(torch.autograd.Function):
         d_packed = torch.empty_like(packed) if P % 4 == 0 else torch.zeros_like(packed)  # alignment padding carries zero gradient
         d_xyz, d_sc, d_rot, d_op, d_sh = _split_packed(d_packed, P, M)
         g = [None if t is None else _f32c(t, dev) for t in (g_color, g_depth, g_alpha)]
-        _, d_means2D, *_ = _backward_impl(ctx.st, xyz, sh, None, op, sc, rot, None, bg, viewmatrix, projmatrix, campos, *g,
-                                          out=dict(means3D=d_xyz, sh=d_sh, opacity=d_op, scales=d_sc, rotations=d_rot))
-        return d_packed, d_means2D, None, None, None
+        _, d_means2D, *rest = _backward_impl(ctx.st, xyz, sh, None, op, sc, rot, None, bg, viewmatrix, projmatrix, campos, *g,
+                                             out=dict(means3D=d_xyz, sh=d_sh, opacity=d_op, scales=d_sc, rotations=d_rot),
+                                             absgrad=ctx.absgrad)
+        return d_packed, d_means2D, None, None, None, rest[6] if ctx.absgrad else None
 
 
 def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, viewmatrices, projmatrices, camposs, tanfovx, tanfovy,
                            image_height, image_width, bg, sh_degree=0, means2D=None, scale_modifier=1.0, raw=False, antialiasing=False,
-                           filter_3d=None):
+                           filter_3d=None, means2D_abs=None):
     """`rasterize_views` over ONE flat fp32 buffer [xyz 3P | scales 3P | rotations 4P | opacities P | shs 3*K*P], each
     field starting on a 16-byte boundary (`packed_layout`; what `dist.pack` produces, broadcast once per parameter
     version).  raw=False: post-activation values, as the rasteriser's classic inputs.  raw=True: the buffer holds the
     optimiser's RAW parameters (log-scales, un-normalised quaternions, opacity logits; SH = cat(f_dc, f_rest)); the
     activations of gaussian_model.py:95-118 and their Jacobians run inside the kernels, so `packed.grad` is the gradient
     of the raw parameters and a training step needs no activation kernels, no pack copy and no autograd nodes besides
-    this one.  antialiasing, filter_3d: as `rasterize_views`.  The backward
+    this one.  antialiasing, filter_3d, means2D_abs: as `rasterize_views`.  The backward
     kernels write the parameter gradients straight into one buffer of the same layout, which becomes `packed.grad`
     as is: no per-tensor gradient accumulation, and on several GPUs that buffer is the all-reduce payload in place.
     V <= MAX_VIEWS.  Returns color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W]."""
@@ -706,7 +742,7 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
     cams = (bg, viewmatrices, projmatrices, camposs, list(tanfovx), list(tanfovy), int(image_height), int(image_width),
             int(sh_degree), float(scale_modifier), bool(raw), bool(antialiasing), filter_3d)
     try:
-        return _RasterizePacked.apply(packed, means2D, int(P), int(sh_coeffs), cams)
+        return _RasterizePacked.apply(packed, means2D, int(P), int(sh_coeffs), cams, means2D_abs)
     except InstanceLimitError:
         if V == 1:
             raise
@@ -714,7 +750,8 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
     outs = [rasterize_views_packed(packed, P, sh_coeffs, viewmatrices=viewmatrices[sl], projmatrices=projmatrices[sl], camposs=camposs[sl],
                                    tanfovx=list(tanfovx)[sl], tanfovy=list(tanfovy)[sl], image_height=image_height,
                                    image_width=image_width, bg=bg, sh_degree=sh_degree, means2D=means2D[sl],
-                                   scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing, filter_3d=filter_3d)
+                                   scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing, filter_3d=filter_3d,
+                                   means2D_abs=None if means2D_abs is None else means2D_abs[sl])
             for sl in (slice(0, h), slice(h, V))]
     return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
 

@@ -213,6 +213,44 @@ int b200gs_backward_deterministic_opts(const b200gs_params *prm, const b200gs_re
                                        void *scratch, size_t scratch_bytes,
                                        void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *stream);
 
+/* ---- absolute screen-space gradients for densification (additive to ABI 4) ------------------------------------------
+ * The absgrad forms take the argument list of b200gs_backward_opts / b200gs_backward_deterministic_opts with one more output
+ * after dL_dcov3D, and compute every other output exactly as those calls do.
+ *   dL_dmeans2D_abs [V,P,3] (device, overwritten; NULL is B200GS_E_ARGS): per (view, Gaussian), the per-pixel terms of
+ *     dL_dmeans2D summed in absolute value per component: ( sum_p |g_p.x|, sum_p |g_p.y|, 0 ), NDC units like dL_dmeans2D,
+ *     where g_p = dL_p / dmean2D is pixel p's term of the signed gradient.  The signed sum cancels where a Gaussian's pixels
+ *     pull its centre in opposite directions; this one does not (the "absgrad" / homodirectional densification statistic).
+ *     Zero where radii == 0.  b200gs_densify_stats accepts it in place of dL_dmeans2D.
+ *   abs_partials (deterministic form only): a caller-owned device array of abs_partials_bytes >= 8 * partial_capacity bytes,
+ *     8-byte aligned (else B200GS_E_BUFFER; NULL is B200GS_E_ARGS): one float2 per partial, at the partial's slot.  It is
+ *     separate from det_buf, whose layout and size (b200gs_deterministic_bytes) do not change.  The absolute sums are then
+ *     bit-reproducible like every other output.
+ * The classic comparator build returns B200GS_E_UNSUPPORTED. */
+int b200gs_backward_absgrad_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                                 const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                                 const float *scales, const float *rotations, const float *cov3D_precomp,
+                                 const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                 const int32_t *radii,
+                                 const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                 const void *image_buf, int64_t num_rendered,
+                                 const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                 float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+                                 float *dL_dscales, float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs,
+                                 void *scratch, size_t scratch_bytes, void *stream);
+int b200gs_backward_deterministic_absgrad_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                                               const float *means3D, const float *shs, const float *colors_precomp,
+                                               const float *opacities, const float *scales, const float *rotations,
+                                               const float *cov3D_precomp, const float *bg, const float *viewmatrix,
+                                               const float *projmatrix, const float *campos, const int32_t *radii,
+                                               const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                               const void *image_buf, int64_t num_rendered,
+                                               const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                               float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                                               float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                               float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes,
+                                               void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials,
+                                               void *abs_partials, size_t abs_partials_bytes, void *stream);
+
 /* ---- 3D smoothing filter: per-Gaussian maximal sampling rate over a camera set (Mip-Splatting's 3D filter) ------------
  * For each of the n_views cameras (viewmatrix [n_views,16] device, tanfovx / tanfovy host [n_views], shared H x W), with
  * (tx, ty, tz) the preprocess's view-space position and fx = W / (2 tanfovx), fy = H / (2 tanfovy): Gaussian k is in view
