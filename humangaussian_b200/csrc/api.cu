@@ -115,12 +115,13 @@ static int read_opts(const b200gs_render_opts *o, bool *aa, const float **f3d)
     return B200GS_OK;
 }
 
-int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
+// b200gs_forward_opts (contrib NULL) and b200gs_forward_contrib_opts (the blend with the contribution scores)
+static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
                         const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
                         const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
                         const float *campos, float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf,
                         size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf,
-                        size_t image_bytes, int64_t *num_rendered, void *stream)
+                        size_t image_bytes, int64_t *num_rendered, void *stream, const ContribOut *contrib)
 {
     bool aa = false;
     const float *f3d = nullptr;
@@ -180,7 +181,8 @@ int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts
         CK(cudaMemcpyAsync(hs->total, total_dev, 8, cudaMemcpyDeviceToHost, st), "D2H num_rendered");
         int64_t cap = instance_capacity < B200GS_MAX_INSTANCES ? instance_capacity : (int64_t)B200GS_MAX_INSTANCES;
         if (cap < 1) cap = 1; // the layout always has room for one instance
-        if (n_vp <= B200GS_DEFERRED_MAX_NVP) {
+        // (the contribution scores are accumulators: a call that does not fit must not reach the blend, so it always waits)
+        if (n_vp <= B200GS_DEFERRED_MAX_NVP && !contrib) {
             // Small batches (the per-view drop-in pattern, the 8-view SDS batch): the host does NOT wait here.  Emit / tile
             // sort / ranges / blend are enqueued sized for the caller's capacity and read the count on the device, so the GPU
             // never idles behind a host round trip (upstream blocks on this read-back in the middle of every forward).  The
@@ -218,7 +220,8 @@ int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts
     (void)HW;
     {
         StageTimer t(B200GS_STAGE_BLEND_FWD, st);
-        launch_blend_fwd(b, st);
+        if (contrib) launch_blend_fwd_contrib(b, *contrib, st);
+        else launch_blend_fwd(b, st);
         g_launches += 1;
     }
     CK(cudaGetLastError(), "forward launch");
@@ -230,6 +233,34 @@ int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts
         if ((int64_t)total > instance_capacity) return B200GS_E_BIN_TOO_SMALL;
     }
     return B200GS_OK;
+}
+
+int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
+                        const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
+                        const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+                        const float *campos, float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf,
+                        size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf,
+                        size_t image_bytes, int64_t *num_rendered, void *stream)
+{
+    return forward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
+                        projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
+                        instance_capacity, image_buf, image_bytes, num_rendered, stream, nullptr);
+}
+
+int b200gs_forward_contrib_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
+                                const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
+                                const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+                                const float *campos, float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
+                                void *geom_buf, size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
+                                void *image_buf, size_t image_bytes, int64_t *num_rendered, uint64_t *weight_sum,
+                                uint32_t *weight_max, uint32_t *touches, void *stream)
+{
+    if (!blend_fwd_has_contrib()) return B200GS_E_UNSUPPORTED;
+    if (!weight_sum || !weight_max || !touches) return B200GS_E_ARGS;
+    const ContribOut co{weight_sum, weight_max, touches};
+    return forward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
+                        projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
+                        instance_capacity, image_buf, image_bytes, num_rendered, stream, &co);
 }
 
 int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
@@ -617,10 +648,23 @@ int b200gs_densify_plan(int32_t P, const b200gs_densify_cfg *cfg, const float *x
     DensifyCfg c;
     c.mode = cfg->mode; c.n_split = cfg->mode == 0 ? cfg->n_split : 0; c.use_screen = cfg->use_screen;
     c.max_grad = cfg->max_grad; c.min_opacity = cfg->min_opacity; c.dense_thresh = cfg->percent_dense_x_extent;
-    c.max_screen_size = cfg->max_screen_size; c.big_ws_thresh = cfg->big_ws_thresh;
+    c.max_screen_size = cfg->max_screen_size; c.big_ws_thresh = cfg->big_ws_thresh; c.remove = nullptr;
     launch_densify_plan(c, P, xyz_gradient_accum, denom, opacity_raw, scaling_raw, plan, counts, (char *)scratch, (cudaStream_t)stream);
     g_launches += 3;
     CK(cudaGetLastError(), "densify_plan launch");
+    return B200GS_OK;
+}
+
+int b200gs_prune_plan(int32_t P, const uint8_t *remove, int32_t *plan, int32_t *counts, void *scratch, size_t scratch_bytes,
+                      void *stream)
+{
+    if (P < 1 || !remove || !plan || !counts || !scratch) return B200GS_E_ARGS;
+    if (scratch_bytes < densify_scratch_bytes(P)) return B200GS_E_BUFFER;
+    DensifyCfg c = {};
+    c.mode = 2; c.remove = remove;
+    launch_densify_plan(c, P, nullptr, nullptr, nullptr, nullptr, plan, counts, (char *)scratch, (cudaStream_t)stream);
+    g_launches += 3;
+    CK(cudaGetLastError(), "prune_plan launch");
     return B200GS_OK;
 }
 

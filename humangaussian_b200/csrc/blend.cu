@@ -39,6 +39,9 @@
 //     blend_bwd_det_abs_kernel are the same bodies with a flush that also sums |q (A dx + B dy)| and |q (B dx + C dy)| into
 //     ScreenGrad's padding (or a float2 per partial); absgrad_out_kernel scales them to dL_dmeans2D_abs.  The default
 //     kernels' SASS does not change.
+//   * Contribution scores (DESIGN.md section 2): blend_fwd_contrib_kernel is the forward body with each hit also folded into
+//     its Gaussian's weight_sum / weight_max / touches (warp reductions, then three atomics from lane 0).  blend_fwd_kernel is
+//     the same body's other instantiation.
 //   * The compile-time switches below are the A/B experiments DESIGN.md section 5 lists: the
 //     product is BWD_T_DIV=1 and BWD_PARK=16, everything else 0.
 #include "common.cuh"
@@ -115,7 +118,29 @@ struct FwdPixel {
 // 13.6 of 32 lanes blend per visit, so a branch would diverge and the warp would issue both sides anyway.  A lane that does
 // not blend keeps C0..C2, Dd, Aa, last and used bit for bit and T up to its sign: its updates are predicated off, never
 // scaled by a zero weight (c * 0 is not an exact no-op for every colour a caller may pass).
-__device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float fpy, FwdPixel &p)
+// Contribution scores (DESIGN.md section 2): one slab hit's warp-wide share of its Gaussian's three accumulators.  A touch is a
+// hit on a live pixel (it blends, or it is the terminating hit); a blend adds q(w) = rn(w * 2^24) and competes with the bits
+// of w for the maximum (w > 0, so unsigned order is float order).  32 lanes * q < 2^29 fits the u32 lane sum.  The ballot
+// is warp-uniform, so the whole warp skips a hit no pixel touched; lane 0 then issues the three reductions.
+__device__ __forceinline__ void contrib_hit(bool touch, bool blend, float w, uint32_t gid, const ContribOut &co)
+{
+    const uint32_t b = __ballot_sync(FULL, touch);
+    if (b == 0u) return;
+    const uint32_t mx = __reduce_max_sync(FULL, blend ? __float_as_uint(w) : 0u);
+    const uint32_t sm = __reduce_add_sync(FULL, blend ? __float2uint_rn(fmul(w, 16777216.0f)) : 0u);
+    if ((threadIdx.x & 31) == 0) {
+        atomicAdd(co.touches + gid, (uint32_t)__popc(b));
+        if (mx != 0u) {
+            atomicMax(co.weight_max + gid, mx);
+            atomicAdd(reinterpret_cast<unsigned long long *>(co.weight_sum) + gid, (unsigned long long)sm);
+        }
+    }
+}
+
+// CONTRIB: the contribution variant also folds the hit into the scores of Gaussian gid (contrib_hit); the pixel's update is
+// the same code.
+template <bool CONTRIB>
+__device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float fpy, FwdPixel &p, uint32_t gid, const ContribOut &co)
 {
     const float4 g0 = s[0], q1 = s[1], q2 = s[2];
     const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
@@ -125,6 +150,7 @@ __device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float 
     const bool hit = !(power > 0.0f) & !(alpha < GS_ALPHA_MIN);
     const bool blend = hit & !(test_T < GS_T_MIN);
     const float w = fmul(alpha, p.T);
+    const bool live = p.T > 0.0f; // (read before the update)
     if (blend) {
         p.C0 = ffma(q2.x, w, p.C0); p.C1 = ffma(q2.y, w, p.C1); p.C2 = ffma(q2.z, w, p.C2);
         p.Dd = ffma(q2.w, w, p.Dd);
@@ -133,18 +159,22 @@ __device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float 
         p.used |= __float_as_uint(g0.w);
     }
     p.T = blend ? test_T : (hit ? -fabsf(p.T) : p.T);
+    if (CONTRIB) contrib_hit(hit & live, blend, w, gid, co);
 }
 
-// Blends the cnt hits staged in slab s, in order, two per iteration.
-__device__ __forceinline__ void fwd_blend_slab(const float4 *s, int cnt, float fpx, float fpy, FwdPixel &p)
+// Blends the cnt hits staged in slab s, in order, two per iteration.  gids: the hits' Gaussian indices (CONTRIB only).
+template <bool CONTRIB>
+__device__ __forceinline__ void fwd_blend_slab(const float4 *s, int cnt, float fpx, float fpy, FwdPixel &p, const uint32_t *gids,
+                                               const ContribOut &co)
 {
     const float4 *const end2 = s + 3 * (cnt & ~1);
 #pragma unroll 1
     for (; s != end2; s += 6) {
-        fwd_blend_hit(s, fpx, fpy, p);
-        fwd_blend_hit(s + 3, fpx, fpy, p);
+        fwd_blend_hit<CONTRIB>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co);
+        fwd_blend_hit<CONTRIB>(s + 3, fpx, fpy, p, CONTRIB ? gids[1] : 0u, co);
+        if (CONTRIB) gids += 2;
     }
-    if (cnt & 1) fwd_blend_hit(s, fpx, fpy, p);
+    if (cnt & 1) fwd_blend_hit<CONTRIB>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co);
 }
 
 // Writes the pixel's outputs (out-of-image pixels write nothing).
@@ -164,7 +194,11 @@ __device__ __forceinline__ void fwd_store_pixel(const BlendArgs &a, int v, int p
 }
 
 #if !FWD_BULK
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_kernel(BlendArgs a)
+// The body of the F6 kernels.  CONTRIB (contribution scores, DESIGN.md section 2): compaction also writes each hit's Gaussian
+// index (record index - v*P) into the warp's 32-word gids array, and every hit is folded into co; everything else is the
+// same code.
+template <bool CONTRIB>
+__device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gid_slabs)[32], const ContribOut &co)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
 
@@ -212,6 +246,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_
             g2 = __ldg(recs4 + 3 * (size_t)id_c + 2);
         }
         const float4 g0_h = g0_c;
+        const uint32_t id_h = id_c;
         id_c = id_n;
         g0_c = make_float4(0.f, 0.f, -1.f, -1.f);
         if (base + 32 + lane < n_total) g0_c = __ldg(recs4 + 3 * (size_t)id_c);
@@ -223,16 +258,33 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_
                 s[0] = make_float4(g0_h.x, g0_h.y, __uint_as_float((uint32_t)(base + lane + 1)), __uint_as_float(bit));
                 s[1] = make_float4(fmul(-0.5f, g1.x), -g1.y, fmul(-0.5f, g1.z), g1.w);
                 s[2] = g2;
+                if (CONTRIB) gid_slabs[warp][__popc(b & lt)] = id_h - (uint32_t)v * (uint32_t)a.P;
             }
             __syncwarp();
             p.used = 0u;
-            fwd_blend_slab(slab, __popc(b), fpx, fpy, p);
+            fwd_blend_slab<CONTRIB>(slab, __popc(b), fpx, fpy, p, CONTRIB ? gid_slabs[warp] : nullptr, co);
             m = __reduce_or_sync(FULL, p.used);
             __syncwarp();
         }
         if (lane == 0) *cm = m;
     }
     if (inside) fwd_store_pixel(a, v, px, py, p);
+}
+
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_kernel(BlendArgs a)
+{
+    blend_fwd_body<false>(a, nullptr, ContribOut{});
+}
+
+// F6 with the contribution scores.  At F6's cap of 56 registers it spills 8 bytes in the hit loop; 16 blocks (64 registers,
+// 32 warps/SM, the backward's occupancy) removes the spill (DESIGN.md section 5)
+#ifndef FWD_CONTRIB_MIN_BLOCKS
+#define FWD_CONTRIB_MIN_BLOCKS 16
+#endif
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_CONTRIB_MIN_BLOCKS) blend_fwd_contrib_kernel(BlendArgs a, ContribOut co)
+{
+    __shared__ uint32_t gids[WARPS_PER_CTA][32];
+    blend_fwd_body<true>(a, gids, co);
 }
 
 #endif // !FWD_BULK
@@ -371,7 +423,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_
             }
             __syncwarp();
             p.used = 0u;
-            fwd_blend_slab(sl.rec, __popc(b), fpx, fpy, p);
+            fwd_blend_slab<false>(sl.rec, __popc(b), fpx, fpy, p, nullptr, ContribOut{});
             m = __reduce_or_sync(FULL, p.used);
             __syncwarp();
         }
@@ -393,6 +445,18 @@ void launch_blend_fwd(const BlendArgs &a, cudaStream_t st)
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
     blend_fwd_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
 }
+
+#if !FWD_BULK
+int blend_fwd_has_contrib() { return 1; }
+void launch_blend_fwd_contrib(const BlendArgs &a, const ContribOut &co, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
+    blend_fwd_contrib_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, co);
+}
+#else
+int blend_fwd_has_contrib() { return 0; } // the contribution variant exists for the default kernel only
+void launch_blend_fwd_contrib(const BlendArgs &, const ContribOut &, cudaStream_t) {}
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // B1

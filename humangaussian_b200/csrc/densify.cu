@@ -8,7 +8,8 @@
 //   stats   one thread per Gaussian folds a V-view batch: sum of the view-space gradients, max radius, then
 //           accum += |sum.xy|, denom += 1, max_radii2D = max(...) where visible (GaussianDreamer.py:385-391 +
 //           gaussian_model.py:433-437);
-//   plan    per Gaussian: clone? split? survive the final opacity / size prune? (for itself and for its children);
+//   plan    per Gaussian: clone? split? survive the final opacity / size prune? (for itself and for its children) -- or, for
+//           b200gs_prune_plan, survive a caller's removal mask (classify mode 2);
 //           three kernels (block counts -> scan of block counts -> block-local ranks) turn the four flag streams
 //           into FINAL destination rows, in the reference's output order
 //              [surviving unsplit originals | surviving clones | surviving children copy 0 | ... copy N-1];
@@ -31,6 +32,11 @@ __device__ __forceinline__ Flags classify(const DensifyCfg &c, int i, const floa
                                            const float *__restrict__ opacity, const float *__restrict__ scaling)
 {
     Flags f;
+    if (c.mode == 2) { // prune by a caller's mask (b200gs_prune_plan): survivors keep their order, nothing is added
+        f.keep = c.remove[i] == 0;
+        f.clone = f.split_sel = f.split_kept = false;
+        return f;
+    }
     const float e0 = expf(scaling[3 * i]), e1 = expf(scaling[3 * i + 1]), e2 = expf(scaling[3 * i + 2]);
     const float smax = fmaxf(e0, fmaxf(e1, e2));
     const bool low_op = sigmoidf_(opacity[i]) < c.min_opacity;

@@ -105,6 +105,14 @@ int launch_test_sort32(uint32_t *ka, uint32_t *kb, uint32_t *va, uint32_t *vb, i
 size_t test_sort32_scratch_bytes(int64_t n);
 
 void launch_blend_fwd(const BlendArgs &a, cudaStream_t st);
+// contribution scores (DESIGN.md section 2): per Gaussian [P], in/out, folded over every pixel of every view of the launch
+struct ContribOut {
+    uint64_t *weight_sum; // sum of q(w) = rn(w * 2^24) over the blends
+    uint32_t *weight_max; // max of the bits of w over the blends
+    uint32_t *touches;    // blends plus terminating hits
+};
+int blend_fwd_has_contrib(); // 0 in the classic comparator and the bulk-copy build
+void launch_blend_fwd_contrib(const BlendArgs &a, const ContribOut &co, cudaStream_t st);
 void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st);
 int blend_sgrad_is_moments(); // which ScreenGrad format the linked blend_bwd writes
 
@@ -166,13 +174,14 @@ int launch_knn3(int P, const float *pts, float *mean_d2, char *scratch, size_t s
 
 // densify / prune (densify.cu)
 struct DensifyCfg {
-    int mode;            // 0 = densify_and_prune, 1 = prune_only
+    int mode;            // 0 = densify_and_prune, 1 = prune_only, 2 = prune by mask (keep = !remove[i])
     int n_split;         // children per split parent (reference: 2)
     int use_screen;      // reference's `if max_screen_size:` branch
     float max_grad, min_opacity;
     float dense_thresh;  // percent_dense * extent
     float max_screen_size;
     float big_ws_thresh; // 0.1 * extent (mode 0) or size_thresh (mode 1)
+    const uint8_t *remove; // [P], mode 2
 };
 size_t densify_scratch_bytes(int P);
 void launch_densify_stats(int P, int V, const float *grads, const int32_t *radii, const uint8_t *update_mask, float *accum, float *denom,

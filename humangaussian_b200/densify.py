@@ -8,6 +8,7 @@ bookkeeping that feeds it (threestudio/systems/GaussianDreamer.py:378-408), with
     params, moments, stats = densify_and_prune(params, moments, stats, max_grad, min_opacity, extent, max_screen_size,
                                                percent_dense)               # every densify_prune_interval steps
     params, moments, stats = prune_only(params, moments, stats, min_opacity, size_thresh)
+    params, moments, stats = prune_points(params, moments, stats, remove)  # any rule's bool [P] mask, e.g. contribution
     install_into_optimizer(optimizer, params, moments)                      # what cat_tensors_to_optimizer /
                                                                             # _prune_optimizer do to torch.optim.Adam
 
@@ -31,6 +32,9 @@ from .rasterizer import _check, _ptr, _stream, load_library
 
 GROUPS = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
 ROLE_COPY, ROLE_XYZ, ROLE_SCALING, ROLE_MOMENT = 0, 1, 2, 3
+
+
+MODE_PRUNE_MASK = 2  # b200gs_prune_plan (not a b200gs_densify_cfg mode)
 
 
 class _Cfg(C.Structure):  # == b200gs_densify_cfg
@@ -95,7 +99,7 @@ class _Surgery:
     destination, which may be a view into a larger buffer (the packed form moves each field into its place in the new
     flat buffer).  Callers run inside `torch.cuda.device(dev)`.  P >= 1."""
 
-    def __init__(self, cfg: _Cfg, stats: DensifyStats, opacity, scaling, rotation, noise, generator):
+    def __init__(self, cfg: _Cfg, stats: DensifyStats, opacity, scaling, rotation, noise, generator, remove=None):
         L = self.L = load_library()
         dev, P = scaling.device, scaling.shape[0]
         self.cfg, self.dev, self.P, self.rotation, self.scaling = cfg, dev, P, rotation, scaling
@@ -104,10 +108,17 @@ class _Surgery:
         counts = torch.empty(5, dtype=torch.int32, device=dev)
         scratch = torch.empty(L.b200gs_densify_scratch_bytes(P), dtype=torch.uint8, device=dev)
         self.st = _stream(dev)
-        _check(L.b200gs_densify_plan(P, C.byref(cfg), _ptr(stats.xyz_gradient_accum), _ptr(stats.denom), _ptr(opacity),
-                                     _ptr(scaling), _ptr(self.plan), _ptr(counts), _ptr(scratch), scratch.numel(), self.st), "densify_plan")
+        if cfg.mode == MODE_PRUNE_MASK:
+            _check(L.b200gs_prune_plan(P, _ptr(remove), _ptr(self.plan), _ptr(counts), _ptr(scratch), scratch.numel(), self.st),
+                   "prune_plan")
+        else:
+            _check(L.b200gs_densify_plan(P, C.byref(cfg), _ptr(stats.xyz_gradient_accum), _ptr(stats.denom), _ptr(opacity),
+                                         _ptr(scaling), _ptr(self.plan), _ptr(counts), _ptr(scratch), scratch.numel(), self.st),
+                   "densify_plan")
         self.counts = counts.cpu()  # the one host sync of the call
         n_keep, n_clone, S_sel, S_kept, P_new = (int(x) for x in self.counts)
+        if cfg.mode == MODE_PRUNE_MASK and P_new == 0:
+            raise ValueError("b200gs: the prune mask removes every Gaussian")
         self.P_new = P_new
         self.ch = (C.c_int32 * 5)(n_keep, n_clone, S_sel, S_kept, P_new)
         if cfg.mode == 0 and noise is None:
@@ -135,7 +146,7 @@ class _Surgery:
         return DensifyStats(out(stats.xyz_gradient_accum), out(stats.denom), out(stats.max_radii2D))
 
 
-def _run(cfg: _Cfg, params: Dict[str, torch.Tensor], moments, stats: DensifyStats, noise, generator):
+def _run(cfg: _Cfg, params: Dict[str, torch.Tensor], moments, stats: DensifyStats, noise, generator, remove=None):
     xyz = params["xyz"]
     _need_cuda(xyz)
     dev, P = xyz.device, xyz.shape[0]
@@ -144,7 +155,7 @@ def _run(cfg: _Cfg, params: Dict[str, torch.Tensor], moments, stats: DensifyStat
         return ({k: v.clone() for k, v in src.items()}, None if moments is None else {k: (m.clone(), v.clone()) for k, (m, v) in moments.items()},
                 DensifyStats.zeros(0, dev), torch.zeros(5, dtype=torch.int32))
     with torch.cuda.device(dev):
-        s = _Surgery(cfg, stats, src["opacity"], src["scaling"], src["rotation"], noise, generator)
+        s = _Surgery(cfg, stats, src["opacity"], src["scaling"], src["rotation"], noise, generator, remove)
 
         def move(role, t):
             return s.move(role, t, torch.empty((s.P_new,) + tuple(t.shape[1:]), dtype=torch.float32, device=dev))
@@ -177,7 +188,7 @@ def prune_only(params, moments, stats: DensifyStats, min_opacity: float = 0.005,
 
 
 # ---- the same surgery on the packed parameter buffer, for optim.PackedAdam -----------------------------------------
-def _run_packed(cfg: _Cfg, opt: torch.optim.Optimizer, stats: DensifyStats, noise, generator) -> int:
+def _run_packed(cfg: _Cfg, opt: torch.optim.Optimizer, stats: DensifyStats, noise, generator, remove=None) -> int:
     """Plan once from the flat buffer's opacity / scaling fields, move every field of the parameter buffer and of both
     Adam moment buffers straight into its place in new flat buffers (padding zero), install them into `opt`, and replace
     the three tensors of `stats` in place.  The optimiser's step count is kept."""
@@ -193,7 +204,7 @@ def _run_packed(cfg: _Cfg, opt: torch.optim.Optimizer, stats: DensifyStats, nois
     xyz, scaling, rotation, opacity, sh = views(old.detach(), fields)
     state = opt.state.get(old)
     with torch.cuda.device(dev):
-        s = _Surgery(cfg, stats, opacity, scaling, rotation, noise, generator)
+        s = _Surgery(cfg, stats, opacity, scaling, rotation, noise, generator, remove)
         new_fields, new_total = packed_layout(s.P_new, K)
 
         def remap(flat, roles):
@@ -234,6 +245,40 @@ def prune_only_packed(opt: torch.optim.Optimizer, stats: DensifyStats, min_opaci
     """`prune_only` on the packed buffer of an `optim.PackedAdam` (see densify_and_prune_packed); returns the new P."""
     cfg = _Cfg(1, 0, 0, 0.0, float(min_opacity), 0.0, 0.0, float(size_thresh))
     return _run_packed(cfg, opt, stats, None, None)
+
+
+def _remove_mask(remove, P: int, dev) -> torch.Tensor:
+    if not isinstance(remove, torch.Tensor) or remove.dtype != torch.bool or remove.shape != (P,) or remove.device != dev:
+        desc = f"{tuple(remove.shape)} {remove.dtype} on {remove.device}" if isinstance(remove, torch.Tensor) else type(remove).__name__
+        raise ValueError(f"b200gs: remove must be a bool [{P}] tensor on {dev}; got {desc}")
+    return remove.contiguous().view(torch.uint8)
+
+
+def prune_points(params, moments, stats: DensifyStats, remove: torch.Tensor, return_counts: bool = False):
+    """GaussianModel.prune_points (gaussian_model.py:306-315) by a caller's mask: drop every Gaussian where `remove` (bool [P]
+    on the device) is True; survivors keep their order.  Parameters, both Adam moments and the three statistics move
+    together, as in `prune_only`.  Any rule can supply the mask: `contribution.compute_contribution(...).touches == 0`
+    (lossless for the cameras it was scored over), a weight threshold, or a hand mask.  A mask that removes every Gaussian
+    raises ValueError.  Returns (params, moments, stats); the new P is params["xyz"].shape[0]."""
+    dev, P = params["xyz"].device, params["xyz"].shape[0]
+    _need_cuda(params["xyz"])
+    cfg = _Cfg(MODE_PRUNE_MASK, 0, 0, 0.0, 0.0, 0.0, 0.0, 0.0)
+    if P == 0:
+        raise ValueError("b200gs: nothing to prune (P == 0)")
+    p, m, s, counts = _run(cfg, params, moments, stats, None, None, _remove_mask(remove, P, dev))
+    return (p, m, s, counts) if return_counts else (p, m, s)
+
+
+def prune_points_packed(opt: torch.optim.Optimizer, stats: DensifyStats, remove: torch.Tensor) -> int:
+    """`prune_points` on the packed buffer of an `optim.PackedAdam` (see densify_and_prune_packed): the parameter buffer,
+    both moment buffers and `stats` are replaced; returns the new P."""
+    group = opt.param_groups[0]
+    P, dev = int(group["P"]), group["params"][0].device
+    _need_cuda(group["params"][0])
+    if P == 0:
+        raise ValueError("b200gs: nothing to prune (P == 0)")
+    cfg = _Cfg(MODE_PRUNE_MASK, 0, 0, 0.0, 0.0, 0.0, 0.0, 0.0)
+    return _run_packed(cfg, opt, stats, None, None, _remove_mask(remove, P, dev))
 
 
 def moments_from_optimizer(optimizer: torch.optim.Optimizer) -> Dict[str, Tuple[torch.Tensor, torch.Tensor]]:

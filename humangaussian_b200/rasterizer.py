@@ -92,7 +92,7 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed", "b200gs_deterministic_bytes",
            "b200gs_backward_deterministic", "b200gs_forward_opts", "b200gs_backward_opts",
            "b200gs_backward_deterministic_opts", "b200gs_sampling_rate", "b200gs_backward_absgrad_opts",
-           "b200gs_backward_deterministic_absgrad_opts"]
+           "b200gs_backward_deterministic_absgrad_opts", "b200gs_forward_contrib_opts", "b200gs_prune_plan"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -136,6 +136,10 @@ def load_library():
     bdo = L.b200gs_backward_deterministic_opts.argtypes
     L.b200gs_backward_deterministic_absgrad_opts.restype = C.c_int
     L.b200gs_backward_deterministic_absgrad_opts.argtypes = bdo[:30] + [vp] + bdo[30:36] + [vp, sz] + bdo[36:]
+    # the contribution form: b200gs_forward_opts' argument list with the three accumulators after num_rendered
+    fo = L.b200gs_forward_opts.argtypes
+    L.b200gs_forward_contrib_opts.restype = C.c_int
+    L.b200gs_forward_contrib_opts.argtypes = fo[:-1] + [vp, vp, vp] + fo[-1:]
     L.b200gs_sampling_rate.restype = C.c_int
     L.b200gs_sampling_rate.argtypes = [i32, i32, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float), i32, i32, vp, vp]
     L.b200gs_mark_visible.restype = C.c_int
@@ -159,6 +163,8 @@ def load_library():
     L.b200gs_densify_scratch_bytes.restype = sz; L.b200gs_densify_scratch_bytes.argtypes = [i32]
     L.b200gs_densify_plan.restype = C.c_int
     L.b200gs_densify_plan.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    L.b200gs_prune_plan.restype = C.c_int
+    L.b200gs_prune_plan.argtypes = [i32, vp, vp, vp, vp, sz, vp]
     L.b200gs_densify_move.restype = C.c_int
     L.b200gs_densify_move.argtypes = [i32, i32, i32, vp, C.POINTER(i32), i32, vp, vp, vp, vp, vp, vp]
     L.b200gs_adam_packed.restype = C.c_int
@@ -332,11 +338,13 @@ def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=F
 
 def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                   campos, tanfovx, tanfovy, H, W, sh_degree, scale_modifier, prefiltered=False, debug=False, raw=False,
-                  antialiasing=False, filter_3d=None):
+                  antialiasing=False, filter_3d=None, contrib=None):
     """All tensors float32 contiguous on one CUDA device.  viewmatrix/projmatrix [V,4,4], campos [V,3].
     raw: opacities / scales / rotations are GaussianModel's raw parameters (activations fused into the kernels).
     antialiasing: the screen-space mip filter; filter_3d: the 3D smoothing filter's [P] variances (b200gs_render_opts).
-    The state remembers both for the backward."""
+    The state remembers both for the backward.
+    contrib: None, or the contribution accumulators (weight_sum, weight_max, touches), [P] int64 / int32 / int32 device tensors
+    read as u64 / u32 / u32: b200gs_forward_contrib_opts then runs and folds this call's views into them."""
     L = load_library()
     dev = means3D.device
     if dev.type != "cuda":
@@ -366,6 +374,9 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     opts = _render_opts(antialiasing, filter_3d) if (antialiasing or filter_3d is not None) else None
     # with the defaults the plain entry point runs (b200gs_forward == b200gs_forward_opts with NULL options)
     fwd = (lambda *a: L.b200gs_forward_opts(a[0], C.byref(opts), *a[1:])) if opts is not None else L.b200gs_forward
+    if contrib is not None:
+        fwd = lambda *a: L.b200gs_forward_contrib_opts(a[0], None if opts is None else C.byref(opts), *a[1:-1],
+                                                       *[_ptr(t) for t in contrib], a[-1])
     with torch.cuda.device(dev):
         for _ in range(3):
             pkey = (key, stream, cap)
@@ -375,12 +386,16 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
                             binning=torch.empty(L.b200gs_binning_bytes(cap, H, W, P, V), **u8),
                             scratch=torch.empty(max(L.b200gs_backward_scratch_bytes(P, V), 16), **u8))
             geom, image, binning = bufs["geom"], bufs["image"], bufs["binning"]
+            # The contribution forward folds into accumulators, so MAX_INSTANCES (which tests can lower) must stop a call before
+            # its blend: it is passed as the capacity, and the library then refuses the call before binning.
+            call_cap = min(cap, MAX_INSTANCES) if contrib is not None else cap
             rc = fwd(C.byref(prm), _ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities), _ptr(scales),
                                   _ptr(rotations), _ptr(cov3D_precomp), _ptr(bg), _ptr(viewmatrix), _ptr(projmatrix),
                                   _ptr(campos), _ptr(color), _ptr(depth), _ptr(alpha), _ptr(radii), _ptr(geom), geom.numel(),
-                                  _ptr(binning), binning.numel(), cap, _ptr(image), image.numel(), C.byref(n_out), C.c_void_p(stream))
-            if rc == OK and n_out.value > MAX_INSTANCES:  # (the library applies the same limit; this one can be lowered in tests)
-                rc = E_INSTANCES
+                                  _ptr(binning), binning.numel(), call_cap, _ptr(image), image.numel(), C.byref(n_out),
+                                  C.c_void_p(stream))
+            if n_out.value > MAX_INSTANCES and (rc == OK or (contrib is not None and rc == E_BIN_TOO_SMALL)):
+                rc = E_INSTANCES  # (the library applies the same limit; this one can be lowered in tests)
             if rc != E_BIN_TOO_SMALL:
                 break
             cap = int(n_out.value * 1.25) + 1024
@@ -392,7 +407,8 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     _last_num_rendered = int(n_out.value)
     st = _Ctx()
     st.prm, st.tanx, st.tany = prm, tx, ty
-    st.geom, st.binning, st.image, st.scratch, st.capacity, st.num_rendered = geom, binning, image, bufs["scratch"], cap, int(n_out.value)
+    st.geom, st.binning, st.image, st.scratch, st.capacity, st.num_rendered = geom, binning, image, bufs["scratch"], call_cap, \
+        int(n_out.value)
     st.radii, st.V, st.P, st.H, st.W, st.M = radii, V, P, H, W, M
     st.opts, st.f3d = opts, filter_3d  # the backward reads the same variances (st keeps them alive)
     weakref.finalize(st, _pool.give, pkey, bufs)  # when the autograd graph drops the state, the buffers are parked for re-use
@@ -758,7 +774,8 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
 
 # ---- test / debugging access to the forward state (tile and sort indices) -----------------------------------
 def forward_with_state(**kw):
-    """Non-differentiable forward returning outputs + a dict of the intermediate buffers as torch tensors."""
+    """Non-differentiable forward returning outputs + a dict of the intermediate buffers as torch tensors.
+    contrib=(weight_sum, weight_max, touches): the contribution forward, folding into those accumulators (_forward_impl)."""
     L = load_library()
     dev = kw["means3D"].device
     t = lambda k: _f32c(kw.get(k), dev)
@@ -771,7 +788,8 @@ def forward_with_state(**kw):
         t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"), t("cov3D_precomp"),
         _f32c(kw["bg"], dev), _f32c(vm, dev).reshape(V, 4, 4), _f32c(pm, dev).reshape(V, 4, 4), _f32c(cp, dev).reshape(V, 3),
         tanx, tany, int(kw["image_height"]), int(kw["image_width"]), int(kw.get("sh_degree", 0)),
-        float(kw.get("scale_modifier", 1.0)), antialiasing=bool(kw.get("antialiasing", False)), filter_3d=kw.get("filter_3d"))
+        float(kw.get("scale_modifier", 1.0)), raw=bool(kw.get("raw", False)), antialiasing=bool(kw.get("antialiasing", False)),
+        filter_3d=kw.get("filter_3d"), contrib=kw.get("contrib"))
     sv = _StateView()
     _check(L.b200gs_describe_state(C.byref(st.prm), _ptr(st.geom), _ptr(st.binning), st.capacity, _ptr(st.image), C.byref(sv)),
            "describe_state")

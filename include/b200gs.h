@@ -251,6 +251,38 @@ int b200gs_backward_deterministic_absgrad_opts(const b200gs_params *prm, const b
                                                void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials,
                                                void *abs_partials, size_t abs_partials_bytes, void *stream);
 
+/* ---- contribution scores: per-Gaussian blend weights of the forward blend (additive to ABI 4) -----------------------
+ * b200gs_forward_contrib_opts takes b200gs_forward_opts's argument list and computes every output exactly as that call does
+ * (images, radii, state buffers byte-identical), plus three per-Gaussian accumulators over every pixel of every view:
+ *   For pixel p and sorted tile-list entry k of p's tile the blend evaluates power, alpha and test_T = T (1 - alpha).
+ *   touch: power <= 0 and alpha >= 1/255 while the pixel is live (its T before the entry is > 0; out-of-image pixels never
+ *     are).  A touch either blends or is the single terminating hit at which T would drop below 1e-4 (it ends the pixel
+ *     without blending).
+ *   blend: a touch that blends, with weight w = fmul(alpha, T), the float the colour sum uses.
+ *   weight_sum [P] u64 (device, in/out): += sum over blends of q(w) = round-half-even(w * 2^24) (w <= 0.99, so q < 2^24).
+ *     weight_sum * 2^-24 is the sum of weights to within 2^-25 per blend.
+ *   weight_max [P] u32 (device, in/out): max(weight_max, bits of w) over blends (w > 0: unsigned order is float order;
+ *     0 = never blended).  Read it as a float.
+ *   touches [P] u32 (device, in/out): += number of touches.
+ * Integer adds and maxima: any camera set, in calls of any size and order, folds to the same bits, and two runs write
+ * identical bytes.  PRECONDITION: the total pixel count sum(V*H*W) folded into one set of accumulators stays below 2^32
+ * (each pixel adds at most 1 to touches and less than 2^24 to weight_sum, so neither can overflow).
+ * Removing every Gaussian with touches == 0 over a camera set, survivors kept in order, leaves those cameras' colour,
+ * depth and alpha byte-identical and the survivors' radii unchanged (DESIGN.md section 2).
+ * This call always waits for the instance count before the blend: one that returns B200GS_E_BIN_TOO_SMALL or
+ * B200GS_E_INSTANCES has not touched the accumulators.  A NULL accumulator is B200GS_E_ARGS; the classic comparator build
+ * returns B200GS_E_UNSUPPORTED. */
+int b200gs_forward_contrib_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                                const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                                const float *scales, const float *rotations, const float *cov3D_precomp,
+                                const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
+                                void *geom_buf, size_t geom_bytes,
+                                void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
+                                void *image_buf, size_t image_bytes,
+                                int64_t *num_rendered, uint64_t *weight_sum, uint32_t *weight_max, uint32_t *touches,
+                                void *stream);
+
 /* ---- 3D smoothing filter: per-Gaussian maximal sampling rate over a camera set (Mip-Splatting's 3D filter) ------------
  * For each of the n_views cameras (viewmatrix [n_views,16] device, tanfovx / tanfovy host [n_views], shared H x W), with
  * (tx, ty, tz) the preprocess's view-space position and fx = W / (2 tanfovx), fy = H / (2 tanfovy): Gaussian k is in view
@@ -318,6 +350,12 @@ size_t b200gs_densify_scratch_bytes(int32_t P);
 int b200gs_densify_plan(int32_t P, const b200gs_densify_cfg *cfg, const float *xyz_gradient_accum, const float *denom,
                         const float *opacity_raw, const float *scaling_raw, int32_t *plan, int32_t *counts,
                         void *scratch, size_t scratch_bytes, void *stream);
+
+/* Plans a prune by mask in the same plan [4,P] / counts [5] layout, for b200gs_densify_move with n_split = 0: Gaussian i
+ * survives iff remove[i] == 0 (remove [P] uint8, device), survivors keep their order, nothing is cloned or split
+ * (counts = n_keep, 0, 0, 0, n_keep).  scratch: b200gs_densify_scratch_bytes(P).  P >= 1. */
+int b200gs_prune_plan(int32_t P, const uint8_t *remove, int32_t *plan, int32_t *counts, void *scratch, size_t scratch_bytes,
+                      void *stream);
 
 /* Moves one [P,row_floats] array to its planned [P_new,row_floats] place.  role: */
 enum { B200GS_ROLE_COPY = 0,    /* new rows repeat the parent row (f_dc, f_rest, opacity, rotation; statistics in mode 1) */
