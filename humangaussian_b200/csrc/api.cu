@@ -115,13 +115,32 @@ static int read_opts(const b200gs_render_opts *o, bool *aa, const float **f3d)
     return B200GS_OK;
 }
 
+// b200gs_normals_io: the fields every normals call reads (the build, the struct, the workspace; no axis without scales)
+static int check_normals_io(const b200gs_normals_io *n, const float *cov3D_precomp)
+{
+    if (!blend_has_normals()) return B200GS_E_UNSUPPORTED;
+    if (!n || n->struct_bytes < (int32_t)sizeof(b200gs_normals_io) || !n->gauss_normals || cov3D_precomp) return B200GS_E_ARGS;
+    if (((uintptr_t)n->gauss_normals) & 15) return B200GS_E_BUFFER;
+    return B200GS_OK;
+}
+static NormalArgs normal_args(const b200gs_params *prm, const float *means3D, const float *scales, const float *rotations,
+                              const float *campos)
+{
+    NormalArgs n;
+    n.P = prm->P; n.V = prm->n_views; n.raw = prm->raw_params != 0;
+    n.means_view_stride = prm->means3D_per_view ? (size_t)3 * prm->P : 0;
+    n.means = means3D; n.scales = scales; n.rots = rotations; n.campos = campos;
+    return n;
+}
+
 // b200gs_forward_opts (contrib NULL) and b200gs_forward_contrib_opts (the blend with the contribution scores)
 static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
                         const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
                         const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
                         const float *campos, float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf,
                         size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf,
-                        size_t image_bytes, int64_t *num_rendered, void *stream, const ContribOut *contrib)
+                        size_t image_bytes, int64_t *num_rendered, void *stream, const ContribOut *contrib,
+                        const b200gs_normals_io *nrm = nullptr)
 {
     bool aa = false;
     const float *f3d = nullptr;
@@ -130,6 +149,11 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
     rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
     if (f3d && cov3D_precomp) return B200GS_E_ARGS; // the 3D filter widens scales; a precomputed covariance has none
+    if (nrm) {
+        rc = check_normals_io(nrm, cov3D_precomp);
+        if (rc) return rc;
+        if (!nrm->out_normal) return B200GS_E_ARGS;
+    }
     if (!means3D || !opacities || !bg || !viewmatrix || !projmatrix || !campos || !out_color || !out_depth || !out_alpha ||
         !radii || !geom_buf || !binning_buf || !image_buf || !num_rendered)
         return B200GS_E_ARGS;
@@ -163,8 +187,12 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
         a.radii = radii; a.recs = (GeomRec *)(gb + GL.recs); a.tiles_touched = (uint32_t *)(gb + GL.tiles_touched);
         a.rects = (uint2 *)(gb + GL.rects); a.clamped = (uint8_t *)(gb + GL.clamped);
         a.dkeys = (uint32_t *)(bb + BL.dkeys_in); a.order_in = (uint32_t *)(bb + BL.order_in);
-        { StageTimer t(B200GS_STAGE_PREPROCESS, st); launch_preprocess_fwd(a, V, aa, f3d, st); }
-        g_launches += 1;
+        {
+            StageTimer t(B200GS_STAGE_PREPROCESS, st);
+            launch_preprocess_fwd(a, V, aa, f3d, st);
+            if (nrm) launch_normal_prep(normal_args(prm, means3D, scales, rotations, campos), (float4 *)nrm->gauss_normals, st);
+        }
+        g_launches += nrm ? 2 : 1;
         uint32_t *offsets = (uint32_t *)(gb + GL.offsets); // inclusive scan of tiles_touched in DEPTH order
         const int64_t n_vp = (int64_t)P * V;
         const uint32_t *order_sorted = nullptr;
@@ -221,6 +249,7 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
     {
         StageTimer t(B200GS_STAGE_BLEND_FWD, st);
         if (contrib) launch_blend_fwd_contrib(b, *contrib, st);
+        else if (nrm) launch_blend_fwd_nrm(b, (const float4 *)nrm->gauss_normals, nrm->out_normal, st);
         else launch_blend_fwd(b, st);
         g_launches += 1;
     }
@@ -263,6 +292,20 @@ int b200gs_forward_contrib_opts(const b200gs_params *prm, const b200gs_render_op
                         instance_capacity, image_buf, image_bytes, num_rendered, stream, &co);
 }
 
+int b200gs_forward_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+                                const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                                const float *scales, const float *rotations, const float *cov3D_precomp, const float *bg,
+                                const float *viewmatrix, const float *projmatrix, const float *campos, float *out_color,
+                                float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf, size_t geom_bytes,
+                                void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf,
+                                size_t image_bytes, int64_t *num_rendered, void *stream)
+{
+    if (!nrm) return B200GS_E_ARGS;
+    return forward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
+                        projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
+                        instance_capacity, image_buf, image_bytes, num_rendered, stream, nullptr, nrm);
+}
+
 int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
                    const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
                    const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
@@ -291,11 +334,24 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
                          float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
                          size_t scratch_bytes, void *stream, bool det, void *det_buf, size_t det_bytes, int64_t partial_capacity,
                          int64_t *n_partials, bool absgrad = false, float *dL_dmeans2D_abs = nullptr, void *abs_partials = nullptr,
-                         size_t abs_partials_bytes = 0)
+                         size_t abs_partials_bytes = 0, const b200gs_normals_io *nio = nullptr)
 {
     bool aa = false;
     const float *f3d = nullptr;
     if (absgrad && !blend_bwd_has_absgrad()) return B200GS_E_UNSUPPORTED;
+    // a normals call without dL_dnormal is exactly the call without normals
+    const b200gs_normals_io *nrm = nio && nio->struct_bytes >= (int32_t)sizeof(b200gs_normals_io) && !nio->dL_dnormal ? nullptr : nio;
+    if (nrm) {
+        const int rc = check_normals_io(nrm, cov3D_precomp);
+        if (rc) return rc;
+        if (!nrm->normal_wn) return B200GS_E_ARGS;
+        if (((uintptr_t)nrm->normal_wn) & 15) return B200GS_E_BUFFER;
+        if (det) {
+            if (!nrm->nrm_partials) return B200GS_E_ARGS;
+            if ((((uintptr_t)nrm->nrm_partials) & 15) || (partial_capacity > 0 && nrm->nrm_partials_bytes < (size_t)partial_capacity * 16))
+                return B200GS_E_BUFFER;
+        }
+    }
     if (read_opts(opts, &aa, &f3d)) return B200GS_E_ARGS;
     if (f3d && cov3D_precomp) return B200GS_E_ARGS;
     if (absgrad && !dL_dmeans2D_abs) return B200GS_E_ARGS;
@@ -333,6 +389,9 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     if (det && det_bytes < DL.total) return B200GS_E_BUFFER;
 
     if (!det) CK(cudaMemsetAsync(scratch, 0, (size_t)P * V * sizeof(ScreenGrad), st), "memset scratch");
+    if (!det && nrm) CK(cudaMemsetAsync(nrm->normal_wn, 0, (size_t)P * V * 16, st), "memset normal_wn");
+    const NrmBwd nb{nrm ? (const float4 *)nrm->gauss_normals : nullptr, nrm ? nrm->dL_dnormal : nullptr,
+                    nrm ? (float4 *)nrm->normal_wn : nullptr, nrm ? (float4 *)nrm->nrm_partials : nullptr};
     BlendBwdArgs b;
     b.H = H; b.W = W; b.grid_x = gx; b.grid_y = gy; b.V = V; b.P = P;
     b.ranges = (const uint2 *)(bb + BL.ranges); b.point_list = (const uint32_t *)(bb + BL.vals_out);
@@ -344,7 +403,8 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     b.sgrad = scratch;
     if (!det) {
         StageTimer t(B200GS_STAGE_BLEND_BWD, st);
-        if (absgrad) launch_blend_bwd_abs(b, nullptr, st);
+        if (nrm) launch_blend_bwd_nrm(b, nullptr, absgrad, nb, st);
+        else if (absgrad) launch_blend_bwd_abs(b, nullptr, st);
         else launch_blend_bwd(b, st);
     } else {
         // pre-pass -> (the one host wait: the partial count) -> B1 with per-partial stores -> fixed-order reduce.  The wait
@@ -379,10 +439,12 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
         float2 *abs_p = absgrad ? (float2 *)abs_partials : nullptr;
         const DetFlush flush{pa.pm, pa.base, partials, abs_p};
         if (H_partials > 0) {
-            if (absgrad) launch_blend_bwd_abs(b, &flush, st);
+            if (nrm) launch_blend_bwd_nrm(b, &flush, absgrad, nb, st);
+            else if (absgrad) launch_blend_bwd_abs(b, &flush, st);
             else launch_blend_bwd_det(b, flush, st);
         }
-        launch_det_reduce(pa, n_vp, partials, abs_p, scratch, st);
+        if (nrm) launch_det_reduce_nrm(pa, n_vp, partials, abs_p, scratch, nb.partials, nb.wn, st);
+        else launch_det_reduce(pa, n_vp, partials, abs_p, scratch, st);
         g_launches += (H_partials > 0) + 1;
     }
     if (absgrad) {
@@ -404,8 +466,13 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     a.dL_dmeans3D = dL_dmeans3D; a.dL_dmeans2D = dL_dmeans2D; a.dL_dsh = dL_dsh; a.dL_dcolors = dL_dcolors;
     a.dL_dopacity = dL_dopacity; a.dL_dscales = dL_dscales; a.dL_drots = dL_drots; a.dL_dcov3D = dL_dcov3D;
     a.f3d_var = f3d;
-    { StageTimer t(B200GS_STAGE_PREPROCESS_BWD, st); launch_preprocess_bwd(a, aa, f3d != nullptr, st); }
-    g_launches += det ? 1 : 2; // (the deterministic blend stage counted its own launches)
+    {
+        StageTimer t(B200GS_STAGE_PREPROCESS_BWD, st);
+        launch_preprocess_bwd(a, aa, f3d != nullptr, st);
+        // dL/dn through the rotations, added to what the preprocess backward wrote
+        if (nrm) launch_normal_bwd(normal_args(prm, means3D, scales, rotations, campos), radii, nb.gauss_normals, nb.wn, dL_drots, st);
+    }
+    g_launches += (det ? 1 : 2) + (nrm ? 1 : 0); // (the deterministic blend stage counted its own launches)
     CK(cudaGetLastError(), "backward launch");
     return B200GS_OK;
 }
@@ -505,6 +572,71 @@ int b200gs_backward_deterministic_absgrad_opts(const b200gs_params *prm, const b
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
                          scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials, true, dL_dmeans2D_abs,
                          abs_partials, abs_partials_bytes);
+}
+
+// the normals forms of the four backward entry points: b200gs_normals_io after opts (include/b200gs.h)
+int b200gs_backward_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+    const float *means3D, const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
+    const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+    const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+    float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
+    float *dL_drots, float *dL_dcov3D, void *scratch, size_t scratch_bytes, void *stream)
+{
+    if (!nrm) return B200GS_E_ARGS;
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr, false, nullptr, nullptr, 0, nrm);
+}
+
+int b200gs_backward_deterministic_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+    const float *means3D, const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
+    const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+    const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+    float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
+    float *dL_drots, float *dL_dcov3D, void *scratch, size_t scratch_bytes, void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials,
+    void *stream)
+{
+    if (!nrm) return B200GS_E_ARGS;
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials, false, nullptr,
+                         nullptr, 0, nrm);
+}
+
+int b200gs_backward_absgrad_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+    const float *means3D, const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
+    const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+    const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+    float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
+    float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream)
+{
+    if (!nrm) return B200GS_E_ARGS;
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr, true, dL_dmeans2D_abs, nullptr, 0, nrm);
+}
+
+int b200gs_backward_deterministic_absgrad_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+    const b200gs_normals_io *nrm, const float *means3D, const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
+    const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
+    const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+    float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
+    float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *det_buf,
+    size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *abs_partials, size_t abs_partials_bytes, void *stream)
+{
+    if (!nrm) return B200GS_E_ARGS;
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials, true,
+                         dL_dmeans2D_abs, abs_partials, abs_partials_bytes, nrm);
 }
 
 int b200gs_sampling_rate(int32_t P, int32_t n_views, const float *means3D, const float *viewmatrix, const float *tanfovx,

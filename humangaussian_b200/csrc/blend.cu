@@ -42,6 +42,10 @@
 //   * Contribution scores (DESIGN.md section 2): blend_fwd_contrib_kernel is the forward body with each hit also folded into
 //     its Gaussian's weight_sum / weight_max / touches (warp reductions, then three atomics from lane 0).  blend_fwd_kernel is
 //     the same body's other instantiation.
+//   * Normal maps (DESIGN.md section 2): blend_fwd_nrm_kernel and the four B1 nrm kernels are the same bodies with an NRM flag:
+//     each hit's normal (normals.cu's gauss_normals) is staged next to its slab record, the forward keeps three more sums
+//     per pixel, the backward adds n . dL/dN to cg and the flush sums Wn = sum w dL/dN.  The default kernels' SASS does not
+//     change.
 //   * The compile-time switches below are the A/B experiments DESIGN.md section 5 lists: the
 //     product is BWD_T_DIV=1 and BWD_PARK=16, everything else 0.
 #include "common.cuh"
@@ -139,8 +143,11 @@ __device__ __forceinline__ void contrib_hit(bool touch, bool blend, float w, uin
 
 // CONTRIB: the contribution variant also folds the hit into the scores of Gaussian gid (contrib_hit); the pixel's update is
 // the same code.
-template <bool CONTRIB>
-__device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float fpy, FwdPixel &p, uint32_t gid, const ContribOut &co)
+// NRM (normal maps, DESIGN.md section 2): the hit's normal n (its slab word ns) is accumulated as N_c = fma(n_c, w, N_c) under
+// the colour's predicate.
+template <bool CONTRIB, bool NRM = false>
+__device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float fpy, FwdPixel &p, uint32_t gid, const ContribOut &co,
+                                              const float4 *ns = nullptr, float *N = nullptr)
 {
     const float4 g0 = s[0], q1 = s[1], q2 = s[2];
     const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
@@ -158,23 +165,29 @@ __device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float 
         p.last = __float_as_uint(g0.z);
         p.used |= __float_as_uint(g0.w);
     }
+    if (NRM) {
+        const float4 n = *ns;
+        if (blend) { N[0] = ffma(n.x, w, N[0]); N[1] = ffma(n.y, w, N[1]); N[2] = ffma(n.z, w, N[2]); }
+    }
     p.T = blend ? test_T : (hit ? -fabsf(p.T) : p.T);
     if (CONTRIB) contrib_hit(hit & live, blend, w, gid, co);
 }
 
 // Blends the cnt hits staged in slab s, in order, two per iteration.  gids: the hits' Gaussian indices (CONTRIB only).
-template <bool CONTRIB>
+// NRM: ns holds the hits' normals, N the pixel's three normal sums.
+template <bool CONTRIB, bool NRM = false>
 __device__ __forceinline__ void fwd_blend_slab(const float4 *s, int cnt, float fpx, float fpy, FwdPixel &p, const uint32_t *gids,
-                                               const ContribOut &co)
+                                               const ContribOut &co, const float4 *ns = nullptr, float *N = nullptr)
 {
     const float4 *const end2 = s + 3 * (cnt & ~1);
 #pragma unroll 1
     for (; s != end2; s += 6) {
-        fwd_blend_hit<CONTRIB>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co);
-        fwd_blend_hit<CONTRIB>(s + 3, fpx, fpy, p, CONTRIB ? gids[1] : 0u, co);
+        fwd_blend_hit<CONTRIB, NRM>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co, ns, N);
+        fwd_blend_hit<CONTRIB, NRM>(s + 3, fpx, fpy, p, CONTRIB ? gids[1] : 0u, co, NRM ? ns + 1 : ns, N);
         if (CONTRIB) gids += 2;
+        if (NRM) ns += 2;
     }
-    if (cnt & 1) fwd_blend_hit<CONTRIB>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co);
+    if (cnt & 1) fwd_blend_hit<CONTRIB, NRM>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co, ns, N);
 }
 
 // Writes the pixel's outputs (out-of-image pixels write nothing).
@@ -197,8 +210,12 @@ __device__ __forceinline__ void fwd_store_pixel(const BlendArgs &a, int v, int p
 // The body of the F6 kernels.  CONTRIB (contribution scores, DESIGN.md section 2): compaction also writes each hit's Gaussian
 // index (record index - v*P) into the warp's 32-word gids array, and every hit is folded into co; everything else is the
 // same code.
-template <bool CONTRIB>
-__device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gid_slabs)[32], const ContribOut &co)
+// NRM (normal maps, DESIGN.md section 2): hit lanes also gather gauss_normals[record index] into the warp's 32-entry nrm_slabs
+// row, the pixel keeps three normal sums, and the pixel writes them to out_normal [V,3,H,W].
+template <bool CONTRIB, bool NRM = false>
+__device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gid_slabs)[32], const ContribOut &co,
+                                               float4 (*nrm_slabs)[32] = nullptr, const float4 *gauss_normals = nullptr,
+                                               float *out_normal = nullptr)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
 
@@ -225,6 +242,7 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
     uint32_t *const cmask = a.cmask + ((size_t)(range.x >> 5) + vt) * 8 + patch;
 
     FwdPixel p = {inside ? 1.0f : 0.0f, 0.f, 0.f, 0.f, 0.f, 0.f, 0u, 0u};
+    float N[3] = {0.f, 0.f, 0.f};
 
     // software pipeline, two deep: while chunk c is blended the support boxes of chunk c+1 and the ids of chunk c+2
     // are in flight (the id -> record address dependency never sits on the critical path)
@@ -240,10 +258,11 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
         if (__all_sync(FULL, !(p.T > 0.0f))) break;
         const bool hit = box_hits_patch(g0_c, fx0, fy0, fx1, fy1);
         const uint32_t b = __ballot_sync(FULL, hit);
-        float4 g1, g2;
+        float4 g1, g2, gn;
         if (hit) {
             g1 = __ldg(recs4 + 3 * (size_t)id_c + 1);
             g2 = __ldg(recs4 + 3 * (size_t)id_c + 2);
+            if (NRM) gn = __ldg(gauss_normals + id_c);
         }
         const float4 g0_h = g0_c;
         const uint32_t id_h = id_c;
@@ -259,16 +278,25 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
                 s[1] = make_float4(fmul(-0.5f, g1.x), -g1.y, fmul(-0.5f, g1.z), g1.w);
                 s[2] = g2;
                 if (CONTRIB) gid_slabs[warp][__popc(b & lt)] = id_h - (uint32_t)v * (uint32_t)a.P;
+                if (NRM) nrm_slabs[warp][__popc(b & lt)] = gn;
             }
             __syncwarp();
             p.used = 0u;
-            fwd_blend_slab<CONTRIB>(slab, __popc(b), fpx, fpy, p, CONTRIB ? gid_slabs[warp] : nullptr, co);
+            fwd_blend_slab<CONTRIB, NRM>(slab, __popc(b), fpx, fpy, p, CONTRIB ? gid_slabs[warp] : nullptr, co,
+                                         NRM ? nrm_slabs[warp] : nullptr, N);
             m = __reduce_or_sync(FULL, p.used);
             __syncwarp();
         }
         if (lane == 0) *cm = m;
     }
-    if (inside) fwd_store_pixel(a, v, px, py, p);
+    if (inside) {
+        fwd_store_pixel(a, v, px, py, p);
+        if (NRM) {
+            const size_t HW = (size_t)a.H * a.W, pix = (size_t)py * a.W + px;
+            float *on = out_normal + (size_t)v * 3 * HW + pix;
+            on[0] = N[0]; on[HW] = N[1]; on[2 * HW] = N[2];
+        }
+    }
 }
 
 __global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_kernel(BlendArgs a)
@@ -285,6 +313,17 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_CONTRIB_MIN_BLOCKS) bl
 {
     __shared__ uint32_t gids[WARPS_PER_CTA][32];
     blend_fwd_body<true>(a, gids, co);
+}
+
+// F6 with the normal image (DESIGN.md section 5 lists its registers at this bound)
+#ifndef FWD_NRM_MIN_BLOCKS
+#define FWD_NRM_MIN_BLOCKS 16
+#endif
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_NRM_MIN_BLOCKS) blend_fwd_nrm_kernel(BlendArgs a, const float4 *gauss_normals,
+                                                                                             float *out_normal)
+{
+    __shared__ float4 nrm[WARPS_PER_CTA][32];
+    blend_fwd_body<false, true>(a, nullptr, ContribOut{}, nrm, gauss_normals, out_normal);
 }
 
 #endif // !FWD_BULK
@@ -453,9 +492,17 @@ void launch_blend_fwd_contrib(const BlendArgs &a, const ContribOut &co, cudaStre
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
     blend_fwd_contrib_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, co);
 }
+int blend_has_normals() { return 1; }
+void launch_blend_fwd_nrm(const BlendArgs &a, const float4 *gauss_normals, float *out_normal, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
+    blend_fwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal);
+}
 #else
 int blend_fwd_has_contrib() { return 0; } // the contribution variant exists for the default kernel only
 void launch_blend_fwd_contrib(const BlendArgs &, const ContribOut &, cudaStream_t) {}
+int blend_has_normals() { return 0; } // nor the normal maps (their backward kernels are not launched either)
+void launch_blend_fwd_nrm(const BlendArgs &, const float4 *, float *, cudaStream_t) {}
 #endif
 
 // ------------------------------------------------------------------------------------------------
@@ -496,9 +543,13 @@ __device__ __forceinline__ void red_add_v2(float *p, float a, float b)
 // Ay = sum |q (B dx + C dy)| over the slot's pixels, with the record's conic (word 1, still in L1 from the hit loop's staging
 // load); B dy and C dy are folded once per row.  They go to ScreenGrad's padding (the third RED becomes a v4), or in
 // deterministic mode to the partial's own float2 of det.abs_partials.  The ten sums are formed exactly as without ABS.
-template <bool DET, bool ABS>
+// NRM (normal maps, DESIGN.md section 2): the flush also sums Wn = sum w * dL/dN over the slot's pixels, dL/dN from the
+// warp's second pixel table npix (laid out as pk.pix).  Atomic mode adds (Wn, 0) to nb.wn[record] with one more v4 RED;
+// deterministic mode stores it to nb.partials[slot].  Everything else is formed exactly as without NRM.
+template <bool DET, bool ABS, bool NRM = false>
 __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, float fx0, float fy_part, float *sgrad,
-                                           const BlendBwdArgs &a, const DetFlush &det)
+                                           const BlendBwdArgs &a, const DetFlush &det, const float4 *npix = nullptr,
+                                           const NrmBwd *nb = nullptr)
 {
     __syncwarp();
     const int h = lane % BWD_PARK, part = lane / BWD_PARK;
@@ -509,7 +560,7 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
 #pragma unroll
     for (int k = 0; k < 8; k++) dxk[k] = fsub(s.x, fadd(fx0, (float)k));
     float S0 = 0.f, Sx = 0.f, Sy = 0.f, Sxx = 0.f, Sxy = 0.f, Syy = 0.f, W0 = 0.f, W1 = 0.f, W2 = 0.f, W3 = 0.f;
-    float Ax = 0.f, Ay = 0.f;
+    float Ax = 0.f, Ay = 0.f, N0 = 0.f, N1 = 0.f, N2 = 0.f;
 #pragma unroll
     for (int r = 0; r < BWD_PARK / 8; r++) {
         const int p0 = BWD_PARK * part + 8 * r; // first pixel of the row
@@ -533,6 +584,10 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
                 Ax += fabsf(v.x * fmaf(conic.x, dxk[k], Bdy));
                 Ay += fabsf(v.x * fmaf(conic.y, dxk[k], Cdy));
             }
+            if (NRM) {
+                const float4 gn = npix[p0 + k + part];
+                N0 = fmaf(v.y, gn.x, N0); N1 = fmaf(v.y, gn.y, N1); N2 = fmaf(v.y, gn.z, N2);
+            }
         }
         const float dy = fsub(s.y, fadd(fy_part, (float)r));
         const float qy = R0 * dy;
@@ -547,6 +602,7 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
         W0 += __shfl_xor_sync(FULL, W0, o); W1 += __shfl_xor_sync(FULL, W1, o); W2 += __shfl_xor_sync(FULL, W2, o);
         W3 += __shfl_xor_sync(FULL, W3, o);
         if (ABS) { Ax += __shfl_xor_sync(FULL, Ax, o); Ay += __shfl_xor_sync(FULL, Ay, o); }
+        if (NRM) { N0 += __shfl_xor_sync(FULL, N0, o); N1 += __shfl_xor_sync(FULL, N1, o); N2 += __shfl_xor_sync(FULL, N2, o); }
     }
     if (DET) {
         if (h < n) {
@@ -562,6 +618,7 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
                 rec[4] = make_float2(W2, W3);
                 if (ABS) det.abs_partials[slot] = make_float2(Ax, Ay);
             }
+            if (NRM && part == 1) nb->partials[slot] = make_float4(N0, N1, N2, 0.f);
         }
     } else if (h < n) {
         // ScreenGrad as moments: S0, Sx, Sy, Sxx | Sxy, Syy, w.gC0, w.gC1 | w.gC2, w.gD (| Ax, Ay in the padding with ABS)
@@ -574,14 +631,18 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
             if (ABS) red_add_v4(rec + 8, W2, W3, Ax, Ay);
             else red_add_v2(rec + 8, W2, W3);
         }
+        if (NRM && part == 1) red_add_v4(reinterpret_cast<float *>(nb->wn + __float_as_uint(s.w)), N0, N1, N2, 0.f);
     }
     __syncwarp();
 }
 
 // The body of the B1 kernels: DET selects the flush (vector REDs into ScreenGrad, or stores of per-(instance, patch)
 // partials), ABS adds the absolute sums to it; everything else is the same code.
-template <bool DET, bool ABS>
-__device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetFlush &det)
+// NRM (normal maps): contributing lanes also stage gauss_normals[record] in the warp's nslab row, the pixel's dL/dN goes to
+// the second pixel table npix, cg gains n . dL/dN, and the flush sums Wn (park_flush).
+template <bool DET, bool ABS, bool NRM = false>
+__device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetFlush &det, float4 (*nslabs)[32] = nullptr,
+                                               float4 (*npixs)[32 + PARK_LANES] = nullptr, const NrmBwd *nb = nullptr)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
     __shared__ WarpPark parks[WARPS_PER_CTA];
@@ -609,6 +670,7 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
     const uint32_t lt = (1u << lane) - 1u;
 
     float T_final = 1.f, gC0 = 0.f, gC1 = 0.f, gC2 = 0.f, gD = 0.f, gA = 0.f;
+    float4 gN = make_float4(0.f, 0.f, 0.f, 0.f);
     int last = 0;
     if (inside) {
         T_final = a.final_T[v * HW + pix];
@@ -619,6 +681,10 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
         }
         if (a.dL_ddepth) gD = a.dL_ddepth[v * HW + pix];
         if (a.dL_dalpha) gA = a.dL_dalpha[v * HW + pix];
+        if (NRM) {
+            const float *g = nb->dL_dnormal + (size_t)v * 3 * HW;
+            gN = make_float4(g[pix], g[HW + pix], g[2 * HW + pix], 0.f);
+        }
     }
     int wmax = last; // list positions at or beyond the patch's largest n_contrib cannot contribute here
     wmax = max(wmax, __shfl_xor_sync(FULL, wmax, 16));
@@ -630,6 +696,7 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
 
     const float bg_dot = a.bg[0] * gC0 + a.bg[1] * gC1 + a.bg[2] * gC2;
     pk.pix[lane + lane / BWD_PARK] = make_float4(gC0, gC1, gC2, gD); // read by the flushes, after their __syncwarp
+    if (NRM) npixs[warp][lane + lane / BWD_PARK] = gN;
     int np = 0;                                                      // park slots in use (warp-uniform)
     const float fx0 = (float)x0, fy_part = (float)(y0 + (lane / BWD_PARK) * (BWD_PARK / 8)); // the flush lane's first row
     float *const sgrad = reinterpret_cast<float *>(a.sgrad);
@@ -665,11 +732,13 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
             sl.rec[3 * s] = make_float4(g0.x, g0.y, __uint_as_float((uint32_t)(32 * c + 31 - lane)), __uint_as_float(id_h));
             sl.rec[3 * s + 1] = make_float4(fmul(-0.5f, g1.x), -g1.y, fmul(-0.5f, g1.z), g1.w);
             sl.rec[3 * s + 2] = g2;
+            if (NRM) nslabs[warp][s] = __ldg(nb->gauss_normals + id_h);
         }
         __syncwarp();
         // The chunk's hits in runs that end at the next flush: one counter (np, the park slot) per hit, and the slab, park
         // and slot-table addresses advance as running pointers.
         const float4 *s = sl.rec;
+        const float4 *ns = NRM ? nslabs[warp] : nullptr;
         for (int left = __popc(mr); left > 0;) {
             const int run = min(left, BWD_PARK - np);
             left -= run;
@@ -685,7 +754,11 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
                 // (every entry the contributor mask staged has a contributing lane: no vote.)  The pixel's update is
                 // computed on every lane and selected: a lane that does not contribute keeps T, rg, last_cg and last_alpha
                 // and parks (0, 0).
-                const float cg = fmaf(q2.x, gC0, fmaf(q2.y, gC1, fmaf(q2.z, gC2, fmaf(q2.w, gD, gA))));
+                float cg = fmaf(q2.x, gC0, fmaf(q2.y, gC1, fmaf(q2.z, gC2, fmaf(q2.w, gD, gA))));
+                if (NRM) { // cg += n . dL/dN, components 2, 1, 0 (the normal image has no background term)
+                    const float4 n = *ns++;
+                    cg = fmaf(n.x, gN.x, fmaf(n.y, gN.y, fmaf(n.z, gN.z, cg)));
+                }
                 const float one_m_a = 1.0f - alpha;
                 float inv; // 1/(1-alpha), 1-alpha in [0.01, 1) where the lane contributes
                 asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv) : "f"(one_m_a));
@@ -709,13 +782,13 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
                 if (lane == 0) pk.hit[np] = g0;
             }
             if (np == BWD_PARK) {
-                park_flush<DET, ABS>(pk, np, lane, fx0, fy_part, sgrad, a, det);
+                park_flush<DET, ABS, NRM>(pk, np, lane, fx0, fy_part, sgrad, a, det, NRM ? npixs[warp] : nullptr, nb);
                 np = 0;
             }
         }
         __syncwarp();
     }
-    if (np > 0) park_flush<DET, ABS>(pk, np, lane, fx0, fy_part, sgrad, a, det);
+    if (np > 0) park_flush<DET, ABS, NRM>(pk, np, lane, fx0, fy_part, sgrad, a, det, NRM ? npixs[warp] : nullptr, nb);
 }
 
 __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_kernel(BlendBwdArgs a)
@@ -752,6 +825,44 @@ void launch_blend_bwd_det(const BlendBwdArgs &a, const DetFlush &det, cudaStream
 {
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
     blend_bwd_det_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, det);
+}
+
+// B1 with the normal term (NRM): atomic / deterministic, without and with the absolute sums.  Each stages the normals and
+// dL/dN in two more per-warp shared arrays.
+#define BWD_NRM_SHARED                                  \
+    __shared__ float4 nslab[WARPS_PER_CTA][32];         \
+    __shared__ float4 npix[WARPS_PER_CTA][32 + PARK_LANES]
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_nrm_kernel(BlendBwdArgs a, NrmBwd nb)
+{
+    BWD_NRM_SHARED;
+    blend_bwd_body<false, false, true>(a, DetFlush{}, nslab, npix, &nb);
+}
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_nrm_abs_kernel(BlendBwdArgs a, NrmBwd nb)
+{
+    BWD_NRM_SHARED;
+    blend_bwd_body<false, true, true>(a, DetFlush{}, nslab, npix, &nb);
+}
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_nrm_kernel(BlendBwdArgs a, DetFlush det, NrmBwd nb)
+{
+    BWD_NRM_SHARED;
+    blend_bwd_body<true, false, true>(a, det, nslab, npix, &nb);
+}
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_nrm_abs_kernel(BlendBwdArgs a, DetFlush det,
+                                                                                                  NrmBwd nb)
+{
+    BWD_NRM_SHARED;
+    blend_bwd_body<true, true, true>(a, det, nslab, npix, &nb);
+}
+void launch_blend_bwd_nrm(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd &n, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
+    if (det) {
+        if (absgrad) blend_bwd_det_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det, n);
+        else blend_bwd_det_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det, n);
+    } else {
+        if (absgrad) blend_bwd_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, n);
+        else blend_bwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, n);
+    }
 }
 
 int blend_bwd_has_absgrad() { return 1; }

@@ -67,6 +67,22 @@ __device__ __forceinline__ float gs_dot3(float a0, float a1, float a2, float b0,
     return ffma(a2, b2, a);
 }
 
+// R(q) of a quaternion q = (r, x, y, z), row-major, in the pinned operation order the covariance uses (preprocess.cu,
+// build_cov3d); column k is the Gaussian's k-th axis, the one the normals (normals.cu) take
+__device__ __forceinline__ void gs_rotmat(const float *q, float R[3][3])
+{
+    const float r = q[0], x = q[1], y = q[2], z = q[3];
+    R[0][0] = ffma(-2.0f, ffma(z, z, fmul(y, y)), 1.0f);
+    R[0][1] = fmul(2.0f, ffma(x, y, -fmul(r, z)));
+    R[0][2] = fmul(2.0f, ffma(x, z, fmul(r, y)));
+    R[1][0] = fmul(2.0f, ffma(x, y, fmul(r, z)));
+    R[1][1] = ffma(-2.0f, ffma(z, z, fmul(x, x)), 1.0f);
+    R[1][2] = fmul(2.0f, ffma(y, z, -fmul(r, x)));
+    R[2][0] = fmul(2.0f, ffma(x, z, -fmul(r, y)));
+    R[2][1] = fmul(2.0f, ffma(y, z, fmul(r, x)));
+    R[2][2] = ffma(-2.0f, ffma(y, y, fmul(x, x)), 1.0f);
+}
+
 // ---- per-(view,Gaussian) geometry record: 48 B, three 16-B words ----------------------------------
 struct __align__(16) GeomRec {
     float px, py;    // pixel-space centre

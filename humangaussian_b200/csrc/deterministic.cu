@@ -86,9 +86,12 @@ __global__ void __launch_bounds__(256) det_plan_kernel(const DetPlanArgs a)
 // One thread per (view, Gaussian), taken in depth order k: vp = order[k] owns the emission indices
 // [offsets[k] - tiles_touched[vp], offsets[k]).
 // ABS: also adds the partials' (Ax, Ay) from abs_partials, same order, into the record's padding.
-template <bool ABS>
+// NRM (normal maps): also adds the partials' normal sums from nrm_partials, same order, and writes them to wn[vp].
+template <bool ABS, bool NRM = false>
 __global__ void __launch_bounds__(256) det_reduce_kernel(const DetPlanArgs a, int64_t n_vp, const float *__restrict__ partials,
-                                                          float *__restrict__ sgrad, const float2 *__restrict__ abs_partials)
+                                                          float *__restrict__ sgrad, const float2 *__restrict__ abs_partials,
+                                                          const float4 *__restrict__ nrm_partials = nullptr,
+                                                          float4 *__restrict__ wn = nullptr)
 {
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_vp) return;
@@ -97,7 +100,7 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const DetPlanArgs a, in
     float s[DET_PARTIAL_FLOATS];
 #pragma unroll
     for (int i = 0; i < DET_PARTIAL_FLOATS; i++) s[i] = 0.0f;
-    float ax = 0.0f, ay = 0.0f;
+    float ax = 0.0f, ay = 0.0f, n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
     for (uint32_t e = e0; e != e0 + n; e++) {
         const uint32_t j = __ldg(a.jpos + e);
         const uint32_t np = (uint32_t)__popc((uint32_t)__ldg(a.pm + j));
@@ -115,12 +118,19 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const DetPlanArgs a, in
                 ax = fadd(ax, x.x);
                 ay = fadd(ay, x.y);
             }
+            if (NRM) {
+                const float4 x = __ldg(nrm_partials + q);
+                n0 = fadd(n0, x.x);
+                n1 = fadd(n1, x.y);
+                n2 = fadd(n2, x.z);
+            }
         }
     }
     float4 *dst = reinterpret_cast<float4 *>(sgrad + (size_t)vp * (sizeof(ScreenGrad) / sizeof(float)));
     dst[0] = make_float4(s[0], s[1], s[2], s[3]);
     dst[1] = make_float4(s[4], s[5], s[6], s[7]);
     dst[2] = make_float4(s[8], s[9], ax, ay);
+    if (NRM) wn[vp] = make_float4(n0, n1, n2, 0.0f);
 }
 
 int launch_det_plan(const DetPlanArgs &a, int64_t n_vp, int n_tiles_all, const DetLayout &L, char *det_base, cudaStream_t st,
@@ -138,4 +148,12 @@ void launch_det_reduce(const DetPlanArgs &a, int64_t n_vp, const float *partials
     const unsigned grid = (unsigned)((n_vp + 255) / 256);
     if (abs_partials) det_reduce_kernel<true><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, abs_partials);
     else det_reduce_kernel<false><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, nullptr);
+}
+
+void launch_det_reduce_nrm(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
+                           const float4 *nrm_partials, float4 *wn, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)((n_vp + 255) / 256);
+    if (abs_partials) det_reduce_kernel<true, true><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, abs_partials, nrm_partials, wn);
+    else det_reduce_kernel<false, true><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, nullptr, nrm_partials, wn);
 }

@@ -163,6 +163,32 @@ void launch_absgrad_out(int64_t n_vp, int H, int W, const int32_t *radii, const 
                         cudaStream_t st);
 void launch_test_exp(const float *x, float *y, int64_t n, cudaStream_t st);
 
+// ---- normal maps (DESIGN.md section 2; normals.cu, and the NRM instantiations of the blend kernels) -----------------------
+struct NormalArgs {
+    int P, V, raw;
+    size_t means_view_stride;                       // as PreArgs
+    const float *means, *scales, *rots, *campos;    // [P,3] or [V,P,3], [P,3], [P,4], [V,3]
+};
+// gauss_normals [V*P]: (sign n, sign) of every (view, Gaussian), n the axis of its smallest activated scale
+void launch_normal_prep(const NormalArgs &a, float4 *gauss_normals, cudaStream_t st);
+// dL_drots[i] += dL/dq of sum over the views with radii > 0 of sign * wn[v*P + i]
+void launch_normal_bwd(const NormalArgs &a, const int32_t *radii, const float4 *gauss_normals, const float4 *wn, float *dL_drots,
+                       cudaStream_t st);
+int blend_has_normals(); // 0 in the classic comparator and the bulk-copy build
+// F6 with the normal image out_normal [V,3,H,W] = sum w * n
+void launch_blend_fwd_nrm(const BlendArgs &a, const float4 *gauss_normals, float *out_normal, cudaStream_t st);
+struct NrmBwd {
+    const float4 *gauss_normals; // [V*P]
+    const float *dL_dnormal;     // [V,3,H,W]
+    float4 *wn;                  // [V*P] atomic mode: sum w * dL/dN of every (view, Gaussian), zeroed by the caller
+    float4 *partials;            // [H] deterministic mode: each partial's three sums, at its slot
+};
+// B1 with the normal term: atomic (det NULL) or deterministic, with or without the absolute sums
+void launch_blend_bwd_nrm(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd &n, cudaStream_t st);
+// the deterministic reduce with the normal partials: also writes wn[vp] = their sums in the same fixed order
+void launch_det_reduce_nrm(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
+                           const float4 *nrm_partials, float4 *wn, cudaStream_t st);
+
 // animation frame path (anim.cu)
 void launch_reattach(int P, int n_frames, int n_verts, int n_faces, const float *vertices, const int32_t *faces, const int32_t *map_face,
                      const float *map_uvw, const float *map_dist, float *xyz, cudaStream_t st);

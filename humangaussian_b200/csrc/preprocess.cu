@@ -19,17 +19,8 @@ __constant__ float c_SH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.45
 
 __device__ __forceinline__ void build_cov3d(const float *s3, float mod, const float *q, float *c6)
 {
-    const float r = q[0], x = q[1], y = q[2], z = q[3];
     float R[3][3];
-    R[0][0] = ffma(-2.0f, ffma(z, z, fmul(y, y)), 1.0f);
-    R[0][1] = fmul(2.0f, ffma(x, y, -fmul(r, z)));
-    R[0][2] = fmul(2.0f, ffma(x, z, fmul(r, y)));
-    R[1][0] = fmul(2.0f, ffma(x, y, fmul(r, z)));
-    R[1][1] = ffma(-2.0f, ffma(z, z, fmul(x, x)), 1.0f);
-    R[1][2] = fmul(2.0f, ffma(y, z, -fmul(r, x)));
-    R[2][0] = fmul(2.0f, ffma(x, z, -fmul(r, y)));
-    R[2][1] = fmul(2.0f, ffma(y, z, fmul(r, x)));
-    R[2][2] = ffma(-2.0f, ffma(y, y, fmul(x, x)), 1.0f);
+    gs_rotmat(q, R);
     const float s[3] = {fmul(mod, s3[0]), fmul(mod, s3[1]), fmul(mod, s3[2])};
     float L[3][3];
 #pragma unroll

@@ -77,6 +77,17 @@ def _check_filter_3d(filter_3d, P, device, cov3D_precomp=None):
     return filter_3d.detach().contiguous()
 
 
+class _NormalsIO(C.Structure):
+    """b200gs_normals_io (include/b200gs.h): the normal map's buffers"""
+    _fields_ = [("struct_bytes", C.c_int32), ("gauss_normals", C.c_void_p), ("out_normal", C.c_void_p), ("dL_dnormal", C.c_void_p),
+                ("normal_wn", C.c_void_p), ("nrm_partials", C.c_void_p), ("nrm_partials_bytes", C.c_size_t)]
+
+
+def _normals_io(gauss_normals, out_normal=None, dL_dnormal=None, normal_wn=None, nrm_partials=None):
+    return _NormalsIO(C.sizeof(_NormalsIO), _ptr(gauss_normals), _ptr(out_normal), _ptr(dL_dnormal), _ptr(normal_wn),
+                      _ptr(nrm_partials), 0 if nrm_partials is None else nrm_partials.numel())
+
+
 class _StateView(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("geom_records", "tiles_touched", "offsets", "clamped", "sorted_tile_keys",
                                           "depth_order", "point_list", "ranges", "final_T", "n_contrib",
@@ -92,7 +103,9 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed", "b200gs_deterministic_bytes",
            "b200gs_backward_deterministic", "b200gs_forward_opts", "b200gs_backward_opts",
            "b200gs_backward_deterministic_opts", "b200gs_sampling_rate", "b200gs_backward_absgrad_opts",
-           "b200gs_backward_deterministic_absgrad_opts", "b200gs_forward_contrib_opts", "b200gs_prune_plan"]
+           "b200gs_backward_deterministic_absgrad_opts", "b200gs_forward_contrib_opts", "b200gs_prune_plan",
+           "b200gs_forward_normals_opts", "b200gs_backward_normals_opts", "b200gs_backward_deterministic_normals_opts",
+           "b200gs_backward_absgrad_normals_opts", "b200gs_backward_deterministic_absgrad_normals_opts"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -140,6 +153,13 @@ def load_library():
     fo = L.b200gs_forward_opts.argtypes
     L.b200gs_forward_contrib_opts.restype = C.c_int
     L.b200gs_forward_contrib_opts.argtypes = fo[:-1] + [vp, vp, vp] + fo[-1:]
+    # the normals forms: the *_opts argument lists with the b200gs_normals_io pointer after opts
+    for name, base in (("forward", fo), ("backward", bo), ("backward_deterministic", bdo),
+                       ("backward_absgrad", L.b200gs_backward_absgrad_opts.argtypes),
+                       ("backward_deterministic_absgrad", L.b200gs_backward_deterministic_absgrad_opts.argtypes)):
+        fn = getattr(L, f"b200gs_{name}_normals_opts")
+        fn.restype = C.c_int
+        fn.argtypes = base[:2] + [C.POINTER(_NormalsIO)] + base[2:]
     L.b200gs_sampling_rate.restype = C.c_int
     L.b200gs_sampling_rate.argtypes = [i32, i32, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float), i32, i32, vp, vp]
     L.b200gs_mark_visible.restype = C.c_int
@@ -325,7 +345,7 @@ def release_cached_buffers():
 class _Ctx:
     """What one forward keeps for its backward (upstream keeps geomBuffer/binningBuffer/imgBuffer the same way)."""
     __slots__ = ("prm", "tanx", "tany", "geom", "binning", "image", "scratch", "capacity", "num_rendered", "radii", "V", "P", "H",
-                 "W", "M", "opts", "f3d", "__weakref__")
+                 "W", "M", "opts", "f3d", "gauss_normals", "normal", "normal_wn", "__weakref__")
 
 
 def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=False, per_view_means=False, raw=False):
@@ -338,13 +358,15 @@ def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=F
 
 def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                   campos, tanfovx, tanfovy, H, W, sh_degree, scale_modifier, prefiltered=False, debug=False, raw=False,
-                  antialiasing=False, filter_3d=None, contrib=None):
+                  antialiasing=False, filter_3d=None, contrib=None, normals=False):
     """All tensors float32 contiguous on one CUDA device.  viewmatrix/projmatrix [V,4,4], campos [V,3].
     raw: opacities / scales / rotations are GaussianModel's raw parameters (activations fused into the kernels).
     antialiasing: the screen-space mip filter; filter_3d: the 3D smoothing filter's [P] variances (b200gs_render_opts).
     The state remembers both for the backward.
     contrib: None, or the contribution accumulators (weight_sum, weight_max, touches), [P] int64 / int32 / int32 device tensors
-    read as u64 / u32 / u32: b200gs_forward_contrib_opts then runs and folds this call's views into them."""
+    read as u64 / u32 / u32: b200gs_forward_contrib_opts then runs and folds this call's views into them.
+    normals=True: b200gs_forward_normals_opts runs; the state holds the normal image `normal` [V,3,H,W] and the per-(view,
+    Gaussian) normals `gauss_normals` [V,P,4] its backward reads."""
     L = load_library()
     dev = means3D.device
     if dev.type != "cuda":
@@ -360,6 +382,10 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
             ((scales is not None or rotations is not None) and cov3D_precomp is not None):
         raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
     M = 0 if shs is None else shs.shape[1]
+    if normals and cov3D_precomp is not None:
+        raise ValueError("b200gs: normals take each Gaussian's shortest scale axis; a precomputed covariance has none")
+    if normals and contrib is not None:
+        raise ValueError("b200gs: the contribution forward does not render normals")
     filter_3d = _check_filter_3d(filter_3d, P, dev, cov3D_precomp)
     prm, tx, ty = _make_params(P, V, sh_degree, M, H, W, scale_modifier, tanfovx, tanfovy, prefiltered, debug, per_view_means, raw)
     u8 = dict(dtype=torch.uint8, device=dev)
@@ -374,6 +400,12 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     opts = _render_opts(antialiasing, filter_3d) if (antialiasing or filter_3d is not None) else None
     # with the defaults the plain entry point runs (b200gs_forward == b200gs_forward_opts with NULL options)
     fwd = (lambda *a: L.b200gs_forward_opts(a[0], C.byref(opts), *a[1:])) if opts is not None else L.b200gs_forward
+    gauss_normals = normal = None
+    if normals:
+        gauss_normals = torch.empty(V, P, 4, dtype=torch.float32, device=dev)
+        normal = torch.empty(V, 3, H, W, dtype=torch.float32, device=dev)
+        nio = _normals_io(gauss_normals, normal)
+        fwd = lambda *a: L.b200gs_forward_normals_opts(a[0], None if opts is None else C.byref(opts), C.byref(nio), *a[1:])
     if contrib is not None:
         fwd = lambda *a: L.b200gs_forward_contrib_opts(a[0], None if opts is None else C.byref(opts), *a[1:-1],
                                                        *[_ptr(t) for t in contrib], a[-1])
@@ -411,14 +443,16 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
         int(n_out.value)
     st.radii, st.V, st.P, st.H, st.W, st.M = radii, V, P, H, W, M
     st.opts, st.f3d = opts, filter_3d  # the backward reads the same variances (st keeps them alive)
+    st.gauss_normals, st.normal, st.normal_wn = gauss_normals, normal, None
     weakref.finalize(st, _pool.give, pkey, bufs)  # when the autograd graph drops the state, the buffers are parked for re-use
     return color, radii, depth, alpha, st
 
 
-def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_abs=None):
+def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_abs=None, nio=None):
     """b200gs_backward_deterministic with the work buffer from _det_pool, sized by the partial-capacity hint; a call whose
     partials do not fit is repeated with room for the count it reported (at most two retries).  d_means2D_abs: the absgrad
-    form, with its float2-per-partial array pooled beside the work buffer."""
+    form, with its float2-per-partial array pooled beside the work buffer.  nio: the normals form (_NormalsIO with dL_dnormal),
+    with its float4-per-partial array pooled the same way."""
     P, V, H, W = st.P, st.V, st.H, st.W
     key = (dev.index, P, V, H, W)
     pcap = _partial_hint.get(key, max(1 << 16, 2 * st.num_rendered))
@@ -426,14 +460,27 @@ def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_ab
     stream = torch.cuda.current_stream(dev).cuda_stream
     for _ in range(3):
         # sized for the forward's instance capacity (>= its count), so the pool key stays the same from call to call
-        pkey = (dev.index, stream, st.capacity, pcap, P, V, d_means2D_abs is not None)
+        pkey = (dev.index, stream, st.capacity, pcap, P, V, d_means2D_abs is not None, nio is not None)
         bufs = _det_pool.take(pkey)
         if bufs is None:
             bufs = dict(det=torch.empty(L.b200gs_deterministic_bytes(st.capacity, pcap, P, V), dtype=torch.uint8, device=dev))
             if d_means2D_abs is not None:
                 bufs["abs"] = torch.empty(max(8 * pcap, 16), dtype=torch.uint8, device=dev)
+            if nio is not None:
+                bufs["nrm"] = torch.empty(max(16 * pcap, 16), dtype=torch.uint8, device=dev)
         det = bufs["det"]
-        if d_means2D_abs is not None:
+        opts_p = C.byref(st.opts) if st.opts is not None else None
+        if nio is not None:
+            nio.nrm_partials, nio.nrm_partials_bytes = _ptr(bufs["nrm"]), bufs["nrm"].numel()
+            if d_means2D_abs is not None:
+                ab = bufs["abs"]
+                rc = L.b200gs_backward_deterministic_absgrad_normals_opts(
+                    args[0], opts_p, C.byref(nio), *args[1:29], _ptr(d_means2D_abs), *args[29:], _ptr(det), det.numel(), pcap,
+                    C.byref(n_out), _ptr(ab), ab.numel(), C.c_void_p(stream))
+            else:
+                rc = L.b200gs_backward_deterministic_normals_opts(args[0], opts_p, C.byref(nio), *args[1:], _ptr(det), det.numel(),
+                                                                  pcap, C.byref(n_out), C.c_void_p(stream))
+        elif d_means2D_abs is not None:
             ab = bufs["abs"]
             opts = C.byref(st.opts) if st.opts is not None else None
             rc = L.b200gs_backward_deterministic_absgrad_opts(args[0], opts, *args[1:29], _ptr(d_means2D_abs), *args[29:], _ptr(det),
@@ -459,12 +506,16 @@ def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_ab
 
 
 def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
-                   projmatrix, campos, g_color, g_depth, g_alpha, out=None, det_state=None, absgrad=False):
+                   projmatrix, campos, g_color, g_depth, g_alpha, out=None, det_state=None, absgrad=False, g_normal=None):
     """`out` (optional): dict of preallocated contiguous fp32 gradient buffers by name (means3D, sh, opacity, scales,
     rotations) -- the packed entry points them into one flat buffer so that B3 writes the all-reduce payload in place.
 
     absgrad=True: the absgrad entry points run, and a ninth value is returned: dL_dmeans2D_abs [V,P,3], the per-pixel terms
     of dL_dmeans2D summed in absolute value (include/b200gs.h).  Every other gradient is what absgrad=False gives.
+
+    g_normal [V,3,H,W] (a forward with normals=True): the normals entry points run, dL/dN reaches the opacities, means and
+    colours through the blend weights and the rotations through the normals; st.normal_wn then holds the [V,P,4] sums Wn.
+    None: the call without normals.
 
     Under torch.use_deterministic_algorithms(True) the backward is the library's deterministic one: the same gradients up
     to float rounding, bit-identical from run to run (one host wait per call, for its partial count).  `det_state`
@@ -493,9 +544,20 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
             _ptr(st.binning), st.capacity, _ptr(st.image), st.num_rendered, _ptr(g_color), _ptr(g_depth), _ptr(g_alpha),
             _ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh), _ptr(d_col), _ptr(d_op), _ptr(d_sc), _ptr(d_rot), _ptr(d_cov),
             _ptr(scratch), scratch.numel())
+    nio = None
+    if g_normal is not None and st.gauss_normals is not None:
+        st.normal_wn = torch.empty(V, P, 4, **f)
+        nio = _normals_io(st.gauss_normals, None, g_normal, st.normal_wn)
     with torch.cuda.device(dev):
         if torch.are_deterministic_algorithms_enabled():
-            rc = _backward_deterministic(L, st, dev, args, det_state, d_abs)
+            rc = _backward_deterministic(L, st, dev, args, det_state, d_abs, nio)
+        elif nio is not None:
+            opts_p = C.byref(st.opts) if st.opts is not None else None
+            if absgrad:
+                rc = L.b200gs_backward_absgrad_normals_opts(args[0], opts_p, C.byref(nio), *args[1:29], _ptr(d_abs), *args[29:],
+                                                            _stream(dev))
+            else:
+                rc = L.b200gs_backward_normals_opts(args[0], opts_p, C.byref(nio), *args[1:], _stream(dev))
         elif absgrad:
             rc = L.b200gs_backward_absgrad_opts(args[0], C.byref(st.opts) if st.opts is not None else None, *args[1:29], _ptr(d_abs),
                                                 *args[29:], _stream(dev))
@@ -524,7 +586,7 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, squeeze,
-                means2D_abs=None):
+                means2D_abs=None, normals=False):
         bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, prefiltered, debug = cams[:12]
         raw = bool(cams[12]) if len(cams) > 12 else False
         aa = bool(cams[13]) if len(cams) > 13 else False
@@ -532,7 +594,8 @@ class _RasterizeViews(torch.autograd.Function):
         dev = means3D.device
         args = [_f32c(t, dev) for t in (means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)]
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
-        color, radii, depth, alpha, st = _forward_impl(*args, *camt, tanx, tany, H, W, deg, mod, prefiltered, debug, raw, aa, f3d)
+        color, radii, depth, alpha, st = _forward_impl(*args, *camt, tanx, tany, H, W, deg, mod, prefiltered, debug, raw, aa, f3d,
+                                                       normals=normals)
         ctx.st, ctx.squeeze, ctx.absgrad = st, squeeze, means2D_abs is not None
         _save(ctx, args + camt)
         ctx.in_shapes = [None if t is None else t.shape for t in (means3D, means2D, shs, colors_precomp, opacities, scales,
@@ -540,23 +603,28 @@ class _RasterizeViews(torch.autograd.Function):
         ctx.mark_non_differentiable(radii)
         if squeeze:
             return color[0], radii[0], depth[0], alpha[0]
+        if normals:
+            # an output the loss does not use gets None, not zeros: a normal image returned but not in the loss then runs the
+            # plain backward kernels (the C ABI's dL_dnormal = NULL), and an unused image is skipped like a zero one
+            ctx.set_materialize_grads(False)
+            return color, radii, depth, alpha, st.normal
         return color, radii, depth, alpha
 
     @staticmethod
-    def backward(ctx, g_color, g_radii, g_depth, g_alpha):
+    def backward(ctx, g_color, g_radii, g_depth, g_alpha, g_normal=None):
         st = ctx.st  # kept until the graph is freed: a second backward (retain_graph=True) recomputes from the same state
         means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix, campos = _saved(ctx)
         dev = means3D.device
         g = [None if t is None else _f32c(t, dev) for t in (g_color, g_depth, g_alpha)]
         d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov, *d_abs = _backward_impl(
             st, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix, campos, *g,
-            absgrad=ctx.absgrad)
+            absgrad=ctx.absgrad, g_normal=None if g_normal is None else _f32c(g_normal, dev))
         if ctx.squeeze:
             d_means2D = d_means2D[0]
         # gradients take the shape the caller passed (e.g. opacities [P] or [P,1])
         grads = [g if (g is None or shp is None) else g.reshape(shp)
                  for g, shp in zip((d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov), ctx.in_shapes)]
-        return (*grads, None, None, d_abs[0] if d_abs else None)
+        return (*grads, None, None, d_abs[0] if d_abs else None, None)
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -619,8 +687,15 @@ class GaussianRasterizer(nn.Module):
 
 def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, tanfovx, tanfovy, image_height, image_width,
                     bg, sh_degree=0, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
-                    means2D=None, scale_modifier=1.0, raw=False, antialiasing=False, filter_3d=None, means2D_abs=None):
+                    means2D=None, scale_modifier=1.0, raw=False, antialiasing=False, filter_3d=None, means2D_abs=None,
+                    normals=False):
     """Render V cameras of one Gaussian set in ONE call (one preprocess/sort/blend launch set, one host sync).
+
+    normals=True: a fifth output, the normal image [V,3,H,W] = sum over each pixel's blends of w * n, n the world-space axis of
+    the Gaussian's smallest scale flipped to face the camera (unnormalised, no background, 0 where nothing blends; DESIGN.md
+    section 2).  It is differentiable: its gradient reaches the opacities, means and colours through the blend weights and
+    the rotations through n.  Every other output is unchanged.  Not with cov3D_precomp (ValueError).  comp_normal() turns it
+    into threestudio's normal map.
 
     means2D_abs: None, or a [V,P,3] fp32 gradient sink like means2D (zeros, requires_grad): the backward then fills its
     .grad with the absolute screen-space gradient -- per (view, Gaussian) the per-pixel terms of means2D's gradient summed
@@ -653,9 +728,9 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                                 scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
                                 means2D=None if means2D is None else means2D[i:i + MAX_VIEWS], scale_modifier=scale_modifier, raw=raw,
                                 antialiasing=antialiasing, filter_3d=filter_3d,
-                                means2D_abs=None if means2D_abs is None else means2D_abs[i:i + MAX_VIEWS])
+                                means2D_abs=None if means2D_abs is None else means2D_abs[i:i + MAX_VIEWS], normals=normals)
                 for i in range(0, V, MAX_VIEWS)]
-        return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
+        return tuple(torch.cat([o[k] for o in outs], 0) for k in range(5 if normals else 4))
     _check_filter_3d(filter_3d, means3D.shape[-2], means3D.device, cov3D_precomp)
     if means2D is None:
         means2D = torch.zeros(V, means3D.shape[-2], 3, dtype=torch.float32, device=means3D.device)
@@ -663,7 +738,7 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
             int(sh_degree), float(scale_modifier), False, False, bool(raw), bool(antialiasing), filter_3d)
     try:
         return _RasterizeViews.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, False,
-                                     means2D_abs)
+                                     means2D_abs, bool(normals))
     except InstanceLimitError:
         if V == 1:
             raise
@@ -674,9 +749,9 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                             image_height=image_height, image_width=image_width, bg=bg, sh_degree=sh_degree, shs=shs,
                             colors_precomp=colors_precomp, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
                             means2D=means2D[sl], scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing,
-                            filter_3d=filter_3d, means2D_abs=None if means2D_abs is None else means2D_abs[sl])
+                            filter_3d=filter_3d, means2D_abs=None if means2D_abs is None else means2D_abs[sl], normals=normals)
             for sl in (slice(0, h), slice(h, V))]
-    return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
+    return tuple(torch.cat([o[k] for o in outs], 0) for k in range(5 if normals else 4))
 
 
 # ---- packed entry: one flat SoA parameter buffer in, one flat gradient buffer out ---------------------------------
@@ -705,20 +780,23 @@ def _split_packed(flat: torch.Tensor, P: int, M: int):
 
 class _RasterizePacked(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, packed, means2D, P, M, cams, means2D_abs=None):
+    def forward(ctx, packed, means2D, P, M, cams, means2D_abs=None, normals=False):
         bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, raw, aa, f3d = cams
         dev = packed.device
         xyz, sc, rot, op, sh = _split_packed(packed.detach(), P, M)
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
         color, radii, depth, alpha, st = _forward_impl(xyz, sh, None, op, sc, rot, None, *camt, tanx, tany, H, W, deg, mod, raw=raw,
-                                                       antialiasing=aa, filter_3d=f3d)
+                                                       antialiasing=aa, filter_3d=f3d, normals=normals)
         ctx.st, ctx.P, ctx.M, ctx.absgrad = st, P, M, means2D_abs is not None
         ctx.save_for_backward(packed, *camt)
         ctx.mark_non_differentiable(radii)
+        if normals:
+            ctx.set_materialize_grads(False)  # as _RasterizeViews: an unused normal image costs no normal backward
+            return color, radii, depth, alpha, st.normal
         return color, radii, depth, alpha
 
     @staticmethod
-    def backward(ctx, g_color, g_radii, g_depth, g_alpha):
+    def backward(ctx, g_color, g_radii, g_depth, g_alpha, g_normal=None):
         packed, bg, viewmatrix, projmatrix, campos = ctx.saved_tensors
         packed = packed.detach()
         P, M, dev = ctx.P, ctx.M, packed.device
@@ -728,20 +806,20 @@ class _RasterizePacked(torch.autograd.Function):
         g = [None if t is None else _f32c(t, dev) for t in (g_color, g_depth, g_alpha)]
         _, d_means2D, *rest = _backward_impl(ctx.st, xyz, sh, None, op, sc, rot, None, bg, viewmatrix, projmatrix, campos, *g,
                                              out=dict(means3D=d_xyz, sh=d_sh, opacity=d_op, scales=d_sc, rotations=d_rot),
-                                             absgrad=ctx.absgrad)
-        return d_packed, d_means2D, None, None, None, rest[6] if ctx.absgrad else None
+                                             absgrad=ctx.absgrad, g_normal=None if g_normal is None else _f32c(g_normal, dev))
+        return d_packed, d_means2D, None, None, None, rest[6] if ctx.absgrad else None, None
 
 
 def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, viewmatrices, projmatrices, camposs, tanfovx, tanfovy,
                            image_height, image_width, bg, sh_degree=0, means2D=None, scale_modifier=1.0, raw=False, antialiasing=False,
-                           filter_3d=None, means2D_abs=None):
+                           filter_3d=None, means2D_abs=None, normals=False):
     """`rasterize_views` over ONE flat fp32 buffer [xyz 3P | scales 3P | rotations 4P | opacities P | shs 3*K*P], each
     field starting on a 16-byte boundary (`packed_layout`; what `dist.pack` produces, broadcast once per parameter
     version).  raw=False: post-activation values, as the rasteriser's classic inputs.  raw=True: the buffer holds the
     optimiser's RAW parameters (log-scales, un-normalised quaternions, opacity logits; SH = cat(f_dc, f_rest)); the
     activations of gaussian_model.py:95-118 and their Jacobians run inside the kernels, so `packed.grad` is the gradient
     of the raw parameters and a training step needs no activation kernels, no pack copy and no autograd nodes besides
-    this one.  antialiasing, filter_3d, means2D_abs: as `rasterize_views`.  The backward
+    this one.  antialiasing, filter_3d, means2D_abs, normals: as `rasterize_views`.  The backward
     kernels write the parameter gradients straight into one buffer of the same layout, which becomes `packed.grad`
     as is: no per-tensor gradient accumulation, and on several GPUs that buffer is the all-reduce payload in place.
     V <= MAX_VIEWS.  Returns color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W]."""
@@ -758,7 +836,7 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
     cams = (bg, viewmatrices, projmatrices, camposs, list(tanfovx), list(tanfovy), int(image_height), int(image_width),
             int(sh_degree), float(scale_modifier), bool(raw), bool(antialiasing), filter_3d)
     try:
-        return _RasterizePacked.apply(packed, means2D, int(P), int(sh_coeffs), cams, means2D_abs)
+        return _RasterizePacked.apply(packed, means2D, int(P), int(sh_coeffs), cams, means2D_abs, bool(normals))
     except InstanceLimitError:
         if V == 1:
             raise
@@ -767,15 +845,17 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
                                    tanfovx=list(tanfovx)[sl], tanfovy=list(tanfovy)[sl], image_height=image_height,
                                    image_width=image_width, bg=bg, sh_degree=sh_degree, means2D=means2D[sl],
                                    scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing, filter_3d=filter_3d,
-                                   means2D_abs=None if means2D_abs is None else means2D_abs[sl])
+                                   means2D_abs=None if means2D_abs is None else means2D_abs[sl], normals=normals)
             for sl in (slice(0, h), slice(h, V))]
-    return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4))
+    return tuple(torch.cat([o[k] for o in outs], 0) for k in range(5 if normals else 4))
 
 
 # ---- test / debugging access to the forward state (tile and sort indices) -----------------------------------
 def forward_with_state(**kw):
     """Non-differentiable forward returning outputs + a dict of the intermediate buffers as torch tensors.
-    contrib=(weight_sum, weight_max, touches): the contribution forward, folding into those accumulators (_forward_impl)."""
+    contrib=(weight_sum, weight_max, touches): the contribution forward, folding into those accumulators (_forward_impl).
+    normals=True: the normals forward; the normal image [V,3,H,W] is then a fifth output after alpha, and the state also holds
+    "gauss_normals" [V*P,4] (sign * n, sign) of every (view, Gaussian)."""
     L = load_library()
     dev = kw["means3D"].device
     t = lambda k: _f32c(kw.get(k), dev)
@@ -789,7 +869,7 @@ def forward_with_state(**kw):
         _f32c(kw["bg"], dev), _f32c(vm, dev).reshape(V, 4, 4), _f32c(pm, dev).reshape(V, 4, 4), _f32c(cp, dev).reshape(V, 3),
         tanx, tany, int(kw["image_height"]), int(kw["image_width"]), int(kw.get("sh_degree", 0)),
         float(kw.get("scale_modifier", 1.0)), raw=bool(kw.get("raw", False)), antialiasing=bool(kw.get("antialiasing", False)),
-        filter_3d=kw.get("filter_3d"), contrib=kw.get("contrib"))
+        filter_3d=kw.get("filter_3d"), contrib=kw.get("contrib"), normals=bool(kw.get("normals", False)))
     sv = _StateView()
     _check(L.b200gs_describe_state(C.byref(st.prm), _ptr(st.geom), _ptr(st.binning), st.capacity, _ptr(st.image), C.byref(sv)),
            "describe_state")
@@ -820,17 +900,24 @@ def forward_with_state(**kw):
     dbits = state["recs"][:, 11].contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
     pl = state["point_list"].to(torch.int64) & 0xFFFFFFFF
     state["sorted_keys"] = ((state["sorted_tile_keys"].to(torch.int64) & 0xFFFFFFFF) << 32) | dbits[pl]
+    if st.normal is not None:
+        state["gauss_normals"] = st.gauss_normals.reshape(V * P, 4).clone()
+        return color, radii, depth, alpha, st.normal, state, st
     return color, radii, depth, alpha, state, st
 
 
-def forward_backward_with_state(g_color, g_depth, g_alpha, **kw):
+def forward_backward_with_state(g_color, g_depth, g_alpha, g_normal=None, **kw):
     """forward_with_state(**kw), then the backward of that same call for the image gradients g_color [V,3,H,W],
     g_depth [V,1,H,W], g_alpha [V,1,H,W].  Returns (color, radii, depth, alpha, state, sums): `sums` [V,P,12] float32 is
     the backward blend's ScreenGrad record of every (view, Gaussian) -- record v*P + g, in the format
     blend_sgrad_is_moments() names (csrc/common.cuh) -- copied out before the state buffers can be re-used.  Under
     torch.use_deterministic_algorithms(True) the deterministic backward runs, and `state` also holds its "patch_masks"
-    (uint8 per sorted instance, bit p = a partial for patch p of the instance's tile) and "n_partials"."""
-    color, radii, depth, alpha, state, st = forward_with_state(**kw)
+    (uint8 per sorted instance, bit p = a partial for patch p of the instance's tile) and "n_partials".
+    normals=True: the normal image is a fifth output after alpha, and g_normal [V,3,H,W] (None: no normal gradient) its
+    gradient; with g_normal, `state` also holds "normal_wn" [V,P,4], the sums Wn = sum w * dL/dN (DESIGN.md section 2)."""
+    outs = forward_with_state(**kw)
+    color, radii, depth, alpha = outs[:4]
+    state, st = outs[-2:]
     dev = kw["means3D"].device
     V, P = st.V, st.P
     t = lambda k: _f32c(kw.get(k), dev)
@@ -838,10 +925,15 @@ def forward_backward_with_state(g_color, g_depth, g_alpha, **kw):
     det_state = {}
     _backward_impl(st, t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"),
                    t("cov3D_precomp"), _f32c(kw["bg"], dev), t("viewmatrix").reshape(V, 4, 4), t("projmatrix").reshape(V, 4, 4),
-                   t("campos").reshape(V, 3), *g, det_state=det_state)
+                   t("campos").reshape(V, 3), *g, det_state=det_state,
+                   g_normal=None if g_normal is None else _f32c(g_normal, dev).reshape(V, 3, st.H, st.W))
     state.update(det_state)
+    if st.normal_wn is not None:
+        state["normal_wn"] = st.normal_wn.clone()
     nbytes = V * P * 48
     sums = st.scratch[:nbytes].view(torch.float32).reshape(V, P, 12).clone()
+    if st.normal is not None:
+        return color, radii, depth, alpha, st.normal, state, sums
     return color, radii, depth, alpha, state, sums
 
 

@@ -14,6 +14,7 @@ from __future__ import annotations
 import math
 
 import torch
+import torch.nn.functional as F
 
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, rasterize_views
 
@@ -24,6 +25,14 @@ class PipelineParams:
     compute_cov3D_python = False
     debug = False
     antialiasing = False  # the screen-space mip filter (rasterizer.rasterize_views); the name upstream 3DGS gives it
+
+
+def comp_normal(normal, alpha):
+    """threestudio's normal map from the rasteriser's normal image: (F.normalize(N) + 1) / 2 * alpha, channels last.
+    normal [...,3,H,W] (rasterize_views(normals=True)), alpha [...,1,H,W]; returns [...,H,W,3] in [0, 1] for alpha in [0, 1].
+    A pixel where nothing blended has N = 0, which F.normalize keeps at 0 (so it becomes alpha / 2 = 0 there)."""
+    n = F.normalize(normal, dim=-3)
+    return ((n + 1.0) * 0.5 * alpha).movedim(-3, -1)
 
 
 def _raw_tensors(pc):
@@ -37,7 +46,7 @@ def _raw_tensors(pc):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, fused_activations=False, filter_3d=None,
-           absgrad=False):
+           absgrad=False, normals=False):
     """fused_activations=True (optional fast path, SURVEY.md 8f-1): instead of calling the getters (sigmoid / exp /
     F.normalize: three kernels + autograd nodes per view, gaussian_model.py:95-118) the raw parameter tensors go straight
     to the rasteriser, which applies the activations and their Jacobians inside its kernels.  Same dict, same gradients
@@ -46,7 +55,9 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
     rasterize_views (GaussianRasterizer keeps upstream's surface, which has no such input).
     absgrad=True: the dict also holds "viewspace_points_abs" [P,3], whose .grad the backward fills with the absolute
     screen-space gradient (rasterizer.rasterize_views, means2D_abs), the densification statistic that does not cancel; the
-    call then goes through rasterize_views as with filter_3d."""
+    call then goes through rasterize_views as with filter_3d.
+    normals=True: the dict also holds "normal_3dgs" [3,H,W], the differentiable normal image (rasterize_views' normals=True),
+    through rasterize_views as with filter_3d."""
     aa = bool(getattr(pipe, "antialiasing", False))
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
@@ -72,26 +83,30 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
         colors = override_color
     raw = _raw_tensors(pc) if fused_activations else None
     m2d_abs = extra["viewspace_points_abs"][None] if absgrad else None
-    if raw is None and (filter_3d is not None or absgrad):
-        image, radii, depth, alpha = rasterize_views(
+    if raw is None and (filter_3d is not None or absgrad or normals):
+        outs = rasterize_views(
             means3D=xyz, opacities=pc.get_opacity, viewmatrices=viewpoint_camera.world_view_transform[None],
             projmatrices=viewpoint_camera.full_proj_transform[None], camposs=viewpoint_camera.camera_center[None],
             tanfovx=[settings.tanfovx], tanfovy=[settings.tanfovy], image_height=settings.image_height, image_width=settings.image_width,
             bg=bg_color, sh_degree=pc.active_sh_degree, shs=shs, colors_precomp=colors, scales=pc.get_scaling,
             rotations=pc.get_rotation, means2D=screenspace_points[None], scale_modifier=scaling_modifier, antialiasing=aa,
-            filter_3d=filter_3d, means2D_abs=m2d_abs)
-        image, radii, depth, alpha = image[0], radii[0], depth[0], alpha[0]
+            filter_3d=filter_3d, means2D_abs=m2d_abs, normals=normals)
+        image, radii, depth, alpha = outs[0][0], outs[1][0], outs[2][0], outs[3][0]
+        if normals:
+            extra["normal_3dgs"] = outs[4][0]
         return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
                 "depth_3dgs": depth, "alpha_3dgs": alpha, **extra}
     if raw is not None:
         op, sc, rot = raw[0], raw[1], raw[2]
-        image, radii, depth, alpha = rasterize_views(
+        outs = rasterize_views(
             means3D=xyz, opacities=op, viewmatrices=viewpoint_camera.world_view_transform[None], projmatrices=viewpoint_camera.full_proj_transform[None],
             camposs=viewpoint_camera.camera_center[None], tanfovx=[settings.tanfovx], tanfovy=[settings.tanfovy], image_height=settings.image_height,
             image_width=settings.image_width, bg=bg_color, sh_degree=pc.active_sh_degree, shs=shs, colors_precomp=colors, scales=sc, rotations=rot,
             means2D=screenspace_points[None], scale_modifier=scaling_modifier, raw=True, antialiasing=aa, filter_3d=filter_3d,
-            means2D_abs=m2d_abs)
-        image, radii, depth, alpha = image[0], radii[0], depth[0], alpha[0]
+            means2D_abs=m2d_abs, normals=normals)
+        image, radii, depth, alpha = outs[0][0], outs[1][0], outs[2][0], outs[3][0]
+        if normals:
+            extra["normal_3dgs"] = outs[4][0]
         return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
                 "depth_3dgs": depth, "alpha_3dgs": alpha, **extra}
     image, radii, depth, alpha = rasterizer(means3D=xyz, means2D=screenspace_points, shs=shs, colors_precomp=colors,
@@ -124,14 +139,16 @@ class _StackSinks(torch.autograd.Function):
         return (None, *g.unbind(0))
 
 
-def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False, filter_3d=None, absgrad=False):
+def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False, filter_3d=None, absgrad=False, normals=False):
     """All cameras share image size.  Returns the dict of `render` with a leading view axis:
     render [V,3,H,W], depth_3dgs/alpha_3dgs [V,1,H,W], radii [V,P], viewspace_points [V,P,3] (its .grad is [V,P,3]),
     plus viewspace_point_list: V leaf tensors [P,3] whose .grad backward fills -- what the reference's
     `self.viewspace_point_list` holds (GaussianDreamer.py:242-250) and on_before_optimizer_step sums (:385-387).
     antialiasing, filter_3d: the screen-space mip filter and the 3D smoothing filter, as `rasterizer.rasterize_views`.
     absgrad=True: also viewspace_points_abs [V,P,3], whose .grad is the absolute screen-space gradient (`rasterize_views`'
-    means2D_abs) -- the densification statistic that does not cancel."""
+    means2D_abs) -- the densification statistic that does not cancel.
+    normals=True: also normal_3dgs [V,3,H,W] (rasterize_views' normal image) and comp_normal [V,H,W,3], threestudio's normal
+    map of it (`comp_normal`), both differentiable."""
     xyz = pc.get_xyz
     V = len(cameras)
     vm, pm, cp, tanx, tany = stack_cameras(cameras, xyz.device)
@@ -145,11 +162,15 @@ def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False
     extra = {}
     if absgrad:
         extra["viewspace_points_abs"] = torch.zeros(V, xyz.shape[0], 3, dtype=torch.float32, device=xyz.device, requires_grad=True)
-    image, radii, depth, alpha = rasterize_views(
+    outs = rasterize_views(
         means3D=xyz, opacities=pc.get_opacity, viewmatrices=vm, projmatrices=pm, camposs=cp, tanfovx=tanx, tanfovy=tany,
         image_height=int(cameras[0].image_height), image_width=int(cameras[0].image_width), bg=bg_color,
         sh_degree=pc.active_sh_degree, shs=pc.get_features, scales=pc.get_scaling, rotations=pc.get_rotation,
         means2D=screenspace_points, scale_modifier=scaling_modifier, antialiasing=antialiasing, filter_3d=filter_3d,
-        means2D_abs=extra.get("viewspace_points_abs"))
+        means2D_abs=extra.get("viewspace_points_abs"), normals=normals)
+    image, radii, depth, alpha = outs[:4]
+    if normals:
+        extra["normal_3dgs"] = outs[4]
+        extra["comp_normal"] = comp_normal(outs[4], alpha)
     return {"render": image, "viewspace_points": screenspace_points, "viewspace_point_list": sinks, "visibility_filter": radii > 0,
             "radii": radii, "depth_3dgs": depth, "alpha_3dgs": alpha, **extra}

@@ -283,6 +283,103 @@ int b200gs_forward_contrib_opts(const b200gs_params *prm, const b200gs_render_op
                                 int64_t *num_rendered, uint64_t *weight_sum, uint32_t *weight_max, uint32_t *touches,
                                 void *stream);
 
+/* ---- normal maps: each Gaussian's shortest-axis normal blended like its colour (additive to ABI 4) ---------------------
+ * For view v and Gaussian g (DESIGN.md section 2):
+ *   axis    k = argmin of the activated scales s (after exp for raw parameters; before scale_modifier and the 3D filter,
+ *           which leave the argmin unchanged in exact arithmetic); on a tie the lowest index wins.
+ *   normal  n = column k of R(q), q the rotation as the covariance uses it (after the in-kernel normalise for raw), formed
+ *           with the covariance's own float operations; not renormalised.
+ *   flip    d = n . (campos_v - mean_{v,g}) as fmul, fma, fma over components 0, 1, 2 of fsub(campos, mean); if d < 0, n
+ *           becomes -n (it faces the camera).  mean is the per-view position with means3D_per_view.  A NaN d keeps the sign.
+ *   image   out_normal[v,c,p] = sum over the blends of pixel p of w n_c, accumulated as N_c = fma(n_c, w, N_c) with the
+ *           colour's w = alpha * T and order.  No background term: [V,3,H,W], world space, unnormalised, 0 where nothing
+ *           blends.
+ *   grads   dL/dN enters dL/dalpha as cg += n . dL/dN.  Wn = sum w dL/dN per (view, Gaussian) is dL/dn; times the flip sign,
+ *           through d(column k of R)/dq (and the normalise Jacobian for raw), it is ADDED to dL_drots.  Scales, means and
+ *           campos get no gradient through n (the argmin and the flip are piecewise constant), only the alpha-path terms.
+ * Colour, depth, alpha, radii and the state buffers are byte-identical to the call without normals, and the deterministic
+ * partial count is unchanged.  cov3D_precomp has no axis: B200GS_E_ARGS.  The classic comparator and the bulk-copy build
+ * return B200GS_E_UNSUPPORTED.
+ *   struct_bytes   sizeof(b200gs_normals_io) (a smaller value is B200GS_E_ARGS)
+ *   gauss_normals  [V*P] x 16 B device workspace, 16-byte aligned: the forward writes (sign n, sign) of every (view, Gaussian);
+ *                  the backward reads it, so it must survive from the forward to its backward like the state buffers
+ *   out_normal     [V,3,H,W] (forward output)
+ *   dL_dnormal     [V,3,H,W] (backward input); NULL = zero: the backward is then exactly the call without normals
+ *   normal_wn      [V*P] x 16 B device workspace, 16-byte aligned (backward with dL_dnormal): the Wn sums
+ *   nrm_partials   deterministic backward with dL_dnormal: nrm_partials_bytes >= 16 * partial_capacity bytes, 16-byte
+ *                  aligned, one float4 per partial at its slot (det_buf's layout and size do not change)
+ * The backward forms take the argument lists of b200gs_backward_opts, b200gs_backward_deterministic_opts and the two absgrad
+ * forms, with the io struct after opts. */
+typedef struct b200gs_normals_io {
+    int32_t struct_bytes;
+    float *gauss_normals;
+    float *out_normal;
+    const float *dL_dnormal;
+    float *normal_wn;
+    void *nrm_partials;
+    size_t nrm_partials_bytes;
+} b200gs_normals_io;
+int b200gs_forward_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+                                const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                                const float *scales, const float *rotations, const float *cov3D_precomp,
+                                const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
+                                void *geom_buf, size_t geom_bytes,
+                                void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
+                                void *image_buf, size_t image_bytes,
+                                int64_t *num_rendered, void *stream);
+int b200gs_backward_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+                                 const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                                 const float *scales, const float *rotations, const float *cov3D_precomp,
+                                 const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                 const int32_t *radii,
+                                 const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                 const void *image_buf, int64_t num_rendered,
+                                 const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                 float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+                                 float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                 void *scratch, size_t scratch_bytes, void *stream);
+int b200gs_backward_deterministic_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                                               const b200gs_normals_io *nrm,
+                                               const float *means3D, const float *shs, const float *colors_precomp,
+                                               const float *opacities, const float *scales, const float *rotations,
+                                               const float *cov3D_precomp, const float *bg, const float *viewmatrix,
+                                               const float *projmatrix, const float *campos, const int32_t *radii,
+                                               const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                               const void *image_buf, int64_t num_rendered,
+                                               const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                               float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                                               float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                               void *scratch, size_t scratch_bytes,
+                                               void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials,
+                                               void *stream);
+int b200gs_backward_absgrad_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+                                         const float *means3D, const float *shs, const float *colors_precomp,
+                                         const float *opacities, const float *scales, const float *rotations,
+                                         const float *cov3D_precomp, const float *bg, const float *viewmatrix,
+                                         const float *projmatrix, const float *campos, const int32_t *radii,
+                                         const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                         const void *image_buf, int64_t num_rendered,
+                                         const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                         float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                                         float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                         float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream);
+int b200gs_backward_deterministic_absgrad_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                                                       const b200gs_normals_io *nrm,
+                                                       const float *means3D, const float *shs, const float *colors_precomp,
+                                                       const float *opacities, const float *scales, const float *rotations,
+                                                       const float *cov3D_precomp, const float *bg, const float *viewmatrix,
+                                                       const float *projmatrix, const float *campos, const int32_t *radii,
+                                                       const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                                       const void *image_buf, int64_t num_rendered,
+                                                       const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                                       float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                                                       float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                                       float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes,
+                                                       void *det_buf, size_t det_bytes, int64_t partial_capacity,
+                                                       int64_t *n_partials, void *abs_partials, size_t abs_partials_bytes,
+                                                       void *stream);
+
 /* ---- 3D smoothing filter: per-Gaussian maximal sampling rate over a camera set (Mip-Splatting's 3D filter) ------------
  * For each of the n_views cameras (viewmatrix [n_views,16] device, tanfovx / tanfovy host [n_views], shared H x W), with
  * (tx, ty, tz) the preprocess's view-space position and fx = W / (2 tanfovx), fy = H / (2 tanfovy): Gaussian k is in view
