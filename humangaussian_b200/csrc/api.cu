@@ -816,6 +816,42 @@ int b200gs_densify_move(int32_t role, int32_t P, int32_t row_floats, const int32
     return B200GS_OK;
 }
 
+int b200gs_mcmc_noise(int32_t P, float *xyz, const float *scaling_raw, const float *rotation_raw, const float *opacity_raw,
+                      const float *eta, float noise_scale, float k, float t, void *stream)
+{
+    if (P < 0 || !xyz || !scaling_raw || !rotation_raw || !opacity_raw || !eta) return B200GS_E_ARGS;
+    if (P == 0) return B200GS_OK;
+    launch_mcmc_noise(P, xyz, scaling_raw, rotation_raw, opacity_raw, eta, noise_scale, k, t, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "mcmc_noise launch");
+    return B200GS_OK;
+}
+
+int b200gs_mcmc_ratio(int32_t P, const int32_t *counts, const float *opacity_raw, const float *scaling_raw, float *new_opacity,
+                      float *new_scaling, void *stream)
+{
+    if (P < 0 || !counts || !opacity_raw || !scaling_raw || !new_opacity || !new_scaling) return B200GS_E_ARGS;
+    if (P == 0) return B200GS_OK;
+    launch_mcmc_ratio(P, counts, opacity_raw, scaling_raw, new_opacity, new_scaling, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "mcmc_ratio launch");
+    return B200GS_OK;
+}
+
+int b200gs_mcmc_move(int32_t role, int32_t P, int32_t P_new, int32_t row_floats, const int32_t *map, const int32_t *counts,
+                     const float *src, float *dst, const float *new_opacity, const float *new_scaling, void *stream)
+{
+    if (role < B200GS_MCMC_ROLE_COPY || role > B200GS_MCMC_ROLE_MOMENT || P < 1 || P_new < 0 || row_floats < 1) return B200GS_E_ARGS;
+    if (!map || !counts || !src || (P_new > 0 && !dst)) return B200GS_E_ARGS;
+    if (role == B200GS_MCMC_ROLE_OPACITY && (row_floats != 1 || !new_opacity)) return B200GS_E_ARGS;
+    if (role == B200GS_MCMC_ROLE_SCALING && (row_floats != 3 || !new_scaling)) return B200GS_E_ARGS;
+    if (P_new == 0) return B200GS_OK;
+    launch_mcmc_move(role, P_new, row_floats, map, counts, src, dst, new_opacity, new_scaling, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "mcmc_move launch");
+    return B200GS_OK;
+}
+
 int b200gs_adam_packed(const b200gs_adam_cfg *cfg, float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
                        void *stream)
 {

@@ -67,6 +67,19 @@ __device__ __forceinline__ float gs_dot3(float a0, float a1, float a2, float b0,
     return ffma(a2, b2, a);
 }
 
+// torch.sigmoid in float32, as the densify plan and the MCMC kernels (densify.cu, mcmc.cu) evaluate it
+__device__ __forceinline__ float gs_sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }
+// F.normalize(dim=1) of a quaternion as torch's CUDA kernels evaluate it in float32: x / max(||x||, 1e-12) (preprocess.cu,
+// mcmc.cu); returns the clamped norm
+__device__ __forceinline__ float gs_normalize4(float *q)
+{
+    const float n2 = fadd(fadd(fmul(q[0], q[0]), fmul(q[1], q[1])), fadd(fmul(q[2], q[2]), fmul(q[3], q[3])));
+    const float n = fmaxf(fsqrt(n2), 1e-12f);
+#pragma unroll
+    for (int k = 0; k < 4; k++) q[k] = fdiv(q[k], n);
+    return n;
+}
+
 // R(q) of a quaternion q = (r, x, y, z), row-major, in the pinned operation order the covariance uses (preprocess.cu,
 // build_cov3d); column k is the Gaussian's k-th axis, the one the normals (normals.cu) take
 __device__ __forceinline__ void gs_rotmat(const float *q, float R[3][3])

@@ -26,8 +26,6 @@ constexpr int DB = 256; // threads per block, one Gaussian per thread
 
 struct Flags { bool keep, clone, split_sel, split_kept; };
 
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
-
 __device__ __forceinline__ Flags classify(const DensifyCfg &c, int i, const float *__restrict__ accum, const float *__restrict__ denom,
                                            const float *__restrict__ opacity, const float *__restrict__ scaling)
 {
@@ -39,7 +37,7 @@ __device__ __forceinline__ Flags classify(const DensifyCfg &c, int i, const floa
     }
     const float e0 = expf(scaling[3 * i]), e1 = expf(scaling[3 * i + 1]), e2 = expf(scaling[3 * i + 2]);
     const float smax = fmaxf(e0, fmaxf(e1, e2));
-    const bool low_op = sigmoidf_(opacity[i]) < c.min_opacity;
+    const bool low_op = gs_sigmoidf(opacity[i]) < c.min_opacity;
     if (c.mode == 1) { // prune_only (gaussian_model.py:423-430)
         f.keep = !(low_op || smax > c.big_ws_thresh);
         f.clone = f.split_sel = f.split_kept = false;

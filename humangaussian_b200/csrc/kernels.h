@@ -217,6 +217,17 @@ void launch_densify_plan(const DensifyCfg &c, int P, const float *accum, const f
 void launch_densify_move(int role, int P, int rf, const int *plan, const float *src, float *dst, int n_split, int S_sel, int S_kept,
                          const float *rotation, const float *scaling, const float *noise, cudaStream_t st);
 
+// MCMC densification (mcmc.cu; DESIGN.md section 2).  Raw parameters; counts [P] = times each row was drawn as a source.
+// xyz [P,3] += the opacity-gated position noise of the eta [P,3] draws
+void launch_mcmc_noise(int P, float *xyz, const float *scaling, const float *rotation, const float *opacity, const float *eta,
+                       float noise_scale, float k, float t, cudaStream_t st);
+// rows with counts > 0: new_opacity [P] / new_scaling [P,3] = the split ratio's raw values (other rows are not written)
+void launch_mcmc_ratio(int P, const int *counts, const float *opacity, const float *scaling, float *new_opacity, float *new_scaling,
+                       cudaStream_t st);
+// dst[i] = src[map[i]] for i < P_new (role B200GS_MCMC_ROLE_*: reset rows take the ratio's values or zero moments)
+void launch_mcmc_move(int role, int P_new, int rf, const int *map, const int *counts, const float *src, float *dst,
+                      const float *new_opacity, const float *new_scaling, cudaStream_t st);
+
 // Adam over the packed buffer (optim.cu).  Groups in the reference's order (gaussian_model.py:156-163).
 enum { ADAM_GROUP_XYZ = 0, ADAM_GROUP_F_DC = 1, ADAM_GROUP_F_REST = 2, ADAM_GROUP_OPACITY = 3, ADAM_GROUP_SCALING = 4,
        ADAM_GROUP_ROTATION = 5 };

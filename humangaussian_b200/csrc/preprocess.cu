@@ -81,16 +81,8 @@ __device__ __forceinline__ float gs_filter3d(float *s, float v, float *t, float 
     return fsqrt(fmul(fmul(r[0], r[1]), r[2]));
 }
 
-// torch.sigmoid / F.normalize(dim=1) as torch's CUDA kernels evaluate them in float32
+// torch.sigmoid as torch's CUDA kernels evaluate it in float32 (F.normalize: gs_normalize4, common.cuh)
 __device__ __forceinline__ float gs_sigmoid(float x) { return fdiv(1.0f, fadd(1.0f, expf(-x))); }
-__device__ __forceinline__ float gs_normalize4(float *q)
-{
-    const float n2 = fadd(fadd(fmul(q[0], q[0]), fmul(q[1], q[1])), fadd(fmul(q[2], q[2]), fmul(q[3], q[3])));
-    const float n = fmaxf(fsqrt(n2), 1e-12f);
-#pragma unroll
-    for (int k = 0; k < 4; k++) q[k] = fdiv(q[k], n);
-    return n;
-}
 
 // ------------------------------------------------------------------------------------------------
 // F1.  One thread per Gaussian; the thread loads its attributes ONCE (128-bit loads for the SH block when the

@@ -217,16 +217,25 @@ def _run_packed(cfg: _Cfg, opt: torch.optim.Optimizer, stats: DensifyStats, nois
         if state:
             new_moments = tuple(remap(state[k], (ROLE_MOMENT,) * 5) for k in ("exp_avg", "exp_avg_sq"))
         new_stats = s.new_stats(stats)
-    # what _prune_optimizer / cat_tensors_to_optimizer do (gaussian_model.py:284-341): new leaf, moved moments, same step
+    install_packed(opt, new_flat, new_moments, s.P_new)
+    stats.xyz_gradient_accum, stats.denom, stats.max_radii2D = new_stats.xyz_gradient_accum, new_stats.denom, new_stats.max_radii2D
+    return s.P_new
+
+
+def install_packed(opt: torch.optim.Optimizer, new_flat: torch.Tensor, new_moments, P_new: int) -> None:
+    """What _prune_optimizer / cat_tensors_to_optimizer do (gaussian_model.py:284-341), for an `optim.PackedAdam`: `new_flat`
+    becomes the parameter leaf, `new_moments` (exp_avg, exp_avg_sq) in the same layout, or None when the optimiser has no
+    state yet, its moments, and group["P"] = P_new.  The step count is kept."""
+    group = opt.param_groups[0]
+    old = group["params"][0]
+    state = opt.state.get(old)
     leaf = torch.nn.Parameter(new_flat) if isinstance(old, torch.nn.Parameter) else new_flat.requires_grad_(True)
     group["params"][0] = leaf
-    group["P"] = s.P_new
+    group["P"] = P_new
     opt.state.pop(old, None)
     if new_moments is not None:
         state["exp_avg"], state["exp_avg_sq"] = new_moments
         opt.state[leaf] = state
-    stats.xyz_gradient_accum, stats.denom, stats.max_radii2D = new_stats.xyz_gradient_accum, new_stats.denom, new_stats.max_radii2D
-    return s.P_new
 
 
 def densify_and_prune_packed(opt: torch.optim.Optimizer, stats: DensifyStats, max_grad: float, min_opacity: float, extent: float,

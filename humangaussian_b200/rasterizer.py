@@ -105,7 +105,8 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_backward_deterministic_opts", "b200gs_sampling_rate", "b200gs_backward_absgrad_opts",
            "b200gs_backward_deterministic_absgrad_opts", "b200gs_forward_contrib_opts", "b200gs_prune_plan",
            "b200gs_forward_normals_opts", "b200gs_backward_normals_opts", "b200gs_backward_deterministic_normals_opts",
-           "b200gs_backward_absgrad_normals_opts", "b200gs_backward_deterministic_absgrad_normals_opts"]
+           "b200gs_backward_absgrad_normals_opts", "b200gs_backward_deterministic_absgrad_normals_opts", "b200gs_mcmc_noise",
+           "b200gs_mcmc_ratio", "b200gs_mcmc_move"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -187,6 +188,12 @@ def load_library():
     L.b200gs_prune_plan.argtypes = [i32, vp, vp, vp, vp, sz, vp]
     L.b200gs_densify_move.restype = C.c_int
     L.b200gs_densify_move.argtypes = [i32, i32, i32, vp, C.POINTER(i32), i32, vp, vp, vp, vp, vp, vp]
+    L.b200gs_mcmc_noise.restype = C.c_int
+    L.b200gs_mcmc_noise.argtypes = [i32, vp, vp, vp, vp, vp, C.c_float, C.c_float, C.c_float, vp]
+    L.b200gs_mcmc_ratio.restype = C.c_int
+    L.b200gs_mcmc_ratio.argtypes = [i32, vp, vp, vp, vp, vp, vp]
+    L.b200gs_mcmc_move.restype = C.c_int
+    L.b200gs_mcmc_move.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     L.b200gs_adam_packed.restype = C.c_int
     L.b200gs_adam_packed.argtypes = [vp, vp, vp, vp, vp, vp]
     L.b200gs_last_cuda_error.restype = C.c_char_p

@@ -465,6 +465,37 @@ int b200gs_densify_move(int32_t role, int32_t P, int32_t row_floats, const int32
                         int32_t n_split, const float *src, float *dst, const float *rotation_raw, const float *scaling_raw,
                         const float *noise, void *stream);
 
+/* ---- MCMC densification (3DGS-MCMC, Kheradmand et al., NeurIPS 2024): relocation of dead Gaussians, growth to a budget
+ * and position noise, in place of the gradient-threshold rule above.  Parameters are the RAW optimiser arrays
+ * (opacity logits [P], log-scales [P,3], un-normalised quaternions [P,4]); any row stride-exact fp32 array works, so the
+ * packed buffer's field views and separate tensors both do.  sigma(x) = 1/(1+expf(-x)) in float32.
+ *
+ * b200gs_mcmc_noise: the per-step exploration term, one thread per Gaussian, one launch, no host sync:
+ *   xyz_i += noise_scale * sigma(-k (sigma(opacity_i) - t)) * Sigma_i eta_i,   Sigma_i = R(q^_i) diag(exp(2 scaling_i)) R(q^_i)^T
+ *   q^ = q / max(||q||, 1e-12) and R as the preprocess forms them; eta [P,3] standard-normal draws (an input);
+ *   noise_scale = lambda_noise * lr_xyz (the lr of the step just taken).  Only xyz [P,3] is written. */
+int b200gs_mcmc_noise(int32_t P, float *xyz, const float *scaling_raw, const float *rotation_raw, const float *opacity_raw,
+                      const float *eta, float noise_scale, float k, float t, void *stream);
+
+/* b200gs_mcmc_ratio: for every row s with c = counts[s] > 0 (s was drawn c times as a source; counts [P] int32, device),
+ * the raw opacity and log-scales that all n = min(c+1, 51) members of s (s and its copies) take, in float64, rounded once:
+ *   o = sigma(opacity_s);  o' = clamp(1 - (1-o)^(1/n), 0.005, 1 - 2^-23);
+ *   D = sum_{k=0}^{n-1} C(n,k+1) (-1)^k o'^(k+1) / sqrt(k+1);
+ *   new_opacity[s] = log(o' / (1-o')),  new_scaling[s,j] = log(exp(scaling_s,j) o / D).
+ * new_opacity [P], new_scaling [P,3]: rows with counts == 0 are not written. */
+int b200gs_mcmc_ratio(int32_t P, const int32_t *counts, const float *opacity_raw, const float *scaling_raw, float *new_opacity,
+                      float *new_scaling, void *stream);
+
+/* b200gs_mcmc_move: gathers one [P,row_floats] array into [P_new,row_floats]: dst[i] = src[map[i]] (map [P_new] int32 in
+ * [0,P), device).  Row i is reset iff counts[map[i]] > 0; there the role decides:  */
+enum { B200GS_MCMC_ROLE_COPY = 0,    /* always the source row (xyz, rotation, SH) */
+       B200GS_MCMC_ROLE_OPACITY = 1, /* new_opacity[map[i]] (row_floats 1) */
+       B200GS_MCMC_ROLE_SCALING = 2, /* new_scaling[map[i]] (row_floats 3) */
+       B200GS_MCMC_ROLE_MOMENT = 3 };/* zero (Adam exp_avg / exp_avg_sq) */
+/* Relocation: map = identity except map[dead_j] = sample_j; growth: map = identity ++ samples.  dst must not alias src. */
+int b200gs_mcmc_move(int32_t role, int32_t P, int32_t P_new, int32_t row_floats, const int32_t *map, const int32_t *counts,
+                     const float *src, float *dst, const float *new_opacity, const float *new_scaling, void *stream);
+
 /* ---- Adam over the packed parameter buffer (the reference's optimiser, gaussian_model.py:156-165) ------------------
  * One step of torch.optim.Adam (amsgrad=False, weight_decay=0, maximize=False) over the flat fp32 buffer
  * [xyz 3P | scaling 3P | rotation 4P | opacity P | sh 3*sh_coeffs*P] that the packed forward reads and the packed backward
