@@ -30,6 +30,11 @@ constexpr int D_BITS = 8, D_IPT = 12, D_TILE = THREADS * D_IPT;   // depth sort:
 constexpr int T_BITS = 9, T_IPT = 12, T_TILE = THREADS * T_IPT;   // tile sort: u32 keys
 constexpr int MAXP = 5;
 constexpr int SCAN_TILE = THREADS * SCAN_IPT;
+// The depth order is read from order_in after the pre-sort by the deterministic backward's plan (api.cu, backward_impl)
+// and by b200gs_describe_state: right only when the ping-pong passes end in the buffer they started from.
+static_assert(((32 + D_BITS - 1) / D_BITS) % 2 == 0,
+              "odd depth pre-sort pass count: the depth order ends in BinLayout::order, so backward_impl's pa.order and "
+              "b200gs_describe_state's depth_order (api.cu) must read it there instead of order_in");
 
 // scratch of one radix sort: digit totals + the [digit][CTA] count matrix (re-used by every pass)
 static size_t sort_scratch_bytes(int64_t n, int tile, int bins)

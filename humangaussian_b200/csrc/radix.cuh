@@ -249,7 +249,8 @@ __global__ void __launch_bounds__(THREADS) lookback_scan_kernel(const Load load,
 {
     // status: bit 63 = prefix ready, bit 62 = aggregate ready, low 56 bits = value (the exact running sum: fewer than 2^32
     // entries of at most 2^24 each cannot reach 2^56).  out[] keeps the low 32 bits; the callers check the exact total before
-    // anything relies on the 32-bit values (api.cu).
+    // anything relies on the 32-bit values (api.cu).  One CTA's own aggregate is summed in 32 bits, so it is exact while
+    // TILE entries stay below 2^32 together: tiles_touched up to 2^21 tiles per view (about 512 Mpx images).
     constexpr int TILE = THREADS * SCAN_IPT;
     __shared__ uint32_t s_bid, s_wsum[WARPS];
     __shared__ uint64_t s_excl;
