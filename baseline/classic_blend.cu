@@ -183,6 +183,10 @@ void launch_absgrad_out(int64_t, int, int, const int32_t *, const GeomRec *, con
 int blend_has_normals() { return 0; }
 void launch_blend_fwd_nrm(const BlendArgs &, const float4 *, float *, cudaStream_t) {}
 void launch_blend_bwd_nrm(const BlendBwdArgs &, const DetFlush *, bool, const NrmBwd &, cudaStream_t) {}
+// nor the geometry outputs: the geometry entry points return B200GS_E_UNSUPPORTED before these would run
+int blend_has_geometry() { return 0; }
+void launch_blend_fwd_geo(const BlendArgs &, const float4 *, float *, const GeoFwd &, cudaStream_t) {}
+void launch_blend_bwd_geo(const BlendBwdArgs &, const DetFlush *, bool, const NrmBwd *, const GeoBwd &, cudaStream_t) {}
 __global__ void classic_exp_kernel(const float *x, float *y, int64_t n)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -123,6 +123,14 @@ static int check_normals_io(const b200gs_normals_io *n, const float *cov3D_preco
     if (((uintptr_t)n->gauss_normals) & 15) return B200GS_E_BUFFER;
     return B200GS_OK;
 }
+// b200gs_geometry_io: the fields every geometry call reads (the build, the struct, the median-position workspace)
+static int check_geometry_io(const b200gs_geometry_io *g)
+{
+    if (!blend_has_geometry()) return B200GS_E_UNSUPPORTED;
+    if (!g || g->struct_bytes < (int32_t)sizeof(b200gs_geometry_io) || !g->median_pos) return B200GS_E_ARGS;
+    if (((uintptr_t)g->median_pos) & 3) return B200GS_E_BUFFER;
+    return B200GS_OK;
+}
 static NormalArgs normal_args(const b200gs_params *prm, const float *means3D, const float *scales, const float *rotations,
                               const float *campos)
 {
@@ -140,7 +148,7 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
                         const float *campos, float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf,
                         size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf,
                         size_t image_bytes, int64_t *num_rendered, void *stream, const ContribOut *contrib,
-                        const b200gs_normals_io *nrm = nullptr)
+                        const b200gs_normals_io *nrm = nullptr, const b200gs_geometry_io *geo = nullptr)
 {
     bool aa = false;
     const float *f3d = nullptr;
@@ -153,6 +161,11 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
         rc = check_normals_io(nrm, cov3D_precomp);
         if (rc) return rc;
         if (!nrm->out_normal) return B200GS_E_ARGS;
+    }
+    if (geo) {
+        rc = check_geometry_io(geo);
+        if (rc) return rc;
+        if (!geo->out_median || !geo->out_depth2) return B200GS_E_ARGS;
     }
     if (!means3D || !opacities || !bg || !viewmatrix || !projmatrix || !campos || !out_color || !out_depth || !out_alpha ||
         !radii || !geom_buf || !binning_buf || !image_buf || !num_rendered)
@@ -249,6 +262,9 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
     {
         StageTimer t(B200GS_STAGE_BLEND_FWD, st);
         if (contrib) launch_blend_fwd_contrib(b, *contrib, st);
+        else if (geo)
+            launch_blend_fwd_geo(b, nrm ? (const float4 *)nrm->gauss_normals : nullptr, nrm ? nrm->out_normal : nullptr,
+                                 GeoFwd{geo->out_median, geo->out_depth2, geo->median_pos}, st);
         else if (nrm) launch_blend_fwd_nrm(b, (const float4 *)nrm->gauss_normals, nrm->out_normal, st);
         else launch_blend_fwd(b, st);
         g_launches += 1;
@@ -306,6 +322,20 @@ int b200gs_forward_normals_opts(const b200gs_params *prm, const b200gs_render_op
                         instance_capacity, image_buf, image_bytes, num_rendered, stream, nullptr, nrm);
 }
 
+int b200gs_forward_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+                                 const b200gs_geometry_io *geo, const float *means3D, const float *shs, const float *colors_precomp,
+                                 const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                 const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                 float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf,
+                                 size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
+                                 void *image_buf, size_t image_bytes, int64_t *num_rendered, void *stream)
+{
+    if (!geo) return B200GS_E_ARGS;
+    return forward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
+                        projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
+                        instance_capacity, image_buf, image_bytes, num_rendered, stream, nullptr, nrm, geo);
+}
+
 int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
                    const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
                    const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
@@ -334,11 +364,19 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
                          float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
                          size_t scratch_bytes, void *stream, bool det, void *det_buf, size_t det_bytes, int64_t partial_capacity,
                          int64_t *n_partials, bool absgrad = false, float *dL_dmeans2D_abs = nullptr, void *abs_partials = nullptr,
-                         size_t abs_partials_bytes = 0, const b200gs_normals_io *nio = nullptr)
+                         size_t abs_partials_bytes = 0, const b200gs_normals_io *nio = nullptr,
+                         const b200gs_geometry_io *gio = nullptr)
 {
     bool aa = false;
     const float *f3d = nullptr;
     if (absgrad && !blend_bwd_has_absgrad()) return B200GS_E_UNSUPPORTED;
+    // a geometry call without either geometry gradient is exactly the call without geometry
+    const b200gs_geometry_io *geo =
+        gio && gio->struct_bytes >= (int32_t)sizeof(b200gs_geometry_io) && !gio->dL_dmedian && !gio->dL_ddepth2 ? nullptr : gio;
+    if (geo) {
+        const int rc = check_geometry_io(geo);
+        if (rc) return rc;
+    }
     // a normals call without dL_dnormal is exactly the call without normals
     const b200gs_normals_io *nrm = nio && nio->struct_bytes >= (int32_t)sizeof(b200gs_normals_io) && !nio->dL_dnormal ? nullptr : nio;
     if (nrm) {
@@ -392,6 +430,7 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     if (!det && nrm) CK(cudaMemsetAsync(nrm->normal_wn, 0, (size_t)P * V * 16, st), "memset normal_wn");
     const NrmBwd nb{nrm ? (const float4 *)nrm->gauss_normals : nullptr, nrm ? nrm->dL_dnormal : nullptr,
                     nrm ? (float4 *)nrm->normal_wn : nullptr, nrm ? (float4 *)nrm->nrm_partials : nullptr};
+    const GeoBwd gbw{geo ? geo->dL_dmedian : nullptr, geo ? geo->dL_ddepth2 : nullptr, geo ? geo->median_pos : nullptr};
     BlendBwdArgs b;
     b.H = H; b.W = W; b.grid_x = gx; b.grid_y = gy; b.V = V; b.P = P;
     b.ranges = (const uint2 *)(bb + BL.ranges); b.point_list = (const uint32_t *)(bb + BL.vals_out);
@@ -403,7 +442,8 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     b.sgrad = scratch;
     if (!det) {
         StageTimer t(B200GS_STAGE_BLEND_BWD, st);
-        if (nrm) launch_blend_bwd_nrm(b, nullptr, absgrad, nb, st);
+        if (geo) launch_blend_bwd_geo(b, nullptr, absgrad, nrm ? &nb : nullptr, gbw, st);
+        else if (nrm) launch_blend_bwd_nrm(b, nullptr, absgrad, nb, st);
         else if (absgrad) launch_blend_bwd_abs(b, nullptr, st);
         else launch_blend_bwd(b, st);
     } else {
@@ -439,7 +479,8 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
         float2 *abs_p = absgrad ? (float2 *)abs_partials : nullptr;
         const DetFlush flush{pa.pm, pa.base, partials, abs_p};
         if (H_partials > 0) {
-            if (nrm) launch_blend_bwd_nrm(b, &flush, absgrad, nb, st);
+            if (geo) launch_blend_bwd_geo(b, &flush, absgrad, nrm ? &nb : nullptr, gbw, st);
+            else if (nrm) launch_blend_bwd_nrm(b, &flush, absgrad, nb, st);
             else if (absgrad) launch_blend_bwd_abs(b, &flush, st);
             else launch_blend_bwd_det(b, flush, st);
         }
@@ -637,6 +678,41 @@ int b200gs_backward_deterministic_absgrad_normals_opts(const b200gs_params *prm,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
                          scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials, true,
                          dL_dmeans2D_abs, abs_partials, abs_partials_bytes, nrm);
+}
+
+// the geometry forms of the backward: nullable normals io and absgrad output, then the geometry io (include/b200gs.h)
+int b200gs_backward_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+    const b200gs_geometry_io *geo, const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+    const float *scales, const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix,
+    const float *projmatrix, const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf,
+    int64_t instance_capacity, const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth,
+    const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+    float *dL_dscales, float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream)
+{
+    if (!geo) return B200GS_E_ARGS;
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr, dL_dmeans2D_abs != nullptr, dL_dmeans2D_abs,
+                         nullptr, 0, nrm, geo);
+}
+
+int b200gs_backward_deterministic_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+    const b200gs_normals_io *nrm, const b200gs_geometry_io *geo, const float *means3D, const float *shs, const float *colors_precomp,
+    const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp, const float *bg,
+    const float *viewmatrix, const float *projmatrix, const float *campos, const int32_t *radii, const void *geom_buf,
+    const void *binning_buf, int64_t instance_capacity, const void *image_buf, int64_t num_rendered, const float *dL_dcolor,
+    const float *dL_ddepth, const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+    float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs, void *scratch,
+    size_t scratch_bytes, void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *abs_partials,
+    size_t abs_partials_bytes, void *stream)
+{
+    if (!geo) return B200GS_E_ARGS;
+    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
+                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
+                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
+                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials,
+                         dL_dmeans2D_abs != nullptr, dL_dmeans2D_abs, abs_partials, abs_partials_bytes, nrm, geo);
 }
 
 int b200gs_sampling_rate(int32_t P, int32_t n_views, const float *means3D, const float *viewmatrix, const float *tanfovx,

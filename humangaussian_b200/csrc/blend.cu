@@ -141,13 +141,22 @@ __device__ __forceinline__ void contrib_hit(bool touch, bool blend, float w, uin
     }
 }
 
+// Geometry outputs of a forward pixel (DESIGN.md section 2): the depth second moment, and the depth and 1-based list position
+// of the median entry (0 = none).
+struct GeoPixel {
+    float M2, med;
+    uint32_t mpos;
+};
+
 // CONTRIB: the contribution variant also folds the hit into the scores of Gaussian gid (contrib_hit); the pixel's update is
 // the same code.
 // NRM (normal maps, DESIGN.md section 2): the hit's normal n (its slab word ns) is accumulated as N_c = fma(n_c, w, N_c) under
 // the colour's predicate.
-template <bool CONTRIB, bool NRM = false>
+// GEO (geometry outputs, DESIGN.md section 2): M2 = fma(d*d, w, M2) under the colour's predicate, and a blend whose transmittance
+// before blending is > 0.5 becomes the median (the last such blend wins).
+template <bool CONTRIB, bool NRM = false, bool GEO = false>
 __device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float fpy, FwdPixel &p, uint32_t gid, const ContribOut &co,
-                                              const float4 *ns = nullptr, float *N = nullptr)
+                                              const float4 *ns = nullptr, float *N = nullptr, GeoPixel *gp = nullptr)
 {
     const float4 g0 = s[0], q1 = s[1], q2 = s[2];
     const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
@@ -169,25 +178,30 @@ __device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float 
         const float4 n = *ns;
         if (blend) { N[0] = ffma(n.x, w, N[0]); N[1] = ffma(n.y, w, N[1]); N[2] = ffma(n.z, w, N[2]); }
     }
+    if (GEO) { // (p.T is still the transmittance before this hit; a finished pixel's is <= 0)
+        if (blend) gp->M2 = ffma(fmul(q2.w, q2.w), w, gp->M2);
+        if (blend & (p.T > 0.5f)) { gp->med = q2.w; gp->mpos = __float_as_uint(g0.z); }
+    }
     p.T = blend ? test_T : (hit ? -fabsf(p.T) : p.T);
     if (CONTRIB) contrib_hit(hit & live, blend, w, gid, co);
 }
 
 // Blends the cnt hits staged in slab s, in order, two per iteration.  gids: the hits' Gaussian indices (CONTRIB only).
-// NRM: ns holds the hits' normals, N the pixel's three normal sums.
-template <bool CONTRIB, bool NRM = false>
+// NRM: ns holds the hits' normals, N the pixel's three normal sums.  GEO: gp is the pixel's geometry state.
+template <bool CONTRIB, bool NRM = false, bool GEO = false>
 __device__ __forceinline__ void fwd_blend_slab(const float4 *s, int cnt, float fpx, float fpy, FwdPixel &p, const uint32_t *gids,
-                                               const ContribOut &co, const float4 *ns = nullptr, float *N = nullptr)
+                                               const ContribOut &co, const float4 *ns = nullptr, float *N = nullptr,
+                                               GeoPixel *gp = nullptr)
 {
     const float4 *const end2 = s + 3 * (cnt & ~1);
 #pragma unroll 1
     for (; s != end2; s += 6) {
-        fwd_blend_hit<CONTRIB, NRM>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co, ns, N);
-        fwd_blend_hit<CONTRIB, NRM>(s + 3, fpx, fpy, p, CONTRIB ? gids[1] : 0u, co, NRM ? ns + 1 : ns, N);
+        fwd_blend_hit<CONTRIB, NRM, GEO>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co, ns, N, gp);
+        fwd_blend_hit<CONTRIB, NRM, GEO>(s + 3, fpx, fpy, p, CONTRIB ? gids[1] : 0u, co, NRM ? ns + 1 : ns, N, gp);
         if (CONTRIB) gids += 2;
         if (NRM) ns += 2;
     }
-    if (cnt & 1) fwd_blend_hit<CONTRIB, NRM>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co, ns, N);
+    if (cnt & 1) fwd_blend_hit<CONTRIB, NRM, GEO>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co, ns, N, gp);
 }
 
 // Writes the pixel's outputs (out-of-image pixels write nothing).
@@ -212,10 +226,12 @@ __device__ __forceinline__ void fwd_store_pixel(const BlendArgs &a, int v, int p
 // same code.
 // NRM (normal maps, DESIGN.md section 2): hit lanes also gather gauss_normals[record index] into the warp's 32-entry nrm_slabs
 // row, the pixel keeps three normal sums, and the pixel writes them to out_normal [V,3,H,W].
-template <bool CONTRIB, bool NRM = false>
+// GEO (geometry outputs, DESIGN.md section 2): the pixel keeps M2 and the median (GeoPixel) and writes them to geo's images and
+// median_pos.
+template <bool CONTRIB, bool NRM = false, bool GEO = false>
 __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gid_slabs)[32], const ContribOut &co,
                                                float4 (*nrm_slabs)[32] = nullptr, const float4 *gauss_normals = nullptr,
-                                               float *out_normal = nullptr)
+                                               float *out_normal = nullptr, const GeoFwd *geo = nullptr)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
 
@@ -243,6 +259,7 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
 
     FwdPixel p = {inside ? 1.0f : 0.0f, 0.f, 0.f, 0.f, 0.f, 0.f, 0u, 0u};
     float N[3] = {0.f, 0.f, 0.f};
+    GeoPixel gp = {0.f, 0.f, 0u};
 
     // software pipeline, two deep: while chunk c is blended the support boxes of chunk c+1 and the ids of chunk c+2
     // are in flight (the id -> record address dependency never sits on the critical path)
@@ -282,8 +299,8 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
             }
             __syncwarp();
             p.used = 0u;
-            fwd_blend_slab<CONTRIB, NRM>(slab, __popc(b), fpx, fpy, p, CONTRIB ? gid_slabs[warp] : nullptr, co,
-                                         NRM ? nrm_slabs[warp] : nullptr, N);
+            fwd_blend_slab<CONTRIB, NRM, GEO>(slab, __popc(b), fpx, fpy, p, CONTRIB ? gid_slabs[warp] : nullptr, co,
+                                              NRM ? nrm_slabs[warp] : nullptr, N, &gp);
             m = __reduce_or_sync(FULL, p.used);
             __syncwarp();
         }
@@ -295,6 +312,12 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
             const size_t HW = (size_t)a.H * a.W, pix = (size_t)py * a.W + px;
             float *on = out_normal + (size_t)v * 3 * HW + pix;
             on[0] = N[0]; on[HW] = N[1]; on[2 * HW] = N[2];
+        }
+        if (GEO) {
+            const size_t i = (size_t)v * a.H * a.W + (size_t)py * a.W + px;
+            geo->out_median[i] = gp.med;
+            geo->out_depth2[i] = gp.M2;
+            geo->median_pos[i] = gp.mpos;
         }
     }
 }
@@ -324,6 +347,21 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_NRM_MIN_BLOCKS) blend_
 {
     __shared__ float4 nrm[WARPS_PER_CTA][32];
     blend_fwd_body<false, true>(a, nullptr, ContribOut{}, nrm, gauss_normals, out_normal);
+}
+
+// F6 with the geometry outputs, without and with the normal image (DESIGN.md section 5 lists their registers at this bound)
+#ifndef FWD_GEO_MIN_BLOCKS
+#define FWD_GEO_MIN_BLOCKS 16
+#endif
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_GEO_MIN_BLOCKS) blend_fwd_geo_kernel(BlendArgs a, GeoFwd g)
+{
+    blend_fwd_body<false, false, true>(a, nullptr, ContribOut{}, nullptr, nullptr, nullptr, &g);
+}
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_GEO_MIN_BLOCKS) blend_fwd_nrm_geo_kernel(BlendArgs a, const float4 *gauss_normals,
+                                                                                                 float *out_normal, GeoFwd g)
+{
+    __shared__ float4 nrm[WARPS_PER_CTA][32];
+    blend_fwd_body<false, true, true>(a, nullptr, ContribOut{}, nrm, gauss_normals, out_normal, &g);
 }
 
 #endif // !FWD_BULK
@@ -498,11 +536,20 @@ void launch_blend_fwd_nrm(const BlendArgs &a, const float4 *gauss_normals, float
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
     blend_fwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal);
 }
+int blend_has_geometry() { return 1; }
+void launch_blend_fwd_geo(const BlendArgs &a, const float4 *gauss_normals, float *out_normal, const GeoFwd &g, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
+    if (gauss_normals) blend_fwd_nrm_geo_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal, g);
+    else blend_fwd_geo_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, g);
+}
 #else
 int blend_fwd_has_contrib() { return 0; } // the contribution variant exists for the default kernel only
 void launch_blend_fwd_contrib(const BlendArgs &, const ContribOut &, cudaStream_t) {}
 int blend_has_normals() { return 0; } // nor the normal maps (their backward kernels are not launched either)
 void launch_blend_fwd_nrm(const BlendArgs &, const float4 *, float *, cudaStream_t) {}
+int blend_has_geometry() { return 0; } // nor the geometry outputs
+void launch_blend_fwd_geo(const BlendArgs &, const float4 *, float *, const GeoFwd &, cudaStream_t) {}
 #endif
 
 // ------------------------------------------------------------------------------------------------
@@ -546,16 +593,23 @@ __device__ __forceinline__ void red_add_v2(float *p, float a, float b)
 // NRM (normal maps, DESIGN.md section 2): the flush also sums Wn = sum w * dL/dN over the slot's pixels, dL/dN from the
 // warp's second pixel table npix (laid out as pk.pix).  Atomic mode adds (Wn, 0) to nb.wn[record] with one more v4 RED;
 // deterministic mode stores it to nb.partials[slot].  Everything else is formed exactly as without NRM.
-template <bool DET, bool ABS, bool NRM = false>
+// GEO (geometry outputs, DESIGN.md section 2): the flush also sums Wm = sum w * dL/dM2 and Md = the dL/dmedian of the slot's
+// median pixels (the hit loop's ballot gmed[h], bit p = pixel p), both from the warp's pixel table gpix (laid out as pk.pix),
+// and each part adds 2d * Wm + Md to its W3 before the exchange, d the record's depth (word 11, an L1 hit as the conic is).
+// The depth gradient then reaches the mean through B2's existing depth term; everything else is formed exactly as without GEO.
+template <bool DET, bool ABS, bool NRM = false, bool GEO = false>
 __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, float fx0, float fy_part, float *sgrad,
                                            const BlendBwdArgs &a, const DetFlush &det, const float4 *npix = nullptr,
-                                           const NrmBwd *nb = nullptr)
+                                           const NrmBwd *nb = nullptr, const float2 *gpix = nullptr, const uint32_t *gmed = nullptr)
 {
     __syncwarp();
     const int h = lane % BWD_PARK, part = lane / BWD_PARK;
     const float4 s = pk.hit[h];
     float4 conic = make_float4(0.f, 0.f, 0.f, 0.f);
     if (ABS && h < n) conic = __ldg(reinterpret_cast<const float4 *>(a.recs) + 3 * (size_t)__float_as_uint(s.w) + 1);
+    uint32_t mb = 0u;
+    float Wm = 0.f, Md = 0.f;
+    if (GEO) mb = gmed[h];
     float dxk[8];
 #pragma unroll
     for (int k = 0; k < 8; k++) dxk[k] = fsub(s.x, fadd(fx0, (float)k));
@@ -588,12 +642,21 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
                 const float4 gn = npix[p0 + k + part];
                 N0 = fmaf(v.y, gn.x, N0); N1 = fmaf(v.y, gn.y, N1); N2 = fmaf(v.y, gn.z, N2);
             }
+            if (GEO) {
+                const float2 gg = gpix[p0 + k + part];
+                Wm = fmaf(v.y, gg.x, Wm);
+                if ((mb >> (p0 + k)) & 1u) Md += gg.y;
+            }
         }
         const float dy = fsub(s.y, fadd(fy_part, (float)r));
         const float qy = R0 * dy;
         S0 += R0; Sx += Rx; Sxx += Rxx; Sy += qy;
         Sxy = fmaf(Rx, dy, Sxy);
         Syy = fmaf(qy, dy, Syy);
+    }
+    if (GEO && h < n) {
+        const float d = __ldg(reinterpret_cast<const float *>(a.recs) + 12 * (size_t)__float_as_uint(s.w) + 11);
+        W3 += fmaf(d + d, Wm, Md);
     }
 #pragma unroll
     for (int o = BWD_PARK; o < 32; o <<= 1) {
@@ -640,9 +703,13 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
 // partials), ABS adds the absolute sums to it; everything else is the same code.
 // NRM (normal maps): contributing lanes also stage gauss_normals[record] in the warp's nslab row, the pixel's dL/dN goes to
 // the second pixel table npix, cg gains n . dL/dN, and the flush sums Wn (park_flush).
-template <bool DET, bool ABS, bool NRM = false>
+// GEO (geometry outputs): the pixel's (dL/dM2, dL/dmedian) go to the pixel table gpixs, cg gains d^2 * dL/dM2, every parked hit
+// ballots the lanes whose median it is into gmeds[slot], and the flush folds both depth terms into W3 (park_flush).
+template <bool DET, bool ABS, bool NRM = false, bool GEO = false>
 __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetFlush &det, float4 (*nslabs)[32] = nullptr,
-                                               float4 (*npixs)[32 + PARK_LANES] = nullptr, const NrmBwd *nb = nullptr)
+                                               float4 (*npixs)[32 + PARK_LANES] = nullptr, const NrmBwd *nb = nullptr,
+                                               float2 (*gpixs)[32 + PARK_LANES] = nullptr, uint32_t (*gmeds)[BWD_PARK] = nullptr,
+                                               const GeoBwd *gb = nullptr)
 {
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
     __shared__ WarpPark parks[WARPS_PER_CTA];
@@ -671,6 +738,8 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
 
     float T_final = 1.f, gC0 = 0.f, gC1 = 0.f, gC2 = 0.f, gD = 0.f, gA = 0.f;
     float4 gN = make_float4(0.f, 0.f, 0.f, 0.f);
+    float gM2 = 0.f, gMed = 0.f;
+    uint32_t mpos = 0u; // 1-based list position of the pixel's median entry (0: none)
     int last = 0;
     if (inside) {
         T_final = a.final_T[v * HW + pix];
@@ -685,6 +754,11 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
             const float *g = nb->dL_dnormal + (size_t)v * 3 * HW;
             gN = make_float4(g[pix], g[HW + pix], g[2 * HW + pix], 0.f);
         }
+        if (GEO) {
+            if (gb->dL_ddepth2) gM2 = gb->dL_ddepth2[v * HW + pix];
+            if (gb->dL_dmedian) gMed = gb->dL_dmedian[v * HW + pix];
+            mpos = gb->median_pos[v * HW + pix];
+        }
     }
     int wmax = last; // list positions at or beyond the patch's largest n_contrib cannot contribute here
     wmax = max(wmax, __shfl_xor_sync(FULL, wmax, 16));
@@ -697,6 +771,7 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
     const float bg_dot = a.bg[0] * gC0 + a.bg[1] * gC1 + a.bg[2] * gC2;
     pk.pix[lane + lane / BWD_PARK] = make_float4(gC0, gC1, gC2, gD); // read by the flushes, after their __syncwarp
     if (NRM) npixs[warp][lane + lane / BWD_PARK] = gN;
+    if (GEO) gpixs[warp][lane + lane / BWD_PARK] = make_float2(gM2, gMed);
     int np = 0;                                                      // park slots in use (warp-uniform)
     const float fx0 = (float)x0, fy_part = (float)(y0 + (lane / BWD_PARK) * (BWD_PARK / 8)); // the flush lane's first row
     float *const sgrad = reinterpret_cast<float *>(a.sgrad);
@@ -759,6 +834,7 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
                     const float4 n = *ns++;
                     cg = fmaf(n.x, gN.x, fmaf(n.y, gN.y, fmaf(n.z, gN.z, cg)));
                 }
+                if (GEO) cg = fmaf(fmul(q2.w, q2.w), gM2, cg); // cg += d^2 dL/dM2 (no background term either)
                 const float one_m_a = 1.0f - alpha;
                 float inv; // 1/(1-alpha), 1-alpha in [0.01, 1) where the lane contributes
                 asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv) : "f"(one_m_a));
@@ -780,15 +856,22 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
                 // mean combination is linear and happens once per Gaussian in B2) and the four weights of w
                 *pq = contrib ? make_float2(G * dL_dalpha, alpha * Tc) : make_float2(0.f, 0.f);
                 if (lane == 0) pk.hit[np] = g0;
+                if (GEO) { // the lanes whose median this hit is (pos is 0-based, mpos 1-based)
+                    const uint32_t mb = __ballot_sync(FULL, contrib & ((uint32_t)pos + 1u == mpos));
+                    if (lane == 0) gmeds[warp][np] = mb;
+                }
             }
             if (np == BWD_PARK) {
-                park_flush<DET, ABS, NRM>(pk, np, lane, fx0, fy_part, sgrad, a, det, NRM ? npixs[warp] : nullptr, nb);
+                park_flush<DET, ABS, NRM, GEO>(pk, np, lane, fx0, fy_part, sgrad, a, det, NRM ? npixs[warp] : nullptr, nb,
+                                               GEO ? gpixs[warp] : nullptr, GEO ? gmeds[warp] : nullptr);
                 np = 0;
             }
         }
         __syncwarp();
     }
-    if (np > 0) park_flush<DET, ABS, NRM>(pk, np, lane, fx0, fy_part, sgrad, a, det, NRM ? npixs[warp] : nullptr, nb);
+    if (np > 0)
+        park_flush<DET, ABS, NRM, GEO>(pk, np, lane, fx0, fy_part, sgrad, a, det, NRM ? npixs[warp] : nullptr, nb,
+                                       GEO ? gpixs[warp] : nullptr, GEO ? gmeds[warp] : nullptr);
 }
 
 __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_kernel(BlendBwdArgs a)
@@ -863,6 +946,37 @@ void launch_blend_bwd_nrm(const BlendBwdArgs &a, const DetFlush *det, bool absgr
         if (absgrad) blend_bwd_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, n);
         else blend_bwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, n);
     }
+}
+
+// B1 with the geometry gradients (GEO): atomic / deterministic x absgrad off / on x normals off / on.  Each stages the pixels'
+// (dL/dM2, dL/dmedian) and the slots' median ballots in two more per-warp shared arrays (and the NRM forms the normals' two).
+template <bool DET, bool ABS, bool NRM>
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_geo_kernel(BlendBwdArgs a, DetFlush det, NrmBwd nb,
+                                                                                          GeoBwd gb)
+{
+    __shared__ float2 gpix[WARPS_PER_CTA][32 + PARK_LANES];
+    __shared__ uint32_t gmed[WARPS_PER_CTA][BWD_PARK];
+    if (NRM) {
+        BWD_NRM_SHARED;
+        blend_bwd_body<DET, ABS, true, true>(a, det, nslab, npix, &nb, gpix, gmed, &gb);
+    } else {
+        blend_bwd_body<DET, ABS, false, true>(a, det, nullptr, nullptr, nullptr, gpix, gmed, &gb);
+    }
+}
+void launch_blend_bwd_geo(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd *n, const GeoBwd &g, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
+    const DetFlush d = det ? *det : DetFlush{};
+    const NrmBwd nb = n ? *n : NrmBwd{};
+    void (*k)(BlendBwdArgs, DetFlush, NrmBwd, GeoBwd);
+    if (det) {
+        if (n) k = absgrad ? blend_bwd_geo_kernel<true, true, true> : blend_bwd_geo_kernel<true, false, true>;
+        else k = absgrad ? blend_bwd_geo_kernel<true, true, false> : blend_bwd_geo_kernel<true, false, false>;
+    } else {
+        if (n) k = absgrad ? blend_bwd_geo_kernel<false, true, true> : blend_bwd_geo_kernel<false, false, true>;
+        else k = absgrad ? blend_bwd_geo_kernel<false, true, false> : blend_bwd_geo_kernel<false, false, false>;
+    }
+    k<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, d, nb, g);
 }
 
 int blend_bwd_has_absgrad() { return 1; }

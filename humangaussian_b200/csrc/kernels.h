@@ -186,6 +186,23 @@ struct NrmBwd {
 // B1 with the normal term: atomic (det NULL) or deterministic, with or without the absolute sums
 void launch_blend_bwd_nrm(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd &n, cudaStream_t st);
 // the deterministic reduce with the normal partials: also writes wn[vp] = their sums in the same fixed order
+// ---- geometry outputs (DESIGN.md section 2; the GEO instantiations of the blend kernels) ---------------------------------
+int blend_has_geometry(); // 0 in the classic comparator and the bulk-copy build
+struct GeoFwd {
+    float *out_median;    // [V,1,H,W] depth of the last blend with T > 0.5 before it (0: none)
+    float *out_depth2;    // [V,1,H,W] M2 = sum w d^2
+    uint32_t *median_pos; // [V,H,W] 1-based list position of that blend (0: none); read by the backward
+};
+// F6 with the geometry outputs; gauss_normals non-NULL: also the normal image out_normal (the nrm+geo kernel)
+void launch_blend_fwd_geo(const BlendArgs &a, const float4 *gauss_normals, float *out_normal, const GeoFwd &g, cudaStream_t st);
+struct GeoBwd {
+    const float *dL_dmedian;      // [V,1,H,W] or NULL (zero)
+    const float *dL_ddepth2;      // [V,1,H,W] or NULL (zero)
+    const uint32_t *median_pos;   // [V,H,W] the forward's
+};
+// B1 with the geometry gradients folded into W3: atomic (det NULL) or deterministic, with or without the absolute sums, with
+// (n non-NULL) or without the normal term.  The deterministic reduce is the one the same call without geometry runs.
+void launch_blend_bwd_geo(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd *n, const GeoBwd &g, cudaStream_t st);
 void launch_det_reduce_nrm(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
                            const float4 *nrm_partials, float4 *wn, cudaStream_t st);
 

@@ -88,6 +88,17 @@ def _normals_io(gauss_normals, out_normal=None, dL_dnormal=None, normal_wn=None,
                       _ptr(nrm_partials), 0 if nrm_partials is None else nrm_partials.numel())
 
 
+class _GeometryIO(C.Structure):
+    """b200gs_geometry_io (include/b200gs.h): the median depth and depth second moment's buffers"""
+    _fields_ = [("struct_bytes", C.c_int32), ("out_median", C.c_void_p), ("out_depth2", C.c_void_p), ("median_pos", C.c_void_p),
+                ("dL_dmedian", C.c_void_p), ("dL_ddepth2", C.c_void_p)]
+
+
+def _geometry_io(median_pos, out_median=None, out_depth2=None, dL_dmedian=None, dL_ddepth2=None):
+    return _GeometryIO(C.sizeof(_GeometryIO), _ptr(out_median), _ptr(out_depth2), _ptr(median_pos), _ptr(dL_dmedian),
+                       _ptr(dL_ddepth2))
+
+
 class _StateView(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("geom_records", "tiles_touched", "offsets", "clamped", "sorted_tile_keys",
                                           "depth_order", "point_list", "ranges", "final_T", "n_contrib",
@@ -106,7 +117,8 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_backward_deterministic_absgrad_opts", "b200gs_forward_contrib_opts", "b200gs_prune_plan",
            "b200gs_forward_normals_opts", "b200gs_backward_normals_opts", "b200gs_backward_deterministic_normals_opts",
            "b200gs_backward_absgrad_normals_opts", "b200gs_backward_deterministic_absgrad_normals_opts", "b200gs_mcmc_noise",
-           "b200gs_mcmc_ratio", "b200gs_mcmc_move"]
+           "b200gs_mcmc_ratio", "b200gs_mcmc_move", "b200gs_forward_geometry_opts", "b200gs_backward_geometry_opts",
+           "b200gs_backward_deterministic_geometry_opts"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -161,6 +173,13 @@ def load_library():
         fn = getattr(L, f"b200gs_{name}_normals_opts")
         fn.restype = C.c_int
         fn.argtypes = base[:2] + [C.POINTER(_NormalsIO)] + base[2:]
+    # the geometry forms: the nullable normals io and the geometry io after opts; the backward forms take the absgrad forms'
+    # argument lists (dL_dmeans2D_abs and abs_partials nullable)
+    for name, base in (("forward", fo), ("backward", L.b200gs_backward_absgrad_opts.argtypes),
+                       ("backward_deterministic", L.b200gs_backward_deterministic_absgrad_opts.argtypes)):
+        fn = getattr(L, f"b200gs_{name}_geometry_opts")
+        fn.restype = C.c_int
+        fn.argtypes = base[:2] + [C.POINTER(_NormalsIO), C.POINTER(_GeometryIO)] + base[2:]
     L.b200gs_sampling_rate.restype = C.c_int
     L.b200gs_sampling_rate.argtypes = [i32, i32, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float), i32, i32, vp, vp]
     L.b200gs_mark_visible.restype = C.c_int
@@ -352,7 +371,7 @@ def release_cached_buffers():
 class _Ctx:
     """What one forward keeps for its backward (upstream keeps geomBuffer/binningBuffer/imgBuffer the same way)."""
     __slots__ = ("prm", "tanx", "tany", "geom", "binning", "image", "scratch", "capacity", "num_rendered", "radii", "V", "P", "H",
-                 "W", "M", "opts", "f3d", "gauss_normals", "normal", "normal_wn", "__weakref__")
+                 "W", "M", "opts", "f3d", "gauss_normals", "normal", "normal_wn", "median", "depth2", "median_pos", "__weakref__")
 
 
 def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=False, per_view_means=False, raw=False):
@@ -365,7 +384,7 @@ def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=F
 
 def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                   campos, tanfovx, tanfovy, H, W, sh_degree, scale_modifier, prefiltered=False, debug=False, raw=False,
-                  antialiasing=False, filter_3d=None, contrib=None, normals=False):
+                  antialiasing=False, filter_3d=None, contrib=None, normals=False, geometry=False):
     """All tensors float32 contiguous on one CUDA device.  viewmatrix/projmatrix [V,4,4], campos [V,3].
     raw: opacities / scales / rotations are GaussianModel's raw parameters (activations fused into the kernels).
     antialiasing: the screen-space mip filter; filter_3d: the 3D smoothing filter's [P] variances (b200gs_render_opts).
@@ -373,7 +392,9 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     contrib: None, or the contribution accumulators (weight_sum, weight_max, touches), [P] int64 / int32 / int32 device tensors
     read as u64 / u32 / u32: b200gs_forward_contrib_opts then runs and folds this call's views into them.
     normals=True: b200gs_forward_normals_opts runs; the state holds the normal image `normal` [V,3,H,W] and the per-(view,
-    Gaussian) normals `gauss_normals` [V,P,4] its backward reads."""
+    Gaussian) normals `gauss_normals` [V,P,4] its backward reads.
+    geometry=True: b200gs_forward_geometry_opts runs (with the normals io when normals=True); the state holds the images
+    `median` and `depth2` [V,1,H,W] and the median positions `median_pos` [V,H,W] int32 its backward reads."""
     L = load_library()
     dev = means3D.device
     if dev.type != "cuda":
@@ -393,6 +414,8 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
         raise ValueError("b200gs: normals take each Gaussian's shortest scale axis; a precomputed covariance has none")
     if normals and contrib is not None:
         raise ValueError("b200gs: the contribution forward does not render normals")
+    if geometry and contrib is not None:
+        raise ValueError("b200gs: the contribution forward does not render the geometry outputs")
     filter_3d = _check_filter_3d(filter_3d, P, dev, cov3D_precomp)
     prm, tx, ty = _make_params(P, V, sh_degree, M, H, W, scale_modifier, tanfovx, tanfovy, prefiltered, debug, per_view_means, raw)
     u8 = dict(dtype=torch.uint8, device=dev)
@@ -413,6 +436,14 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
         normal = torch.empty(V, 3, H, W, dtype=torch.float32, device=dev)
         nio = _normals_io(gauss_normals, normal)
         fwd = lambda *a: L.b200gs_forward_normals_opts(a[0], None if opts is None else C.byref(opts), C.byref(nio), *a[1:])
+    median = depth2 = median_pos = None
+    if geometry:
+        median = torch.empty(V, 1, H, W, dtype=torch.float32, device=dev)
+        depth2 = torch.empty(V, 1, H, W, dtype=torch.float32, device=dev)
+        median_pos = torch.empty(V, H, W, dtype=torch.int32, device=dev)
+        gio = _geometry_io(median_pos, median, depth2)
+        nio_p = C.byref(nio) if normals else None
+        fwd = lambda *a: L.b200gs_forward_geometry_opts(a[0], None if opts is None else C.byref(opts), nio_p, C.byref(gio), *a[1:])
     if contrib is not None:
         fwd = lambda *a: L.b200gs_forward_contrib_opts(a[0], None if opts is None else C.byref(opts), *a[1:-1],
                                                        *[_ptr(t) for t in contrib], a[-1])
@@ -451,15 +482,17 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     st.radii, st.V, st.P, st.H, st.W, st.M = radii, V, P, H, W, M
     st.opts, st.f3d = opts, filter_3d  # the backward reads the same variances (st keeps them alive)
     st.gauss_normals, st.normal, st.normal_wn = gauss_normals, normal, None
+    st.median, st.depth2, st.median_pos = median, depth2, median_pos
     weakref.finalize(st, _pool.give, pkey, bufs)  # when the autograd graph drops the state, the buffers are parked for re-use
     return color, radii, depth, alpha, st
 
 
-def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_abs=None, nio=None):
+def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_abs=None, nio=None, gio=None):
     """b200gs_backward_deterministic with the work buffer from _det_pool, sized by the partial-capacity hint; a call whose
     partials do not fit is repeated with room for the count it reported (at most two retries).  d_means2D_abs: the absgrad
     form, with its float2-per-partial array pooled beside the work buffer.  nio: the normals form (_NormalsIO with dL_dnormal),
-    with its float4-per-partial array pooled the same way."""
+    with its float4-per-partial array pooled the same way.  gio: the geometry form (_GeometryIO with a geometry gradient),
+    which needs no buffer of its own."""
     P, V, H, W = st.P, st.V, st.H, st.W
     key = (dev.index, P, V, H, W)
     pcap = _partial_hint.get(key, max(1 << 16, 2 * st.num_rendered))
@@ -479,6 +512,12 @@ def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_ab
         opts_p = C.byref(st.opts) if st.opts is not None else None
         if nio is not None:
             nio.nrm_partials, nio.nrm_partials_bytes = _ptr(bufs["nrm"]), bufs["nrm"].numel()
+        if gio is not None:
+            ab = bufs.get("abs")
+            rc = L.b200gs_backward_deterministic_geometry_opts(
+                args[0], opts_p, None if nio is None else C.byref(nio), C.byref(gio), *args[1:29], _ptr(d_means2D_abs), *args[29:],
+                _ptr(det), det.numel(), pcap, C.byref(n_out), _ptr(ab), 0 if ab is None else ab.numel(), C.c_void_p(stream))
+        elif nio is not None:
             if d_means2D_abs is not None:
                 ab = bufs["abs"]
                 rc = L.b200gs_backward_deterministic_absgrad_normals_opts(
@@ -513,7 +552,8 @@ def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_ab
 
 
 def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
-                   projmatrix, campos, g_color, g_depth, g_alpha, out=None, det_state=None, absgrad=False, g_normal=None):
+                   projmatrix, campos, g_color, g_depth, g_alpha, out=None, det_state=None, absgrad=False, g_normal=None,
+                   g_median=None, g_depth2=None):
     """`out` (optional): dict of preallocated contiguous fp32 gradient buffers by name (means3D, sh, opacity, scales,
     rotations) -- the packed entry points them into one flat buffer so that B3 writes the all-reduce payload in place.
 
@@ -523,6 +563,10 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
     g_normal [V,3,H,W] (a forward with normals=True): the normals entry points run, dL/dN reaches the opacities, means and
     colours through the blend weights and the rotations through the normals; st.normal_wn then holds the [V,P,4] sums Wn.
     None: the call without normals.
+
+    g_median, g_depth2 [V,1,H,W] (a forward with geometry=True; None = zero): the geometry entry points run.  dL/dM2 reaches
+    the opacities, means and colours through the blend weights and the means through the depth; dL/dmedian reaches the means
+    of each pixel's median Gaussian through its depth.  With both None the call is the one without geometry.
 
     Under torch.use_deterministic_algorithms(True) the backward is the library's deterministic one: the same gradients up
     to float rounding, bit-identical from run to run (one host wait per call, for its partial count).  `det_state`
@@ -555,9 +599,16 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
     if g_normal is not None and st.gauss_normals is not None:
         st.normal_wn = torch.empty(V, P, 4, **f)
         nio = _normals_io(st.gauss_normals, None, g_normal, st.normal_wn)
+    gio = None
+    if (g_median is not None or g_depth2 is not None) and st.median_pos is not None:
+        gio = _geometry_io(st.median_pos, None, None, g_median, g_depth2)
     with torch.cuda.device(dev):
         if torch.are_deterministic_algorithms_enabled():
-            rc = _backward_deterministic(L, st, dev, args, det_state, d_abs, nio)
+            rc = _backward_deterministic(L, st, dev, args, det_state, d_abs, nio, gio)
+        elif gio is not None:
+            rc = L.b200gs_backward_geometry_opts(args[0], C.byref(st.opts) if st.opts is not None else None,
+                                                 None if nio is None else C.byref(nio), C.byref(gio), *args[1:29], _ptr(d_abs),
+                                                 *args[29:], _stream(dev))
         elif nio is not None:
             opts_p = C.byref(st.opts) if st.opts is not None else None
             if absgrad:
@@ -593,7 +644,7 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, squeeze,
-                means2D_abs=None, normals=False):
+                means2D_abs=None, normals=False, geometry=False):
         bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, prefiltered, debug = cams[:12]
         raw = bool(cams[12]) if len(cams) > 12 else False
         aa = bool(cams[13]) if len(cams) > 13 else False
@@ -602,36 +653,46 @@ class _RasterizeViews(torch.autograd.Function):
         args = [_f32c(t, dev) for t in (means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)]
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
         color, radii, depth, alpha, st = _forward_impl(*args, *camt, tanx, tany, H, W, deg, mod, prefiltered, debug, raw, aa, f3d,
-                                                       normals=normals)
-        ctx.st, ctx.squeeze, ctx.absgrad = st, squeeze, means2D_abs is not None
+                                                       normals=normals, geometry=geometry)
+        ctx.st, ctx.squeeze, ctx.absgrad, ctx.normals = st, squeeze, means2D_abs is not None, normals
         _save(ctx, args + camt)
         ctx.in_shapes = [None if t is None else t.shape for t in (means3D, means2D, shs, colors_precomp, opacities, scales,
                                                                   rotations, cov3D_precomp)]
         ctx.mark_non_differentiable(radii)
         if squeeze:
             return color[0], radii[0], depth[0], alpha[0]
-        if normals:
-            # an output the loss does not use gets None, not zeros: a normal image returned but not in the loss then runs the
-            # plain backward kernels (the C ABI's dL_dnormal = NULL), and an unused image is skipped like a zero one
+        if normals or geometry:
+            # an output the loss does not use gets None, not zeros: a normal or geometry image returned but not in the loss then
+            # runs the plain backward kernels (the C ABI's NULL gradients), and an unused image is skipped like a zero one
             ctx.set_materialize_grads(False)
-            return color, radii, depth, alpha, st.normal
+            return (color, radii, depth, alpha) + ((st.normal,) if normals else ()) + ((st.median, st.depth2) if geometry else ())
         return color, radii, depth, alpha
 
     @staticmethod
-    def backward(ctx, g_color, g_radii, g_depth, g_alpha, g_normal=None):
+    def backward(ctx, g_color, g_radii, g_depth, g_alpha, *g_extra):
         st = ctx.st  # kept until the graph is freed: a second backward (retain_graph=True) recomputes from the same state
         means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix, campos = _saved(ctx)
         dev = means3D.device
         g = [None if t is None else _f32c(t, dev) for t in (g_color, g_depth, g_alpha)]
+        g_normal, g_median, g_depth2 = _extra_grads(g_extra, ctx.normals, dev)
         d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov, *d_abs = _backward_impl(
             st, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix, campos, *g,
-            absgrad=ctx.absgrad, g_normal=None if g_normal is None else _f32c(g_normal, dev))
+            absgrad=ctx.absgrad, g_normal=g_normal, g_median=g_median, g_depth2=g_depth2)
         if ctx.squeeze:
             d_means2D = d_means2D[0]
         # gradients take the shape the caller passed (e.g. opacities [P] or [P,1])
         grads = [g if (g is None or shp is None) else g.reshape(shp)
                  for g, shp in zip((d_means3D, d_means2D, d_sh, d_col, d_op, d_sc, d_rot, d_cov), ctx.in_shapes)]
-        return (*grads, None, None, d_abs[0] if d_abs else None, None)
+        return (*grads, None, None, d_abs[0] if d_abs else None, None, None)
+
+
+def _extra_grads(g_extra, normals, dev):
+    """(g_normal, g_median, g_depth2) from the gradients of the outputs after alpha: the normal image if `normals`, then the
+    median and depth2 images if there are more (None where absent or unused)."""
+    g_extra = list(g_extra)
+    g_normal = g_extra.pop(0) if normals else None
+    g_median, g_depth2 = (g_extra + [None, None])[:2]
+    return tuple(None if t is None else _f32c(t, dev) for t in (g_normal, g_median, g_depth2))
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -695,7 +756,7 @@ class GaussianRasterizer(nn.Module):
 def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, tanfovx, tanfovy, image_height, image_width,
                     bg, sh_degree=0, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
                     means2D=None, scale_modifier=1.0, raw=False, antialiasing=False, filter_3d=None, means2D_abs=None,
-                    normals=False):
+                    normals=False, geometry=False):
     """Render V cameras of one Gaussian set in ONE call (one preprocess/sort/blend launch set, one host sync).
 
     normals=True: a fifth output, the normal image [V,3,H,W] = sum over each pixel's blends of w * n, n the world-space axis of
@@ -703,6 +764,12 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
     section 2).  It is differentiable: its gradient reaches the opacities, means and colours through the blend weights and
     the rotations through n.  Every other output is unchanged.  Not with cov3D_precomp (ValueError).  comp_normal() turns it
     into threestudio's normal map.
+
+    geometry=True: two more outputs after the normal image (or after alpha without normals): `median_depth` [V,1,H,W], the
+    view-space depth of the last blend whose transmittance before it is > 0.5, and `depth2` [V,1,H,W] = sum w * d^2, the depth
+    second moment (no background; both 0 where nothing blends; DESIGN.md section 2).  Both are differentiable: depth2 through
+    the blend weights and the depths, the median through its Gaussian's depth only.  Every other output is unchanged.
+    geometry.depth_distortion(alpha, depth, depth2) forms the depth distortion from them.
 
     means2D_abs: None, or a [V,P,3] fp32 gradient sink like means2D (zeros, requires_grad): the backward then fills its
     .grad with the absolute screen-space gradient -- per (view, Gaussian) the per-pixel terms of means2D's gradient summed
@@ -735,9 +802,10 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                                 scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
                                 means2D=None if means2D is None else means2D[i:i + MAX_VIEWS], scale_modifier=scale_modifier, raw=raw,
                                 antialiasing=antialiasing, filter_3d=filter_3d,
-                                means2D_abs=None if means2D_abs is None else means2D_abs[i:i + MAX_VIEWS], normals=normals)
+                                means2D_abs=None if means2D_abs is None else means2D_abs[i:i + MAX_VIEWS], normals=normals,
+                                geometry=geometry)
                 for i in range(0, V, MAX_VIEWS)]
-        return tuple(torch.cat([o[k] for o in outs], 0) for k in range(5 if normals else 4))
+        return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4 + bool(normals) + 2 * bool(geometry)))
     _check_filter_3d(filter_3d, means3D.shape[-2], means3D.device, cov3D_precomp)
     if means2D is None:
         means2D = torch.zeros(V, means3D.shape[-2], 3, dtype=torch.float32, device=means3D.device)
@@ -745,7 +813,7 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
             int(sh_degree), float(scale_modifier), False, False, bool(raw), bool(antialiasing), filter_3d)
     try:
         return _RasterizeViews.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, cams, False,
-                                     means2D_abs, bool(normals))
+                                     means2D_abs, bool(normals), bool(geometry))
     except InstanceLimitError:
         if V == 1:
             raise
@@ -756,9 +824,10 @@ def rasterize_views(*, means3D, opacities, viewmatrices, projmatrices, camposs, 
                             image_height=image_height, image_width=image_width, bg=bg, sh_degree=sh_degree, shs=shs,
                             colors_precomp=colors_precomp, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
                             means2D=means2D[sl], scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing,
-                            filter_3d=filter_3d, means2D_abs=None if means2D_abs is None else means2D_abs[sl], normals=normals)
+                            filter_3d=filter_3d, means2D_abs=None if means2D_abs is None else means2D_abs[sl], normals=normals,
+                            geometry=geometry)
             for sl in (slice(0, h), slice(h, V))]
-    return tuple(torch.cat([o[k] for o in outs], 0) for k in range(5 if normals else 4))
+    return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4 + bool(normals) + 2 * bool(geometry)))
 
 
 # ---- packed entry: one flat SoA parameter buffer in, one flat gradient buffer out ---------------------------------
@@ -787,23 +856,23 @@ def _split_packed(flat: torch.Tensor, P: int, M: int):
 
 class _RasterizePacked(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, packed, means2D, P, M, cams, means2D_abs=None, normals=False):
+    def forward(ctx, packed, means2D, P, M, cams, means2D_abs=None, normals=False, geometry=False):
         bg, viewmatrix, projmatrix, campos, tanx, tany, H, W, deg, mod, raw, aa, f3d = cams
         dev = packed.device
         xyz, sc, rot, op, sh = _split_packed(packed.detach(), P, M)
         camt = [_f32c(t, dev) for t in (bg, viewmatrix, projmatrix, campos)]
         color, radii, depth, alpha, st = _forward_impl(xyz, sh, None, op, sc, rot, None, *camt, tanx, tany, H, W, deg, mod, raw=raw,
-                                                       antialiasing=aa, filter_3d=f3d, normals=normals)
-        ctx.st, ctx.P, ctx.M, ctx.absgrad = st, P, M, means2D_abs is not None
+                                                       antialiasing=aa, filter_3d=f3d, normals=normals, geometry=geometry)
+        ctx.st, ctx.P, ctx.M, ctx.absgrad, ctx.normals = st, P, M, means2D_abs is not None, normals
         ctx.save_for_backward(packed, *camt)
         ctx.mark_non_differentiable(radii)
-        if normals:
-            ctx.set_materialize_grads(False)  # as _RasterizeViews: an unused normal image costs no normal backward
-            return color, radii, depth, alpha, st.normal
+        if normals or geometry:
+            ctx.set_materialize_grads(False)  # as _RasterizeViews: an unused normal or geometry image costs no backward term
+            return (color, radii, depth, alpha) + ((st.normal,) if normals else ()) + ((st.median, st.depth2) if geometry else ())
         return color, radii, depth, alpha
 
     @staticmethod
-    def backward(ctx, g_color, g_radii, g_depth, g_alpha, g_normal=None):
+    def backward(ctx, g_color, g_radii, g_depth, g_alpha, *g_extra):
         packed, bg, viewmatrix, projmatrix, campos = ctx.saved_tensors
         packed = packed.detach()
         P, M, dev = ctx.P, ctx.M, packed.device
@@ -811,22 +880,23 @@ class _RasterizePacked(torch.autograd.Function):
         d_packed = torch.empty_like(packed) if P % 4 == 0 else torch.zeros_like(packed)  # alignment padding carries zero gradient
         d_xyz, d_sc, d_rot, d_op, d_sh = _split_packed(d_packed, P, M)
         g = [None if t is None else _f32c(t, dev) for t in (g_color, g_depth, g_alpha)]
+        g_normal, g_median, g_depth2 = _extra_grads(g_extra, ctx.normals, dev)
         _, d_means2D, *rest = _backward_impl(ctx.st, xyz, sh, None, op, sc, rot, None, bg, viewmatrix, projmatrix, campos, *g,
                                              out=dict(means3D=d_xyz, sh=d_sh, opacity=d_op, scales=d_sc, rotations=d_rot),
-                                             absgrad=ctx.absgrad, g_normal=None if g_normal is None else _f32c(g_normal, dev))
-        return d_packed, d_means2D, None, None, None, rest[6] if ctx.absgrad else None, None
+                                             absgrad=ctx.absgrad, g_normal=g_normal, g_median=g_median, g_depth2=g_depth2)
+        return d_packed, d_means2D, None, None, None, rest[6] if ctx.absgrad else None, None, None
 
 
 def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, viewmatrices, projmatrices, camposs, tanfovx, tanfovy,
                            image_height, image_width, bg, sh_degree=0, means2D=None, scale_modifier=1.0, raw=False, antialiasing=False,
-                           filter_3d=None, means2D_abs=None, normals=False):
+                           filter_3d=None, means2D_abs=None, normals=False, geometry=False):
     """`rasterize_views` over ONE flat fp32 buffer [xyz 3P | scales 3P | rotations 4P | opacities P | shs 3*K*P], each
     field starting on a 16-byte boundary (`packed_layout`; what `dist.pack` produces, broadcast once per parameter
     version).  raw=False: post-activation values, as the rasteriser's classic inputs.  raw=True: the buffer holds the
     optimiser's RAW parameters (log-scales, un-normalised quaternions, opacity logits; SH = cat(f_dc, f_rest)); the
     activations of gaussian_model.py:95-118 and their Jacobians run inside the kernels, so `packed.grad` is the gradient
     of the raw parameters and a training step needs no activation kernels, no pack copy and no autograd nodes besides
-    this one.  antialiasing, filter_3d, means2D_abs, normals: as `rasterize_views`.  The backward
+    this one.  antialiasing, filter_3d, means2D_abs, normals, geometry: as `rasterize_views`.  The backward
     kernels write the parameter gradients straight into one buffer of the same layout, which becomes `packed.grad`
     as is: no per-tensor gradient accumulation, and on several GPUs that buffer is the all-reduce payload in place.
     V <= MAX_VIEWS.  Returns color [V,3,H,W], radii [V,P], depth [V,1,H,W], alpha [V,1,H,W]."""
@@ -843,7 +913,7 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
     cams = (bg, viewmatrices, projmatrices, camposs, list(tanfovx), list(tanfovy), int(image_height), int(image_width),
             int(sh_degree), float(scale_modifier), bool(raw), bool(antialiasing), filter_3d)
     try:
-        return _RasterizePacked.apply(packed, means2D, int(P), int(sh_coeffs), cams, means2D_abs, bool(normals))
+        return _RasterizePacked.apply(packed, means2D, int(P), int(sh_coeffs), cams, means2D_abs, bool(normals), bool(geometry))
     except InstanceLimitError:
         if V == 1:
             raise
@@ -852,9 +922,10 @@ def rasterize_views_packed(packed: torch.Tensor, P: int, sh_coeffs: int, *, view
                                    tanfovx=list(tanfovx)[sl], tanfovy=list(tanfovy)[sl], image_height=image_height,
                                    image_width=image_width, bg=bg, sh_degree=sh_degree, means2D=means2D[sl],
                                    scale_modifier=scale_modifier, raw=raw, antialiasing=antialiasing, filter_3d=filter_3d,
-                                   means2D_abs=None if means2D_abs is None else means2D_abs[sl], normals=normals)
+                                   means2D_abs=None if means2D_abs is None else means2D_abs[sl], normals=normals,
+                                   geometry=geometry)
             for sl in (slice(0, h), slice(h, V))]
-    return tuple(torch.cat([o[k] for o in outs], 0) for k in range(5 if normals else 4))
+    return tuple(torch.cat([o[k] for o in outs], 0) for k in range(4 + bool(normals) + 2 * bool(geometry)))
 
 
 # ---- test / debugging access to the forward state (tile and sort indices) -----------------------------------
@@ -876,7 +947,8 @@ def forward_with_state(**kw):
         _f32c(kw["bg"], dev), _f32c(vm, dev).reshape(V, 4, 4), _f32c(pm, dev).reshape(V, 4, 4), _f32c(cp, dev).reshape(V, 3),
         tanx, tany, int(kw["image_height"]), int(kw["image_width"]), int(kw.get("sh_degree", 0)),
         float(kw.get("scale_modifier", 1.0)), raw=bool(kw.get("raw", False)), antialiasing=bool(kw.get("antialiasing", False)),
-        filter_3d=kw.get("filter_3d"), contrib=kw.get("contrib"), normals=bool(kw.get("normals", False)))
+        filter_3d=kw.get("filter_3d"), contrib=kw.get("contrib"), normals=bool(kw.get("normals", False)),
+        geometry=bool(kw.get("geometry", False)))
     sv = _StateView()
     _check(L.b200gs_describe_state(C.byref(st.prm), _ptr(st.geom), _ptr(st.binning), st.capacity, _ptr(st.image), C.byref(sv)),
            "describe_state")
@@ -907,13 +979,17 @@ def forward_with_state(**kw):
     dbits = state["recs"][:, 11].contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
     pl = state["point_list"].to(torch.int64) & 0xFFFFFFFF
     state["sorted_keys"] = ((state["sorted_tile_keys"].to(torch.int64) & 0xFFFFFFFF) << 32) | dbits[pl]
+    extra = ()
     if st.normal is not None:
         state["gauss_normals"] = st.gauss_normals.reshape(V * P, 4).clone()
-        return color, radii, depth, alpha, st.normal, state, st
-    return color, radii, depth, alpha, state, st
+        extra += (st.normal,)
+    if st.median is not None:
+        state["median_pos"] = st.median_pos.clone()
+        extra += (st.median, st.depth2)
+    return (color, radii, depth, alpha) + extra + (state, st)
 
 
-def forward_backward_with_state(g_color, g_depth, g_alpha, g_normal=None, **kw):
+def forward_backward_with_state(g_color, g_depth, g_alpha, g_normal=None, g_median=None, g_depth2=None, **kw):
     """forward_with_state(**kw), then the backward of that same call for the image gradients g_color [V,3,H,W],
     g_depth [V,1,H,W], g_alpha [V,1,H,W].  Returns (color, radii, depth, alpha, state, sums): `sums` [V,P,12] float32 is
     the backward blend's ScreenGrad record of every (view, Gaussian) -- record v*P + g, in the format
@@ -921,9 +997,11 @@ def forward_backward_with_state(g_color, g_depth, g_alpha, g_normal=None, **kw):
     torch.use_deterministic_algorithms(True) the deterministic backward runs, and `state` also holds its "patch_masks"
     (uint8 per sorted instance, bit p = a partial for patch p of the instance's tile) and "n_partials".
     normals=True: the normal image is a fifth output after alpha, and g_normal [V,3,H,W] (None: no normal gradient) its
-    gradient; with g_normal, `state` also holds "normal_wn" [V,P,4], the sums Wn = sum w * dL/dN (DESIGN.md section 2)."""
+    gradient; with g_normal, `state` also holds "normal_wn" [V,P,4], the sums Wn = sum w * dL/dN (DESIGN.md section 2).
+    geometry=True: the median and depth2 images follow (after the normal image, if any), and g_median / g_depth2 [V,1,H,W]
+    (None: zero) are their gradients; `state` holds "median_pos"."""
     outs = forward_with_state(**kw)
-    color, radii, depth, alpha = outs[:4]
+    images = outs[:-2]
     state, st = outs[-2:]
     dev = kw["means3D"].device
     V, P = st.V, st.P
@@ -933,15 +1011,15 @@ def forward_backward_with_state(g_color, g_depth, g_alpha, g_normal=None, **kw):
     _backward_impl(st, t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"),
                    t("cov3D_precomp"), _f32c(kw["bg"], dev), t("viewmatrix").reshape(V, 4, 4), t("projmatrix").reshape(V, 4, 4),
                    t("campos").reshape(V, 3), *g, det_state=det_state,
-                   g_normal=None if g_normal is None else _f32c(g_normal, dev).reshape(V, 3, st.H, st.W))
+                   g_normal=None if g_normal is None else _f32c(g_normal, dev).reshape(V, 3, st.H, st.W),
+                   g_median=None if g_median is None else _f32c(g_median, dev).reshape(V, 1, st.H, st.W),
+                   g_depth2=None if g_depth2 is None else _f32c(g_depth2, dev).reshape(V, 1, st.H, st.W))
     state.update(det_state)
     if st.normal_wn is not None:
         state["normal_wn"] = st.normal_wn.clone()
     nbytes = V * P * 48
     sums = st.scratch[:nbytes].view(torch.float32).reshape(V, P, 12).clone()
-    if st.normal is not None:
-        return color, radii, depth, alpha, st.normal, state, sums
-    return color, radii, depth, alpha, state, sums
+    return tuple(images) + (state, sums)
 
 
 def sampling_rate(means3D: torch.Tensor, viewmatrices: torch.Tensor, tanfovx, tanfovy, image_height: int, image_width: int,

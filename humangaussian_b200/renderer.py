@@ -16,6 +16,7 @@ import math
 import torch
 import torch.nn.functional as F
 
+from .geometry import depth_distortion
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, rasterize_views
 
 
@@ -46,7 +47,7 @@ def _raw_tensors(pc):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, fused_activations=False, filter_3d=None,
-           absgrad=False, normals=False):
+           absgrad=False, normals=False, geometry=False):
     """fused_activations=True (optional fast path, SURVEY.md 8f-1): instead of calling the getters (sigmoid / exp /
     F.normalize: three kernels + autograd nodes per view, gaussian_model.py:95-118) the raw parameter tensors go straight
     to the rasteriser, which applies the activations and their Jacobians inside its kernels.  Same dict, same gradients
@@ -57,7 +58,10 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
     screen-space gradient (rasterizer.rasterize_views, means2D_abs), the densification statistic that does not cancel; the
     call then goes through rasterize_views as with filter_3d.
     normals=True: the dict also holds "normal_3dgs" [3,H,W], the differentiable normal image (rasterize_views' normals=True),
-    through rasterize_views as with filter_3d."""
+    through rasterize_views as with filter_3d.
+    geometry=True: the dict also holds "median_depth_3dgs" and "depth2_3dgs" [1,H,W] (rasterize_views' geometry=True) and
+    "distortion_3dgs" [1,H,W], geometry.depth_distortion of alpha, depth and depth2, all differentiable; through
+    rasterize_views as with filter_3d."""
     aa = bool(getattr(pipe, "antialiasing", False))
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
@@ -83,17 +87,19 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
         colors = override_color
     raw = _raw_tensors(pc) if fused_activations else None
     m2d_abs = extra["viewspace_points_abs"][None] if absgrad else None
-    if raw is None and (filter_3d is not None or absgrad or normals):
+    if raw is None and (filter_3d is not None or absgrad or normals or geometry):
         outs = rasterize_views(
             means3D=xyz, opacities=pc.get_opacity, viewmatrices=viewpoint_camera.world_view_transform[None],
             projmatrices=viewpoint_camera.full_proj_transform[None], camposs=viewpoint_camera.camera_center[None],
             tanfovx=[settings.tanfovx], tanfovy=[settings.tanfovy], image_height=settings.image_height, image_width=settings.image_width,
             bg=bg_color, sh_degree=pc.active_sh_degree, shs=shs, colors_precomp=colors, scales=pc.get_scaling,
             rotations=pc.get_rotation, means2D=screenspace_points[None], scale_modifier=scaling_modifier, antialiasing=aa,
-            filter_3d=filter_3d, means2D_abs=m2d_abs, normals=normals)
+            filter_3d=filter_3d, means2D_abs=m2d_abs, normals=normals, geometry=geometry)
         image, radii, depth, alpha = outs[0][0], outs[1][0], outs[2][0], outs[3][0]
         if normals:
             extra["normal_3dgs"] = outs[4][0]
+        if geometry:
+            _geometry_keys(extra, alpha, depth, outs[4 + normals][0], outs[5 + normals][0])
         return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
                 "depth_3dgs": depth, "alpha_3dgs": alpha, **extra}
     if raw is not None:
@@ -103,10 +109,12 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
             camposs=viewpoint_camera.camera_center[None], tanfovx=[settings.tanfovx], tanfovy=[settings.tanfovy], image_height=settings.image_height,
             image_width=settings.image_width, bg=bg_color, sh_degree=pc.active_sh_degree, shs=shs, colors_precomp=colors, scales=sc, rotations=rot,
             means2D=screenspace_points[None], scale_modifier=scaling_modifier, raw=True, antialiasing=aa, filter_3d=filter_3d,
-            means2D_abs=m2d_abs, normals=normals)
+            means2D_abs=m2d_abs, normals=normals, geometry=geometry)
         image, radii, depth, alpha = outs[0][0], outs[1][0], outs[2][0], outs[3][0]
         if normals:
             extra["normal_3dgs"] = outs[4][0]
+        if geometry:
+            _geometry_keys(extra, alpha, depth, outs[4 + normals][0], outs[5 + normals][0])
         return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
                 "depth_3dgs": depth, "alpha_3dgs": alpha, **extra}
     image, radii, depth, alpha = rasterizer(means3D=xyz, means2D=screenspace_points, shs=shs, colors_precomp=colors,
@@ -114,6 +122,12 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
                                             cov3D_precomp=None)
     return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
             "depth_3dgs": depth, "alpha_3dgs": alpha}
+
+
+def _geometry_keys(extra, alpha, depth, median, depth2):
+    extra["median_depth_3dgs"] = median
+    extra["depth2_3dgs"] = depth2
+    extra["distortion_3dgs"] = depth_distortion(alpha, depth, depth2)
 
 
 def stack_cameras(cameras, device):
@@ -139,7 +153,8 @@ class _StackSinks(torch.autograd.Function):
         return (None, *g.unbind(0))
 
 
-def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False, filter_3d=None, absgrad=False, normals=False):
+def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False, filter_3d=None, absgrad=False, normals=False,
+                 geometry=False):
     """All cameras share image size.  Returns the dict of `render` with a leading view axis:
     render [V,3,H,W], depth_3dgs/alpha_3dgs [V,1,H,W], radii [V,P], viewspace_points [V,P,3] (its .grad is [V,P,3]),
     plus viewspace_point_list: V leaf tensors [P,3] whose .grad backward fills -- what the reference's
@@ -148,7 +163,8 @@ def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False
     absgrad=True: also viewspace_points_abs [V,P,3], whose .grad is the absolute screen-space gradient (`rasterize_views`'
     means2D_abs) -- the densification statistic that does not cancel.
     normals=True: also normal_3dgs [V,3,H,W] (rasterize_views' normal image) and comp_normal [V,H,W,3], threestudio's normal
-    map of it (`comp_normal`), both differentiable."""
+    map of it (`comp_normal`), both differentiable.
+    geometry=True: also median_depth_3dgs, depth2_3dgs and distortion_3dgs [V,1,H,W], as `render`'s geometry=True."""
     xyz = pc.get_xyz
     V = len(cameras)
     vm, pm, cp, tanx, tany = stack_cameras(cameras, xyz.device)
@@ -167,10 +183,12 @@ def render_views(cameras, pc, bg_color, scaling_modifier=1.0, antialiasing=False
         image_height=int(cameras[0].image_height), image_width=int(cameras[0].image_width), bg=bg_color,
         sh_degree=pc.active_sh_degree, shs=pc.get_features, scales=pc.get_scaling, rotations=pc.get_rotation,
         means2D=screenspace_points, scale_modifier=scaling_modifier, antialiasing=antialiasing, filter_3d=filter_3d,
-        means2D_abs=extra.get("viewspace_points_abs"), normals=normals)
+        means2D_abs=extra.get("viewspace_points_abs"), normals=normals, geometry=geometry)
     image, radii, depth, alpha = outs[:4]
     if normals:
         extra["normal_3dgs"] = outs[4]
         extra["comp_normal"] = comp_normal(outs[4], alpha)
+    if geometry:
+        _geometry_keys(extra, alpha, depth, outs[4 + normals], outs[5 + normals])
     return {"render": image, "viewspace_points": screenspace_points, "viewspace_point_list": sinks, "visibility_filter": radii > 0,
             "radii": radii, "depth_3dgs": depth, "alpha_3dgs": alpha, **extra}

@@ -380,6 +380,78 @@ int b200gs_backward_deterministic_absgrad_normals_opts(const b200gs_params *prm,
                                                        int64_t *n_partials, void *abs_partials, size_t abs_partials_bytes,
                                                        void *stream);
 
+/* ---- geometry outputs: median depth and depth second moment of the blend (additive to ABI 4) ---------------------------
+ * For view v and pixel p, over the blends of p in the colour's order, with the colour's alpha, T (before the blend),
+ * w = alpha * T and d the Gaussian's view-space depth (DESIGN.md section 2):
+ *   depth2   out_depth2[v,0,p] = M2 = sum w d^2, accumulated as M2 = fma(d * d, w, M2).  No background term; 0 where nothing
+ *            blends.  With alpha and depth: the depth distortion sum_{i<j} w_i w_j (d_i - d_j)^2 = A * M2 - M1^2.
+ *   median   out_median[v,0,p] = d of the LAST blend whose T is > 0.5 (strict, on the float32 T): the blend at which T
+ *            crosses 1/2, or the last blend if T never reaches it.  0 where nothing blends.  median_pos[v,p] = its 1-based
+ *            position in the tile's list (0 = none).
+ *   grads    dL/dM2 enters dL/dalpha as cg += d^2 dL/dM2, and adds sum_p w 2d dL/dM2 to the Gaussian's depth gradient.
+ *            dL/dmedian adds dL/dmedian_p to the depth gradient of p's median Gaussian only (the selection is piecewise
+ *            constant: no alpha-path term).  Both reach the means through the existing depth term.
+ * Colour, depth, alpha, normals, radii and the state buffers are byte-identical to the call without geometry, and the
+ * deterministic partial count is unchanged.  Combines with SH or precomputed colours, raw parameters, cov3D_precomp,
+ * antialiasing, the 3D filter, per-view means, normals, absgrad and the deterministic backward.  The classic comparator and
+ * the bulk-copy build return B200GS_E_UNSUPPORTED; the contribution forward has no geometry form.
+ *   struct_bytes   sizeof(b200gs_geometry_io) (a smaller value is B200GS_E_ARGS)
+ *   out_median     [V,1,H,W] (forward output; NULL in a forward is B200GS_E_ARGS)
+ *   out_depth2     [V,1,H,W] (forward output; NULL in a forward is B200GS_E_ARGS)
+ *   median_pos     [V,H,W] x u32 device workspace, 4-byte aligned (else B200GS_E_BUFFER; NULL is B200GS_E_ARGS): the forward
+ *                  writes it, the backward reads it, so it must survive from the forward to its backward like the state buffers
+ *   dL_dmedian     [V,1,H,W] (backward input); NULL = zero
+ *   dL_ddepth2     [V,1,H,W] (backward input); NULL = zero.  With both NULL the backward is exactly the call without geometry.
+ * Each entry point takes a nullable b200gs_normals_io (NULL: no normals; otherwise as the normals forms, including its
+ * errors) and the geometry io after opts.  The forward takes b200gs_forward_opts' arguments after them.  The backward forms
+ * take the arguments of b200gs_backward_absgrad_opts and b200gs_backward_deterministic_absgrad_opts, with dL_dmeans2D_abs
+ * nullable (NULL: no absolute gradients, and abs_partials is then not read).  A NULL geometry io is B200GS_E_ARGS. */
+typedef struct b200gs_geometry_io {
+    int32_t struct_bytes;
+    float *out_median;
+    float *out_depth2;
+    uint32_t *median_pos;
+    const float *dL_dmedian;
+    const float *dL_ddepth2;
+} b200gs_geometry_io;
+int b200gs_forward_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+                                 const b200gs_geometry_io *geo,
+                                 const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
+                                 const float *scales, const float *rotations, const float *cov3D_precomp,
+                                 const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
+                                 float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
+                                 void *geom_buf, size_t geom_bytes,
+                                 void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
+                                 void *image_buf, size_t image_bytes,
+                                 int64_t *num_rendered, void *stream);
+int b200gs_backward_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
+                                  const b200gs_geometry_io *geo,
+                                  const float *means3D, const float *shs, const float *colors_precomp,
+                                  const float *opacities, const float *scales, const float *rotations,
+                                  const float *cov3D_precomp, const float *bg, const float *viewmatrix,
+                                  const float *projmatrix, const float *campos, const int32_t *radii,
+                                  const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                  const void *image_buf, int64_t num_rendered,
+                                  const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                  float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                                  float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                  float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream);
+int b200gs_backward_deterministic_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
+                                                const b200gs_normals_io *nrm, const b200gs_geometry_io *geo,
+                                                const float *means3D, const float *shs, const float *colors_precomp,
+                                                const float *opacities, const float *scales, const float *rotations,
+                                                const float *cov3D_precomp, const float *bg, const float *viewmatrix,
+                                                const float *projmatrix, const float *campos, const int32_t *radii,
+                                                const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
+                                                const void *image_buf, int64_t num_rendered,
+                                                const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                                float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
+                                                float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
+                                                float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes,
+                                                void *det_buf, size_t det_bytes, int64_t partial_capacity,
+                                                int64_t *n_partials, void *abs_partials, size_t abs_partials_bytes,
+                                                void *stream);
+
 /* ---- 3D smoothing filter: per-Gaussian maximal sampling rate over a camera set (Mip-Splatting's 3D filter) ------------
  * For each of the n_views cameras (viewmatrix [n_views,16] device, tanfovx / tanfovy host [n_views], shared H x W), with
  * (tx, ty, tz) the preprocess's view-space position and fx = W / (2 tanfovx), fy = H / (2 tanfovy): Gaussian k is in view
