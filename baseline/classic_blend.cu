@@ -158,35 +158,21 @@ __global__ void __launch_bounds__(BLOCK_SIZE) classic_bwd(BlendBwdArgs a)
     }
 }
 
-void launch_blend_fwd(const BlendArgs &a, cudaStream_t st)
+// the plain forward and atomic backward only: a call that turns on any optional feature, or the deterministic backward,
+// returns B200GS_E_UNSUPPORTED before a launcher would see it
+int blend_caps() { return 0; }
+void launch_blend_fwd(const BlendArgs &a, const ContribOut *, const float4 *, float *, const GeoFwd *, cudaStream_t st)
 {
     dim3 grid(a.grid_x * a.grid_y, a.V);
     classic_fwd<<<grid, BLOCK_SIZE, 0, st>>>(a);
 }
-void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st)
+void launch_blend_bwd(const BlendBwdArgs &a, const DetFlush *, bool, const NrmBwd *, const GeoBwd *, cudaStream_t st)
 {
     dim3 grid(a.grid_x * a.grid_y, a.V);
     classic_bwd<<<grid, BLOCK_SIZE, 0, st>>>(a);
 }
 int blend_sgrad_is_moments() { return 0; }
-// no contribution scores: b200gs_forward_contrib_opts returns B200GS_E_UNSUPPORTED before this would run
-int blend_fwd_has_contrib() { return 0; }
-void launch_blend_fwd_contrib(const BlendArgs &, const ContribOut &, cudaStream_t) {}
-// no deterministic backward here: b200gs_backward_deterministic returns B200GS_E_UNSUPPORTED before it would launch this
-int blend_bwd_has_deterministic() { return 0; }
-void launch_blend_bwd_det(const BlendBwdArgs &, const DetFlush &, cudaStream_t) {}
-// nor the absolute screen-space gradients: the absgrad entry points return B200GS_E_UNSUPPORTED before these would run
-int blend_bwd_has_absgrad() { return 0; }
-void launch_blend_bwd_abs(const BlendBwdArgs &, const DetFlush *, cudaStream_t) {}
 void launch_absgrad_out(int64_t, int, int, const int32_t *, const GeomRec *, const void *, float *, cudaStream_t) {}
-// nor the normal maps: the normals entry points return B200GS_E_UNSUPPORTED before these would run
-int blend_has_normals() { return 0; }
-void launch_blend_fwd_nrm(const BlendArgs &, const float4 *, float *, cudaStream_t) {}
-void launch_blend_bwd_nrm(const BlendBwdArgs &, const DetFlush *, bool, const NrmBwd &, cudaStream_t) {}
-// nor the geometry outputs: the geometry entry points return B200GS_E_UNSUPPORTED before these would run
-int blend_has_geometry() { return 0; }
-void launch_blend_fwd_geo(const BlendArgs &, const float4 *, float *, const GeoFwd &, cudaStream_t) {}
-void launch_blend_bwd_geo(const BlendBwdArgs &, const DetFlush *, bool, const NrmBwd *, const GeoBwd &, cudaStream_t) {}
 __global__ void classic_exp_kernel(const float *x, float *y, int64_t n)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

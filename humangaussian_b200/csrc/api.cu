@@ -100,37 +100,50 @@ static int check_common(const b200gs_params *p, const float *shs, const float *c
     return B200GS_OK;
 }
 
-// b200gs_render_opts: NULL = the defaults; a struct too short to hold the fields this library reads is an argument error.
-// struct_bytes = 8 is the header before filter3d_var (no 3D filter); a size that cuts that pointer is an argument error.
-static int read_opts(const b200gs_render_opts *o, bool *aa, const float **f3d)
+// One call's options (b200gs_render_opts, include/b200gs.h): the caller's fields, zero past its struct_bytes, and the features
+// they turn on.
+struct Opts {
+    b200gs_render_opts o;
+    bool aa, nrm, geo, contrib, absgrad;
+};
+
+// Parses and checks the options of a forward (bwd false) or backward call: the struct_bytes rule, which features are on, the
+// build's support for them and the deterministic backward (before any other check), and the option fields each feature needs.
+// The deterministic backward's partial arrays are checked with det_buf.
+static int read_opts(const b200gs_render_opts *in, bool bwd, bool det, const float *cov3D_precomp, Opts *r)
 {
-    *aa = false;
-    *f3d = nullptr;
-    if (!o) return B200GS_OK;
-    const int32_t n0 = (int32_t)(offsetof(b200gs_render_opts, antialiasing) + sizeof(o->antialiasing));
-    const int32_t n1 = (int32_t)(offsetof(b200gs_render_opts, filter3d_var) + sizeof(o->filter3d_var));
-    if (o->struct_bytes < n0 || (o->struct_bytes > n0 && o->struct_bytes < n1)) return B200GS_E_ARGS;
-    *aa = o->antialiasing != 0;
-    if (o->struct_bytes >= n1) *f3d = o->filter3d_var;
+    *r = Opts{};
+    if (in) {
+        const int32_t n = in->struct_bytes;
+        if (n != 8 && n != 16 && n < (int32_t)sizeof(b200gs_render_opts)) return B200GS_E_ARGS;
+        memcpy(&r->o, in, n < (int32_t)sizeof(b200gs_render_opts) ? (size_t)n : sizeof(b200gs_render_opts));
+    }
+    const b200gs_render_opts &o = r->o;
+    r->aa = o.antialiasing != 0;
+    r->nrm = o.gauss_normals && (!bwd || o.dL_dnormal);
+    r->geo = bwd ? (o.dL_dmedian || o.dL_ddepth2) : o.median_pos != nullptr;
+    r->contrib = !bwd && (o.weight_sum || o.weight_max || o.touches);
+    r->absgrad = bwd && o.dL_dmeans2D_abs;
+    const int need = (r->contrib ? BLEND_CAP_CONTRIB : 0) | (r->nrm ? BLEND_CAP_NORMALS : 0) | (r->geo ? BLEND_CAP_GEOMETRY : 0) |
+                     (r->absgrad ? BLEND_CAP_ABSGRAD : 0) | (det ? BLEND_CAP_DETERMINISTIC : 0);
+    if (need & ~blend_caps()) return B200GS_E_UNSUPPORTED;
+    if (o.filter3d_var && cov3D_precomp) return B200GS_E_ARGS; // the 3D filter widens scales; a precomputed covariance has none
+    if (r->contrib && (!o.weight_sum || !o.weight_max || !o.touches || r->nrm || r->geo)) return B200GS_E_ARGS;
+    if (bwd && o.dL_dnormal && !o.gauss_normals) return B200GS_E_ARGS;
+    if (r->nrm) { // no axis without scales
+        if (cov3D_precomp) return B200GS_E_ARGS;
+        if (((uintptr_t)o.gauss_normals) & 15) return B200GS_E_BUFFER;
+        if (bwd ? !o.normal_wn : !o.out_normal) return B200GS_E_ARGS;
+        if (bwd && (((uintptr_t)o.normal_wn) & 15)) return B200GS_E_BUFFER;
+    }
+    if (r->geo) {
+        if (!o.median_pos) return B200GS_E_ARGS;
+        if (((uintptr_t)o.median_pos) & 3) return B200GS_E_BUFFER;
+        if (!bwd && (!o.out_median || !o.out_depth2)) return B200GS_E_ARGS;
+    }
     return B200GS_OK;
 }
 
-// b200gs_normals_io: the fields every normals call reads (the build, the struct, the workspace; no axis without scales)
-static int check_normals_io(const b200gs_normals_io *n, const float *cov3D_precomp)
-{
-    if (!blend_has_normals()) return B200GS_E_UNSUPPORTED;
-    if (!n || n->struct_bytes < (int32_t)sizeof(b200gs_normals_io) || !n->gauss_normals || cov3D_precomp) return B200GS_E_ARGS;
-    if (((uintptr_t)n->gauss_normals) & 15) return B200GS_E_BUFFER;
-    return B200GS_OK;
-}
-// b200gs_geometry_io: the fields every geometry call reads (the build, the struct, the median-position workspace)
-static int check_geometry_io(const b200gs_geometry_io *g)
-{
-    if (!blend_has_geometry()) return B200GS_E_UNSUPPORTED;
-    if (!g || g->struct_bytes < (int32_t)sizeof(b200gs_geometry_io) || !g->median_pos) return B200GS_E_ARGS;
-    if (((uintptr_t)g->median_pos) & 3) return B200GS_E_BUFFER;
-    return B200GS_OK;
-}
 static NormalArgs normal_args(const b200gs_params *prm, const float *means3D, const float *scales, const float *rotations,
                               const float *campos)
 {
@@ -141,32 +154,19 @@ static NormalArgs normal_args(const b200gs_params *prm, const float *means3D, co
     return n;
 }
 
-// b200gs_forward_opts (contrib NULL) and b200gs_forward_contrib_opts (the blend with the contribution scores)
 static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
                         const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
                         const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
                         const float *campos, float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf,
                         size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf,
-                        size_t image_bytes, int64_t *num_rendered, void *stream, const ContribOut *contrib,
-                        const b200gs_normals_io *nrm = nullptr, const b200gs_geometry_io *geo = nullptr)
+                        size_t image_bytes, int64_t *num_rendered, void *stream)
 {
-    bool aa = false;
-    const float *f3d = nullptr;
-    int rc = read_opts(opts, &aa, &f3d);
+    Opts op;
+    int rc = read_opts(opts, false, false, cov3D_precomp, &op);
     if (rc) return rc;
+    const b200gs_render_opts &o = op.o;
     rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
-    if (f3d && cov3D_precomp) return B200GS_E_ARGS; // the 3D filter widens scales; a precomputed covariance has none
-    if (nrm) {
-        rc = check_normals_io(nrm, cov3D_precomp);
-        if (rc) return rc;
-        if (!nrm->out_normal) return B200GS_E_ARGS;
-    }
-    if (geo) {
-        rc = check_geometry_io(geo);
-        if (rc) return rc;
-        if (!geo->out_median || !geo->out_depth2) return B200GS_E_ARGS;
-    }
     if (!means3D || !opacities || !bg || !viewmatrix || !projmatrix || !campos || !out_color || !out_depth || !out_alpha ||
         !radii || !geom_buf || !binning_buf || !image_buf || !num_rendered)
         return B200GS_E_ARGS;
@@ -179,7 +179,6 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
     if (geom_bytes < GL.total || image_bytes < IL.total || binning_bytes < BL.total) return B200GS_E_BUFFER;
     if ((((uintptr_t)geom_buf) | ((uintptr_t)binning_buf) | ((uintptr_t)image_buf)) & 15) return B200GS_E_BUFFER; // records are 128-bit accessed
     char *gb = (char *)geom_buf, *bb = (char *)binning_buf, *ib = (char *)image_buf;
-    const size_t HW = (size_t)H * W;
     *num_rendered = 0;
     HostSlot *pending = nullptr;
 
@@ -202,10 +201,10 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
         a.dkeys = (uint32_t *)(bb + BL.dkeys_in); a.order_in = (uint32_t *)(bb + BL.order_in);
         {
             StageTimer t(B200GS_STAGE_PREPROCESS, st);
-            launch_preprocess_fwd(a, V, aa, f3d, st);
-            if (nrm) launch_normal_prep(normal_args(prm, means3D, scales, rotations, campos), (float4 *)nrm->gauss_normals, st);
+            launch_preprocess_fwd(a, V, op.aa, o.filter3d_var, st);
+            if (op.nrm) launch_normal_prep(normal_args(prm, means3D, scales, rotations, campos), (float4 *)o.gauss_normals, st);
         }
-        g_launches += nrm ? 2 : 1;
+        g_launches += op.nrm ? 2 : 1;
         uint32_t *offsets = (uint32_t *)(gb + GL.offsets); // inclusive scan of tiles_touched in DEPTH order
         const int64_t n_vp = (int64_t)P * V;
         const uint32_t *order_sorted = nullptr;
@@ -223,7 +222,7 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
         int64_t cap = instance_capacity < B200GS_MAX_INSTANCES ? instance_capacity : (int64_t)B200GS_MAX_INSTANCES;
         if (cap < 1) cap = 1; // the layout always has room for one instance
         // (the contribution scores are accumulators: a call that does not fit must not reach the blend, so it always waits)
-        if (n_vp <= B200GS_DEFERRED_MAX_NVP && !contrib) {
+        if (n_vp <= B200GS_DEFERRED_MAX_NVP && !op.contrib) {
             // Small batches (the per-view drop-in pattern, the 8-view SDS batch): the host does NOT wait here.  Emit / tile
             // sort / ranges / blend are enqueued sized for the caller's capacity and read the count on the device, so the GPU
             // never idles behind a host round trip (upstream blocks on this read-back in the middle of every forward).  The
@@ -258,15 +257,12 @@ static int forward_impl(const b200gs_params *prm, const b200gs_render_opts *opts
     b.final_T = (float *)(ib + IL.final_T); b.n_contrib = (uint32_t *)(ib + IL.n_contrib);
     b.out_color = out_color; b.out_depth = out_depth; b.out_alpha = out_alpha;
     b.cmask = (uint32_t *)(bb + BL.cmask);
-    (void)HW;
+    const ContribOut co{o.weight_sum, o.weight_max, o.touches};
+    const GeoFwd gf{o.out_median, o.out_depth2, o.median_pos};
     {
         StageTimer t(B200GS_STAGE_BLEND_FWD, st);
-        if (contrib) launch_blend_fwd_contrib(b, *contrib, st);
-        else if (geo)
-            launch_blend_fwd_geo(b, nrm ? (const float4 *)nrm->gauss_normals : nullptr, nrm ? nrm->out_normal : nullptr,
-                                 GeoFwd{geo->out_median, geo->out_depth2, geo->median_pos}, st);
-        else if (nrm) launch_blend_fwd_nrm(b, (const float4 *)nrm->gauss_normals, nrm->out_normal, st);
-        else launch_blend_fwd(b, st);
+        launch_blend_fwd(b, op.contrib ? &co : nullptr, op.nrm ? (const float4 *)o.gauss_normals : nullptr, o.out_normal,
+                         op.geo ? &gf : nullptr, st);
         g_launches += 1;
     }
     CK(cudaGetLastError(), "forward launch");
@@ -289,51 +285,7 @@ int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts
 {
     return forward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
                         projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
-                        instance_capacity, image_buf, image_bytes, num_rendered, stream, nullptr);
-}
-
-int b200gs_forward_contrib_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
-                                const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
-                                const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
-                                const float *campos, float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
-                                void *geom_buf, size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
-                                void *image_buf, size_t image_bytes, int64_t *num_rendered, uint64_t *weight_sum,
-                                uint32_t *weight_max, uint32_t *touches, void *stream)
-{
-    if (!blend_fwd_has_contrib()) return B200GS_E_UNSUPPORTED;
-    if (!weight_sum || !weight_max || !touches) return B200GS_E_ARGS;
-    const ContribOut co{weight_sum, weight_max, touches};
-    return forward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
-                        projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
-                        instance_capacity, image_buf, image_bytes, num_rendered, stream, &co);
-}
-
-int b200gs_forward_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-                                const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
-                                const float *scales, const float *rotations, const float *cov3D_precomp, const float *bg,
-                                const float *viewmatrix, const float *projmatrix, const float *campos, float *out_color,
-                                float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf, size_t geom_bytes,
-                                void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf,
-                                size_t image_bytes, int64_t *num_rendered, void *stream)
-{
-    if (!nrm) return B200GS_E_ARGS;
-    return forward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
-                        projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
-                        instance_capacity, image_buf, image_bytes, num_rendered, stream, nullptr, nrm);
-}
-
-int b200gs_forward_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-                                 const b200gs_geometry_io *geo, const float *means3D, const float *shs, const float *colors_precomp,
-                                 const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
-                                 const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                                 float *out_color, float *out_depth, float *out_alpha, int32_t *radii, void *geom_buf,
-                                 size_t geom_bytes, void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
-                                 void *image_buf, size_t image_bytes, int64_t *num_rendered, void *stream)
-{
-    if (!geo) return B200GS_E_ARGS;
-    return forward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
-                        projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
-                        instance_capacity, image_buf, image_bytes, num_rendered, stream, nullptr, nrm, geo);
+                        instance_capacity, image_buf, image_bytes, num_rendered, stream);
 }
 
 int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
@@ -343,9 +295,9 @@ int b200gs_forward(const b200gs_params *prm, const float *means3D, const float *
                    void *binning_buf, size_t binning_bytes, int64_t instance_capacity, void *image_buf, size_t image_bytes,
                    int64_t *num_rendered, void *stream)
 {
-    return b200gs_forward_opts(prm, nullptr, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
-                               projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf,
-                               binning_bytes, instance_capacity, image_buf, image_bytes, num_rendered, stream);
+    return forward_impl(prm, nullptr, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix,
+                        projmatrix, campos, out_color, out_depth, out_alpha, radii, geom_buf, geom_bytes, binning_buf, binning_bytes,
+                        instance_capacity, image_buf, image_bytes, num_rendered, stream);
 }
 
 size_t b200gs_deterministic_bytes(int64_t num_rendered, int64_t partial_capacity, int32_t P, int32_t V)
@@ -353,8 +305,7 @@ size_t b200gs_deterministic_bytes(int64_t num_rendered, int64_t partial_capacity
     return DetLayout(num_rendered, partial_capacity, (int64_t)(P > 0 ? P : 0) * (V > 0 ? V : 0)).total;
 }
 
-// b200gs_backward (det == false) and b200gs_backward_deterministic (det == true); dL_dmeans2D_abs != NULL: the absgrad forms
-// (abs_partials: the deterministic one's [partial_capacity] float2 array)
+// b200gs_backward[_opts] (det == false) and b200gs_backward_deterministic[_opts] (det == true)
 static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs, const float *colors_precomp,
                          const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
                          const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
@@ -362,51 +313,31 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
                          const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth,
                          const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
                          float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, void *scratch,
-                         size_t scratch_bytes, void *stream, bool det, void *det_buf, size_t det_bytes, int64_t partial_capacity,
-                         int64_t *n_partials, bool absgrad = false, float *dL_dmeans2D_abs = nullptr, void *abs_partials = nullptr,
-                         size_t abs_partials_bytes = 0, const b200gs_normals_io *nio = nullptr,
-                         const b200gs_geometry_io *gio = nullptr)
+                         size_t scratch_bytes, bool det, void *det_buf, size_t det_bytes, int64_t partial_capacity,
+                         int64_t *n_partials, void *stream)
 {
-    bool aa = false;
-    const float *f3d = nullptr;
-    if (absgrad && !blend_bwd_has_absgrad()) return B200GS_E_UNSUPPORTED;
-    // a geometry call without either geometry gradient is exactly the call without geometry
-    const b200gs_geometry_io *geo =
-        gio && gio->struct_bytes >= (int32_t)sizeof(b200gs_geometry_io) && !gio->dL_dmedian && !gio->dL_ddepth2 ? nullptr : gio;
-    if (geo) {
-        const int rc = check_geometry_io(geo);
-        if (rc) return rc;
-    }
-    // a normals call without dL_dnormal is exactly the call without normals
-    const b200gs_normals_io *nrm = nio && nio->struct_bytes >= (int32_t)sizeof(b200gs_normals_io) && !nio->dL_dnormal ? nullptr : nio;
-    if (nrm) {
-        const int rc = check_normals_io(nrm, cov3D_precomp);
-        if (rc) return rc;
-        if (!nrm->normal_wn) return B200GS_E_ARGS;
-        if (((uintptr_t)nrm->normal_wn) & 15) return B200GS_E_BUFFER;
-        if (det) {
-            if (!nrm->nrm_partials) return B200GS_E_ARGS;
-            if ((((uintptr_t)nrm->nrm_partials) & 15) || (partial_capacity > 0 && nrm->nrm_partials_bytes < (size_t)partial_capacity * 16))
-                return B200GS_E_BUFFER;
-        }
-    }
-    if (read_opts(opts, &aa, &f3d)) return B200GS_E_ARGS;
-    if (f3d && cov3D_precomp) return B200GS_E_ARGS;
-    if (absgrad && !dL_dmeans2D_abs) return B200GS_E_ARGS;
+    Opts op;
+    int rc = read_opts(opts, true, det, cov3D_precomp, &op);
+    if (rc) return rc;
+    const b200gs_render_opts &o = op.o;
+    const bool nrm = op.nrm, absgrad = op.absgrad;
     if (det) {
-        if (!blend_bwd_has_deterministic()) return B200GS_E_UNSUPPORTED;
         if (!n_partials || !det_buf || partial_capacity < 0) return B200GS_E_ARGS;
         *n_partials = 0;
         if (num_rendered < 0 || num_rendered > instance_capacity || num_rendered > B200GS_MAX_INSTANCES) return B200GS_E_ARGS;
         if (((uintptr_t)det_buf) & 15) return B200GS_E_BUFFER;
         if (absgrad) {
-            if (!abs_partials) return B200GS_E_ARGS;
-            if ((((uintptr_t)abs_partials) & 7) || abs_partials_bytes < (size_t)partial_capacity * sizeof(float2)) return B200GS_E_BUFFER;
+            if (!o.abs_partials) return B200GS_E_ARGS;
+            if ((((uintptr_t)o.abs_partials) & 7) || o.abs_partials_bytes < (size_t)partial_capacity * sizeof(float2)) return B200GS_E_BUFFER;
+        }
+        if (nrm) {
+            if (!o.nrm_partials) return B200GS_E_ARGS;
+            if ((((uintptr_t)o.nrm_partials) & 15) || o.nrm_partials_bytes < (size_t)partial_capacity * 16) return B200GS_E_BUFFER;
         }
     }
-    int rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
+    rc = check_common(prm, shs, colors_precomp, scales, rotations, cov3D_precomp);
     if (rc) return rc;
-    if ((prm->raw_params || aa || f3d) && !opacities) return B200GS_E_ARGS;
+    if ((prm->raw_params || op.aa || o.filter3d_var) && !opacities) return B200GS_E_ARGS;
     if (!means3D || !bg || !viewmatrix || !projmatrix || !campos || !radii || !geom_buf || !binning_buf || !image_buf ||
         !dL_dmeans3D || !dL_dmeans2D || !dL_dopacity || !scratch)
         return B200GS_E_ARGS;
@@ -427,10 +358,10 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     if (det && det_bytes < DL.total) return B200GS_E_BUFFER;
 
     if (!det) CK(cudaMemsetAsync(scratch, 0, (size_t)P * V * sizeof(ScreenGrad), st), "memset scratch");
-    if (!det && nrm) CK(cudaMemsetAsync(nrm->normal_wn, 0, (size_t)P * V * 16, st), "memset normal_wn");
-    const NrmBwd nb{nrm ? (const float4 *)nrm->gauss_normals : nullptr, nrm ? nrm->dL_dnormal : nullptr,
-                    nrm ? (float4 *)nrm->normal_wn : nullptr, nrm ? (float4 *)nrm->nrm_partials : nullptr};
-    const GeoBwd gbw{geo ? geo->dL_dmedian : nullptr, geo ? geo->dL_ddepth2 : nullptr, geo ? geo->median_pos : nullptr};
+    if (!det && nrm) CK(cudaMemsetAsync(o.normal_wn, 0, (size_t)P * V * 16, st), "memset normal_wn");
+    const NrmBwd nb = nrm ? NrmBwd{(const float4 *)o.gauss_normals, o.dL_dnormal, (float4 *)o.normal_wn, (float4 *)o.nrm_partials}
+                          : NrmBwd{};
+    const GeoBwd gbw{o.dL_dmedian, o.dL_ddepth2, o.median_pos};
     BlendBwdArgs b;
     b.H = H; b.W = W; b.grid_x = gx; b.grid_y = gy; b.V = V; b.P = P;
     b.ranges = (const uint2 *)(bb + BL.ranges); b.point_list = (const uint32_t *)(bb + BL.vals_out);
@@ -442,10 +373,7 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     b.sgrad = scratch;
     if (!det) {
         StageTimer t(B200GS_STAGE_BLEND_BWD, st);
-        if (geo) launch_blend_bwd_geo(b, nullptr, absgrad, nrm ? &nb : nullptr, gbw, st);
-        else if (nrm) launch_blend_bwd_nrm(b, nullptr, absgrad, nb, st);
-        else if (absgrad) launch_blend_bwd_abs(b, nullptr, st);
-        else launch_blend_bwd(b, st);
+        launch_blend_bwd(b, nullptr, absgrad, nrm ? &nb : nullptr, op.geo ? &gbw : nullptr, st);
     } else {
         // pre-pass -> (the one host wait: the partial count) -> B1 with per-partial stores -> fixed-order reduce.  The wait
         // sits after the scan so that a call whose partials do not fit returns before B1 runs; every access of the pre-pass
@@ -476,21 +404,15 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
         if (H_partials > 0xffffffffull) return B200GS_E_RANGE; // 32-bit slots; 160 GB of partials would not fit a device anyway
         if ((int64_t)H_partials > partial_capacity) return B200GS_E_BIN_TOO_SMALL;
         float *partials = (float *)(db + DL.partials);
-        float2 *abs_p = absgrad ? (float2 *)abs_partials : nullptr;
+        float2 *abs_p = absgrad ? (float2 *)o.abs_partials : nullptr;
         const DetFlush flush{pa.pm, pa.base, partials, abs_p};
-        if (H_partials > 0) {
-            if (geo) launch_blend_bwd_geo(b, &flush, absgrad, nrm ? &nb : nullptr, gbw, st);
-            else if (nrm) launch_blend_bwd_nrm(b, &flush, absgrad, nb, st);
-            else if (absgrad) launch_blend_bwd_abs(b, &flush, st);
-            else launch_blend_bwd_det(b, flush, st);
-        }
-        if (nrm) launch_det_reduce_nrm(pa, n_vp, partials, abs_p, scratch, nb.partials, nb.wn, st);
-        else launch_det_reduce(pa, n_vp, partials, abs_p, scratch, st);
+        if (H_partials > 0) launch_blend_bwd(b, &flush, absgrad, nrm ? &nb : nullptr, op.geo ? &gbw : nullptr, st);
+        launch_det_reduce(pa, n_vp, partials, abs_p, scratch, nb.partials, nb.wn, st);
         g_launches += (H_partials > 0) + 1;
     }
     if (absgrad) {
         StageTimer t(B200GS_STAGE_BLEND_BWD, st);
-        launch_absgrad_out(n_vp, H, W, radii, b.recs, scratch, dL_dmeans2D_abs, st);
+        launch_absgrad_out(n_vp, H, W, radii, b.recs, scratch, o.dL_dmeans2D_abs, st);
         g_launches += 1;
     }
 
@@ -506,10 +428,10 @@ static int backward_impl(const b200gs_params *prm, const b200gs_render_opts *opt
     a.recs = (const GeomRec *)(gb + GL.recs); a.moments = blend_sgrad_is_moments();
     a.dL_dmeans3D = dL_dmeans3D; a.dL_dmeans2D = dL_dmeans2D; a.dL_dsh = dL_dsh; a.dL_dcolors = dL_dcolors;
     a.dL_dopacity = dL_dopacity; a.dL_dscales = dL_dscales; a.dL_drots = dL_drots; a.dL_dcov3D = dL_dcov3D;
-    a.f3d_var = f3d;
+    a.f3d_var = o.filter3d_var;
     {
         StageTimer t(B200GS_STAGE_PREPROCESS_BWD, st);
-        launch_preprocess_bwd(a, aa, f3d != nullptr, st);
+        launch_preprocess_bwd(a, op.aa, o.filter3d_var != nullptr, st);
         // dL/dn through the rotations, added to what the preprocess backward wrote
         if (nrm) launch_normal_bwd(normal_args(prm, means3D, scales, rotations, campos), radii, nb.gauss_normals, nb.wn, dL_drots, st);
     }
@@ -530,7 +452,7 @@ int b200gs_backward_opts(const b200gs_params *prm, const b200gs_render_opts *opt
     return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                          campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr);
+                         scratch, scratch_bytes, false, nullptr, 0, 0, nullptr, stream);
 }
 
 int b200gs_backward(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
@@ -545,7 +467,7 @@ int b200gs_backward(const b200gs_params *prm, const float *means3D, const float 
     return backward_impl(prm, nullptr, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                          campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr);
+                         scratch, scratch_bytes, false, nullptr, 0, 0, nullptr, stream);
 }
 
 int b200gs_backward_deterministic_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D,
@@ -561,7 +483,7 @@ int b200gs_backward_deterministic_opts(const b200gs_params *prm, const b200gs_re
     return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                          campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials);
+                         scratch, scratch_bytes, true, det_buf, det_bytes, partial_capacity, n_partials, stream);
 }
 
 int b200gs_backward_deterministic(const b200gs_params *prm, const float *means3D, const float *shs, const float *colors_precomp,
@@ -577,142 +499,7 @@ int b200gs_backward_deterministic(const b200gs_params *prm, const float *means3D
     return backward_impl(prm, nullptr, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
                          campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
                          dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials);
-}
-
-int b200gs_backward_absgrad_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D, const float *shs,
-                                 const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
-                                 const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
-                                 const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf,
-                                 int64_t instance_capacity, const void *image_buf, int64_t num_rendered, const float *dL_dcolor,
-                                 const float *dL_ddepth, const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
-                                 float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                 float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream)
-{
-    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
-                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr, true, dL_dmeans2D_abs);
-}
-
-int b200gs_backward_deterministic_absgrad_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const float *means3D,
-                                               const float *shs, const float *colors_precomp, const float *opacities,
-                                               const float *scales, const float *rotations, const float *cov3D_precomp,
-                                               const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                                               const int32_t *radii, const void *geom_buf, const void *binning_buf,
-                                               int64_t instance_capacity, const void *image_buf, int64_t num_rendered,
-                                               const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                               float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                                               float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                               float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *det_buf,
-                                               size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *abs_partials,
-                                               size_t abs_partials_bytes, void *stream)
-{
-    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
-                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials, true, dL_dmeans2D_abs,
-                         abs_partials, abs_partials_bytes);
-}
-
-// the normals forms of the four backward entry points: b200gs_normals_io after opts (include/b200gs.h)
-int b200gs_backward_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-    const float *means3D, const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
-    const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
-    const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-    float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
-    float *dL_drots, float *dL_dcov3D, void *scratch, size_t scratch_bytes, void *stream)
-{
-    if (!nrm) return B200GS_E_ARGS;
-    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
-                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr, false, nullptr, nullptr, 0, nrm);
-}
-
-int b200gs_backward_deterministic_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-    const float *means3D, const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
-    const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
-    const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-    float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
-    float *dL_drots, float *dL_dcov3D, void *scratch, size_t scratch_bytes, void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials,
-    void *stream)
-{
-    if (!nrm) return B200GS_E_ARGS;
-    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
-                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials, false, nullptr,
-                         nullptr, 0, nrm);
-}
-
-int b200gs_backward_absgrad_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-    const float *means3D, const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
-    const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
-    const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-    float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
-    float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream)
-{
-    if (!nrm) return B200GS_E_ARGS;
-    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
-                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr, true, dL_dmeans2D_abs, nullptr, 0, nrm);
-}
-
-int b200gs_backward_deterministic_absgrad_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
-    const b200gs_normals_io *nrm, const float *means3D, const float *shs, const float *colors_precomp, const float *opacities, const float *scales,
-    const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix, const float *projmatrix,
-    const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-    const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-    float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
-    float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *det_buf,
-    size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *abs_partials, size_t abs_partials_bytes, void *stream)
-{
-    if (!nrm) return B200GS_E_ARGS;
-    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
-                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials, true,
-                         dL_dmeans2D_abs, abs_partials, abs_partials_bytes, nrm);
-}
-
-// the geometry forms of the backward: nullable normals io and absgrad output, then the geometry io (include/b200gs.h)
-int b200gs_backward_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-    const b200gs_geometry_io *geo, const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
-    const float *scales, const float *rotations, const float *cov3D_precomp, const float *bg, const float *viewmatrix,
-    const float *projmatrix, const float *campos, const int32_t *radii, const void *geom_buf, const void *binning_buf,
-    int64_t instance_capacity, const void *image_buf, int64_t num_rendered, const float *dL_dcolor, const float *dL_ddepth,
-    const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
-    float *dL_dscales, float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream)
-{
-    if (!geo) return B200GS_E_ARGS;
-    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
-                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, false, nullptr, 0, 0, nullptr, dL_dmeans2D_abs != nullptr, dL_dmeans2D_abs,
-                         nullptr, 0, nrm, geo);
-}
-
-int b200gs_backward_deterministic_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
-    const b200gs_normals_io *nrm, const b200gs_geometry_io *geo, const float *means3D, const float *shs, const float *colors_precomp,
-    const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp, const float *bg,
-    const float *viewmatrix, const float *projmatrix, const float *campos, const int32_t *radii, const void *geom_buf,
-    const void *binning_buf, int64_t instance_capacity, const void *image_buf, int64_t num_rendered, const float *dL_dcolor,
-    const float *dL_ddepth, const float *dL_dalpha, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-    float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs, void *scratch,
-    size_t scratch_bytes, void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *abs_partials,
-    size_t abs_partials_bytes, void *stream)
-{
-    if (!geo) return B200GS_E_ARGS;
-    return backward_impl(prm, opts, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bg, viewmatrix, projmatrix,
-                         campos, radii, geom_buf, binning_buf, instance_capacity, image_buf, num_rendered, dL_dcolor, dL_ddepth,
-                         dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drots, dL_dcov3D,
-                         scratch, scratch_bytes, stream, true, det_buf, det_bytes, partial_capacity, n_partials,
-                         dL_dmeans2D_abs != nullptr, dL_dmeans2D_abs, abs_partials, abs_partials_bytes, nrm, geo);
+                         scratch, scratch_bytes, true, det_buf, det_bytes, partial_capacity, n_partials, stream);
 }
 
 int b200gs_sampling_rate(int32_t P, int32_t n_views, const float *means3D, const float *viewmatrix, const float *tanfovx,

@@ -517,40 +517,30 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_
 }
 #endif // FWD_BULK
 
-void launch_blend_fwd(const BlendArgs &a, cudaStream_t st)
-{
-    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    blend_fwd_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
-}
-
 #if !FWD_BULK
-int blend_fwd_has_contrib() { return 1; }
-void launch_blend_fwd_contrib(const BlendArgs &a, const ContribOut &co, cudaStream_t st)
+int blend_caps()
 {
-    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    blend_fwd_contrib_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, co);
-}
-int blend_has_normals() { return 1; }
-void launch_blend_fwd_nrm(const BlendArgs &a, const float4 *gauss_normals, float *out_normal, cudaStream_t st)
-{
-    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    blend_fwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal);
-}
-int blend_has_geometry() { return 1; }
-void launch_blend_fwd_geo(const BlendArgs &a, const float4 *gauss_normals, float *out_normal, const GeoFwd &g, cudaStream_t st)
-{
-    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    if (gauss_normals) blend_fwd_nrm_geo_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal, g);
-    else blend_fwd_geo_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, g);
+    return BLEND_CAP_CONTRIB | BLEND_CAP_NORMALS | BLEND_CAP_GEOMETRY | BLEND_CAP_ABSGRAD | BLEND_CAP_DETERMINISTIC;
 }
 #else
-int blend_fwd_has_contrib() { return 0; } // the contribution variant exists for the default kernel only
-void launch_blend_fwd_contrib(const BlendArgs &, const ContribOut &, cudaStream_t) {}
-int blend_has_normals() { return 0; } // nor the normal maps (their backward kernels are not launched either)
-void launch_blend_fwd_nrm(const BlendArgs &, const float4 *, float *, cudaStream_t) {}
-int blend_has_geometry() { return 0; } // nor the geometry outputs
-void launch_blend_fwd_geo(const BlendArgs &, const float4 *, float *, const GeoFwd &, cudaStream_t) {}
+// the contribution, normal and geometry variants exist for the default kernel only (the normals' and geometry's backward
+// kernels are then not launched either)
+int blend_caps() { return BLEND_CAP_ABSGRAD | BLEND_CAP_DETERMINISTIC; }
 #endif
+
+void launch_blend_fwd(const BlendArgs &a, const ContribOut *co, const float4 *gauss_normals, float *out_normal, const GeoFwd *g,
+                      cudaStream_t st)
+{
+    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
+#if !FWD_BULK
+    if (co) blend_fwd_contrib_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *co);
+    else if (g && gauss_normals) blend_fwd_nrm_geo_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal, *g);
+    else if (g) blend_fwd_geo_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *g);
+    else if (gauss_normals) blend_fwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal);
+    else
+#endif
+        blend_fwd_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
+}
 
 // ------------------------------------------------------------------------------------------------
 // B1
@@ -897,19 +887,6 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
     blend_bwd_body<true, true>(a, det);
 }
 
-void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st)
-{
-    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    blend_bwd_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
-}
-
-int blend_bwd_has_deterministic() { return 1; }
-void launch_blend_bwd_det(const BlendBwdArgs &a, const DetFlush &det, cudaStream_t st)
-{
-    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    blend_bwd_det_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, det);
-}
-
 // B1 with the normal term (NRM): atomic / deterministic, without and with the absolute sums.  Each stages the normals and
 // dL/dN in two more per-warp shared arrays.
 #define BWD_NRM_SHARED                                  \
@@ -936,17 +913,6 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
     BWD_NRM_SHARED;
     blend_bwd_body<true, true, true>(a, det, nslab, npix, &nb);
 }
-void launch_blend_bwd_nrm(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd &n, cudaStream_t st)
-{
-    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    if (det) {
-        if (absgrad) blend_bwd_det_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det, n);
-        else blend_bwd_det_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det, n);
-    } else {
-        if (absgrad) blend_bwd_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, n);
-        else blend_bwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, n);
-    }
-}
 
 // B1 with the geometry gradients (GEO): atomic / deterministic x absgrad off / on x normals off / on.  Each stages the pixels'
 // (dL/dM2, dL/dmedian) and the slots' median ballots in two more per-warp shared arrays (and the NRM forms the normals' two).
@@ -963,28 +929,37 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_
         blend_bwd_body<DET, ABS, false, true>(a, det, nullptr, nullptr, nullptr, gpix, gmed, &gb);
     }
 }
-void launch_blend_bwd_geo(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd *n, const GeoBwd &g, cudaStream_t st)
-{
-    const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    const DetFlush d = det ? *det : DetFlush{};
-    const NrmBwd nb = n ? *n : NrmBwd{};
-    void (*k)(BlendBwdArgs, DetFlush, NrmBwd, GeoBwd);
-    if (det) {
-        if (n) k = absgrad ? blend_bwd_geo_kernel<true, true, true> : blend_bwd_geo_kernel<true, false, true>;
-        else k = absgrad ? blend_bwd_geo_kernel<true, true, false> : blend_bwd_geo_kernel<true, false, false>;
-    } else {
-        if (n) k = absgrad ? blend_bwd_geo_kernel<false, true, true> : blend_bwd_geo_kernel<false, false, true>;
-        else k = absgrad ? blend_bwd_geo_kernel<false, true, false> : blend_bwd_geo_kernel<false, false, false>;
-    }
-    k<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, d, nb, g);
-}
 
-int blend_bwd_has_absgrad() { return 1; }
-void launch_blend_bwd_abs(const BlendBwdArgs &a, const DetFlush *det, cudaStream_t st)
+void launch_blend_bwd(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd *n, const GeoBwd *g, cudaStream_t st)
 {
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    if (det) blend_bwd_det_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det);
-    else blend_bwd_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
+    if (g) {
+        const DetFlush d = det ? *det : DetFlush{};
+        const NrmBwd nb = n ? *n : NrmBwd{};
+        void (*k)(BlendBwdArgs, DetFlush, NrmBwd, GeoBwd);
+        if (det) {
+            if (n) k = absgrad ? blend_bwd_geo_kernel<true, true, true> : blend_bwd_geo_kernel<true, false, true>;
+            else k = absgrad ? blend_bwd_geo_kernel<true, true, false> : blend_bwd_geo_kernel<true, false, false>;
+        } else {
+            if (n) k = absgrad ? blend_bwd_geo_kernel<false, true, true> : blend_bwd_geo_kernel<false, false, true>;
+            else k = absgrad ? blend_bwd_geo_kernel<false, true, false> : blend_bwd_geo_kernel<false, false, false>;
+        }
+        k<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, d, nb, *g);
+    } else if (n) {
+        if (det) {
+            if (absgrad) blend_bwd_det_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det, *n);
+            else blend_bwd_det_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det, *n);
+        } else {
+            if (absgrad) blend_bwd_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *n);
+            else blend_bwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *n);
+        }
+    } else if (det) {
+        if (absgrad) blend_bwd_det_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det);
+        else blend_bwd_det_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det);
+    } else {
+        if (absgrad) blend_bwd_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
+        else blend_bwd_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
+    }
 }
 
 // dL_dmeans2D_abs of every (view, Gaussian): the padding sums (Ax, Ay) times o * W/2 and o * H/2, o the record's opacity --

@@ -143,17 +143,11 @@ int launch_det_plan(const DetPlanArgs &a, int64_t n_vp, int n_tiles_all, const D
 }
 
 void launch_det_reduce(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
-                       cudaStream_t st)
+                       const float4 *nrm_partials, float4 *wn, cudaStream_t st)
 {
     const unsigned grid = (unsigned)((n_vp + 255) / 256);
-    if (abs_partials) det_reduce_kernel<true><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, abs_partials);
-    else det_reduce_kernel<false><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, nullptr);
-}
-
-void launch_det_reduce_nrm(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
-                           const float4 *nrm_partials, float4 *wn, cudaStream_t st)
-{
-    const unsigned grid = (unsigned)((n_vp + 255) / 256);
-    if (abs_partials) det_reduce_kernel<true, true><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, abs_partials, nrm_partials, wn);
-    else det_reduce_kernel<false, true><<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, nullptr, nrm_partials, wn);
+    void (*k)(const DetPlanArgs, int64_t, const float *, float *, const float2 *, const float4 *, float4 *);
+    if (nrm_partials) k = abs_partials ? det_reduce_kernel<true, true> : det_reduce_kernel<false, true>;
+    else k = abs_partials ? det_reduce_kernel<true, false> : det_reduce_kernel<false, false>;
+    k<<<grid, 256, 0, st>>>(a, n_vp, partials, (float *)sgrad, abs_partials, nrm_partials, wn);
 }

@@ -104,16 +104,17 @@ int launch_test_sort32(uint32_t *ka, uint32_t *kb, uint32_t *va, uint32_t *vb, i
                        int *result_in_b, cudaStream_t st);
 size_t test_sort32_scratch_bytes(int64_t n);
 
-void launch_blend_fwd(const BlendArgs &a, cudaStream_t st);
+// the optional features of the blend a build implements (blend_caps): all in blend.cu; the bulk-copy build lacks the
+// forward's CONTRIB, NORMALS and GEOMETRY; the classic comparator has none.  The host checks them before any launch.
+enum { BLEND_CAP_CONTRIB = 1, BLEND_CAP_NORMALS = 2, BLEND_CAP_GEOMETRY = 4, BLEND_CAP_ABSGRAD = 8,
+       BLEND_CAP_DETERMINISTIC = 16 };
+int blend_caps();
 // contribution scores (DESIGN.md section 2): per Gaussian [P], in/out, folded over every pixel of every view of the launch
 struct ContribOut {
     uint64_t *weight_sum; // sum of q(w) = rn(w * 2^24) over the blends
     uint32_t *weight_max; // max of the bits of w over the blends
     uint32_t *touches;    // blends plus terminating hits
 };
-int blend_fwd_has_contrib(); // 0 in the classic comparator and the bulk-copy build
-void launch_blend_fwd_contrib(const BlendArgs &a, const ContribOut &co, cudaStream_t st);
-void launch_blend_bwd(const BlendBwdArgs &a, cudaStream_t st);
 int blend_sgrad_is_moments(); // which ScreenGrad format the linked blend_bwd writes
 
 // ---- deterministic backward (deterministic.cu; B1's deterministic instantiation in blend.cu) ------------------------------
@@ -147,18 +148,15 @@ struct DetPlanArgs {
 // bits, *total the exact sum; temp (popc_scan_temp_bytes) is zeroed by the call
 size_t popc_scan_temp_bytes(int64_t n);
 int launch_popc_scan(const uint8_t *pm, uint32_t *incl, int64_t n, char *temp, uint64_t *total, cudaStream_t st);
-int blend_bwd_has_deterministic(); // 0 in the classic comparator
-void launch_blend_bwd_det(const BlendBwdArgs &a, const DetFlush &det, cudaStream_t st);
 // start scatter, plan, scan of popc(pm) -> base and the exact 64-bit partial count at *total_dev
 int launch_det_plan(const DetPlanArgs &a, int64_t n_vp, int n_tiles_all, const DetLayout &L, char *det_base, cudaStream_t st,
                     int *n_launches);
-// abs_partials (NULL: none): their (Ax, Ay) are added in the same order into ScreenGrad's padding, which is zero without them
+// abs_partials (NULL: none): their (Ax, Ay) are added in the same order into ScreenGrad's padding, which is zero without them.
+// nrm_partials (NULL: none): their normal sums are added in the same order and written to wn[vp]
 void launch_det_reduce(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
-                       cudaStream_t st);
-// absolute screen-space gradients (DESIGN.md section 2): B1 with Ax, Ay in ScreenGrad's padding -- atomic (det NULL) or
-// deterministic -- and the pass that writes dL_dmeans2D_abs [V,P,3] from them.  0 in the classic comparator.
-int blend_bwd_has_absgrad();
-void launch_blend_bwd_abs(const BlendBwdArgs &a, const DetFlush *det, cudaStream_t st);
+                       const float4 *nrm_partials, float4 *wn, cudaStream_t st);
+// absolute screen-space gradients (DESIGN.md section 2): B1 writes Ax, Ay into ScreenGrad's padding, and this pass writes
+// dL_dmeans2D_abs [V,P,3] from them
 void launch_absgrad_out(int64_t n_vp, int H, int W, const int32_t *radii, const GeomRec *recs, const void *sgrad, float *out,
                         cudaStream_t st);
 void launch_test_exp(const float *x, float *y, int64_t n, cudaStream_t st);
@@ -174,37 +172,31 @@ void launch_normal_prep(const NormalArgs &a, float4 *gauss_normals, cudaStream_t
 // dL_drots[i] += dL/dq of sum over the views with radii > 0 of sign * wn[v*P + i]
 void launch_normal_bwd(const NormalArgs &a, const int32_t *radii, const float4 *gauss_normals, const float4 *wn, float *dL_drots,
                        cudaStream_t st);
-int blend_has_normals(); // 0 in the classic comparator and the bulk-copy build
-// F6 with the normal image out_normal [V,3,H,W] = sum w * n
-void launch_blend_fwd_nrm(const BlendArgs &a, const float4 *gauss_normals, float *out_normal, cudaStream_t st);
 struct NrmBwd {
     const float4 *gauss_normals; // [V*P]
     const float *dL_dnormal;     // [V,3,H,W]
     float4 *wn;                  // [V*P] atomic mode: sum w * dL/dN of every (view, Gaussian), zeroed by the caller
     float4 *partials;            // [H] deterministic mode: each partial's three sums, at its slot
 };
-// B1 with the normal term: atomic (det NULL) or deterministic, with or without the absolute sums
-void launch_blend_bwd_nrm(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd &n, cudaStream_t st);
-// the deterministic reduce with the normal partials: also writes wn[vp] = their sums in the same fixed order
 // ---- geometry outputs (DESIGN.md section 2; the GEO instantiations of the blend kernels) ---------------------------------
-int blend_has_geometry(); // 0 in the classic comparator and the bulk-copy build
 struct GeoFwd {
     float *out_median;    // [V,1,H,W] depth of the last blend with T > 0.5 before it (0: none)
     float *out_depth2;    // [V,1,H,W] M2 = sum w d^2
     uint32_t *median_pos; // [V,H,W] 1-based list position of that blend (0: none); read by the backward
 };
-// F6 with the geometry outputs; gauss_normals non-NULL: also the normal image out_normal (the nrm+geo kernel)
-void launch_blend_fwd_geo(const BlendArgs &a, const float4 *gauss_normals, float *out_normal, const GeoFwd &g, cudaStream_t st);
 struct GeoBwd {
     const float *dL_dmedian;      // [V,1,H,W] or NULL (zero)
     const float *dL_ddepth2;      // [V,1,H,W] or NULL (zero)
     const uint32_t *median_pos;   // [V,H,W] the forward's
 };
-// B1 with the geometry gradients folded into W3: atomic (det NULL) or deterministic, with or without the absolute sums, with
-// (n non-NULL) or without the normal term.  The deterministic reduce is the one the same call without geometry runs.
-void launch_blend_bwd_geo(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd *n, const GeoBwd &g, cudaStream_t st);
-void launch_det_reduce_nrm(const DetPlanArgs &a, int64_t n_vp, const float *partials, const float2 *abs_partials, void *sgrad,
-                           const float4 *nrm_partials, float4 *wn, cudaStream_t st);
+
+// F6.  Each feature is off when NULL: co the contribution scores (never with the other two); gauss_normals the normal image
+// out_normal [V,3,H,W] = sum w * n; g the geometry outputs.  A build without a feature (blend_caps) ignores its argument.
+void launch_blend_fwd(const BlendArgs &a, const ContribOut *co, const float4 *gauss_normals, float *out_normal, const GeoFwd *g,
+                      cudaStream_t st);
+// B1: atomic (det NULL) or deterministic, with or without the absolute sums (Ax, Ay in ScreenGrad's padding), the normal term
+// (n) and the geometry gradients folded into W3 (g); NULL = off.  The deterministic reduce does not depend on geometry.
+void launch_blend_bwd(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd *n, const GeoBwd *g, cudaStream_t st);
 
 // animation frame path (anim.cu)
 void launch_reattach(int P, int n_frames, int n_verts, int n_faces, const float *vertices, const int32_t *faces, const int32_t *map_face,

@@ -28,7 +28,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200GS_LIB selects another build of the SAME C-ABI (only used to time baseline/libb200gs_classic.so, the
 # classic-structure comparator, through the identical host path).  It is not a fallback: the default is the product.
 LIB_PATH = os.environ.get("B200GS_LIB") or os.path.join(_HERE, "libb200gs.so")
-ABI_VERSION = 4
+ABI_VERSION = 5
 MAX_VIEWS = 64
 MAX_INSTANCES = 0x7FFFFFFF  # (Gaussian, tile) instances per call (B200GS_MAX_INSTANCES); larger batches are split by views
 
@@ -54,12 +54,34 @@ class _Params(C.Structure):
 
 
 class _RenderOpts(C.Structure):
-    """b200gs_render_opts (include/b200gs.h): options of the *_opts entry points"""
-    _fields_ = [("struct_bytes", C.c_int32), ("antialiasing", C.c_int32), ("filter3d_var", C.c_void_p)]
+    """b200gs_render_opts (include/b200gs.h): options of the *_opts entry points; a NULL buffer turns its feature off"""
+    _fields_ = ([("struct_bytes", C.c_int32), ("antialiasing", C.c_int32), ("filter3d_var", C.c_void_p)] +
+                [(n, C.c_void_p) for n in ("gauss_normals", "out_normal", "dL_dnormal", "normal_wn", "nrm_partials")] +
+                [("nrm_partials_bytes", C.c_size_t)] +
+                [(n, C.c_void_p) for n in ("median_pos", "out_median", "out_depth2", "dL_dmedian", "dL_ddepth2", "weight_sum",
+                                           "weight_max", "touches", "dL_dmeans2D_abs", "abs_partials")] +
+                [("abs_partials_bytes", C.c_size_t)])
 
 
-def _render_opts(antialiasing: bool, filter_3d: Optional[torch.Tensor] = None):
-    return _RenderOpts(C.sizeof(_RenderOpts), int(bool(antialiasing)), None if filter_3d is None else filter_3d.data_ptr())
+def _render_opts(antialiasing: bool, filter_3d: Optional[torch.Tensor] = None, **buffers):
+    """b200gs_render_opts: the two filters, and feature buffers by field name (tensors, None = absent).  A *_partials
+    buffer (uint8) also sets its *_bytes field."""
+    o = _RenderOpts(C.sizeof(_RenderOpts), int(bool(antialiasing)), None if filter_3d is None else filter_3d.data_ptr())
+    for name, t in buffers.items():
+        if t is not None:
+            setattr(o, name, _ptr(t))
+            if name.endswith("_partials"):
+                setattr(o, name + "_bytes", t.numel())
+    return o
+
+
+def _opts_or_plain(plain, with_opts, antialiasing, filter_3d, **buffers):
+    """The entry point to call and its options: the plain one when every option is off (b200gs_forward and friends equal
+    their *_opts form with NULL options), else the *_opts form with `opts` bound after `prm`."""
+    if not antialiasing and filter_3d is None and all(t is None for t in buffers.values()):
+        return plain
+    opts = _render_opts(antialiasing, filter_3d, **buffers)
+    return lambda prm, *a: with_opts(prm, C.byref(opts), *a)
 
 
 def _check_filter_3d(filter_3d, P, device, cov3D_precomp=None):
@@ -77,28 +99,6 @@ def _check_filter_3d(filter_3d, P, device, cov3D_precomp=None):
     return filter_3d.detach().contiguous()
 
 
-class _NormalsIO(C.Structure):
-    """b200gs_normals_io (include/b200gs.h): the normal map's buffers"""
-    _fields_ = [("struct_bytes", C.c_int32), ("gauss_normals", C.c_void_p), ("out_normal", C.c_void_p), ("dL_dnormal", C.c_void_p),
-                ("normal_wn", C.c_void_p), ("nrm_partials", C.c_void_p), ("nrm_partials_bytes", C.c_size_t)]
-
-
-def _normals_io(gauss_normals, out_normal=None, dL_dnormal=None, normal_wn=None, nrm_partials=None):
-    return _NormalsIO(C.sizeof(_NormalsIO), _ptr(gauss_normals), _ptr(out_normal), _ptr(dL_dnormal), _ptr(normal_wn),
-                      _ptr(nrm_partials), 0 if nrm_partials is None else nrm_partials.numel())
-
-
-class _GeometryIO(C.Structure):
-    """b200gs_geometry_io (include/b200gs.h): the median depth and depth second moment's buffers"""
-    _fields_ = [("struct_bytes", C.c_int32), ("out_median", C.c_void_p), ("out_depth2", C.c_void_p), ("median_pos", C.c_void_p),
-                ("dL_dmedian", C.c_void_p), ("dL_ddepth2", C.c_void_p)]
-
-
-def _geometry_io(median_pos, out_median=None, out_depth2=None, dL_dmedian=None, dL_ddepth2=None):
-    return _GeometryIO(C.sizeof(_GeometryIO), _ptr(out_median), _ptr(out_depth2), _ptr(median_pos), _ptr(dL_dmedian),
-                       _ptr(dL_ddepth2))
-
-
 class _StateView(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("geom_records", "tiles_touched", "offsets", "clamped", "sorted_tile_keys",
                                           "depth_order", "point_list", "ranges", "final_T", "n_contrib",
@@ -113,12 +113,8 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_knn_scratch_bytes", "b200gs_dist2_knn3", "b200gs_densify_stats", "b200gs_densify_scratch_bytes",
            "b200gs_densify_plan", "b200gs_densify_move", "b200gs_adam_packed", "b200gs_deterministic_bytes",
            "b200gs_backward_deterministic", "b200gs_forward_opts", "b200gs_backward_opts",
-           "b200gs_backward_deterministic_opts", "b200gs_sampling_rate", "b200gs_backward_absgrad_opts",
-           "b200gs_backward_deterministic_absgrad_opts", "b200gs_forward_contrib_opts", "b200gs_prune_plan",
-           "b200gs_forward_normals_opts", "b200gs_backward_normals_opts", "b200gs_backward_deterministic_normals_opts",
-           "b200gs_backward_absgrad_normals_opts", "b200gs_backward_deterministic_absgrad_normals_opts", "b200gs_mcmc_noise",
-           "b200gs_mcmc_ratio", "b200gs_mcmc_move", "b200gs_forward_geometry_opts", "b200gs_backward_geometry_opts",
-           "b200gs_backward_deterministic_geometry_opts"]
+           "b200gs_backward_deterministic_opts", "b200gs_sampling_rate", "b200gs_prune_plan", "b200gs_mcmc_noise",
+           "b200gs_mcmc_ratio", "b200gs_mcmc_move"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -155,31 +151,6 @@ def load_library():
     L.b200gs_backward_deterministic_opts.restype = C.c_int
     L.b200gs_backward_deterministic_opts.argtypes = ([L.b200gs_backward_deterministic.argtypes[0], vp] +
                                                      L.b200gs_backward_deterministic.argtypes[1:])
-    # the absgrad forms: the *_opts argument lists with dL_dmeans2D_abs after dL_dcov3D (and abs_partials after n_partials)
-    bo = L.b200gs_backward_opts.argtypes
-    L.b200gs_backward_absgrad_opts.restype = C.c_int
-    L.b200gs_backward_absgrad_opts.argtypes = bo[:30] + [vp] + bo[30:]
-    bdo = L.b200gs_backward_deterministic_opts.argtypes
-    L.b200gs_backward_deterministic_absgrad_opts.restype = C.c_int
-    L.b200gs_backward_deterministic_absgrad_opts.argtypes = bdo[:30] + [vp] + bdo[30:36] + [vp, sz] + bdo[36:]
-    # the contribution form: b200gs_forward_opts' argument list with the three accumulators after num_rendered
-    fo = L.b200gs_forward_opts.argtypes
-    L.b200gs_forward_contrib_opts.restype = C.c_int
-    L.b200gs_forward_contrib_opts.argtypes = fo[:-1] + [vp, vp, vp] + fo[-1:]
-    # the normals forms: the *_opts argument lists with the b200gs_normals_io pointer after opts
-    for name, base in (("forward", fo), ("backward", bo), ("backward_deterministic", bdo),
-                       ("backward_absgrad", L.b200gs_backward_absgrad_opts.argtypes),
-                       ("backward_deterministic_absgrad", L.b200gs_backward_deterministic_absgrad_opts.argtypes)):
-        fn = getattr(L, f"b200gs_{name}_normals_opts")
-        fn.restype = C.c_int
-        fn.argtypes = base[:2] + [C.POINTER(_NormalsIO)] + base[2:]
-    # the geometry forms: the nullable normals io and the geometry io after opts; the backward forms take the absgrad forms'
-    # argument lists (dL_dmeans2D_abs and abs_partials nullable)
-    for name, base in (("forward", fo), ("backward", L.b200gs_backward_absgrad_opts.argtypes),
-                       ("backward_deterministic", L.b200gs_backward_deterministic_absgrad_opts.argtypes)):
-        fn = getattr(L, f"b200gs_{name}_geometry_opts")
-        fn.restype = C.c_int
-        fn.argtypes = base[:2] + [C.POINTER(_NormalsIO), C.POINTER(_GeometryIO)] + base[2:]
     L.b200gs_sampling_rate.restype = C.c_int
     L.b200gs_sampling_rate.argtypes = [i32, i32, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float), i32, i32, vp, vp]
     L.b200gs_mark_visible.restype = C.c_int
@@ -371,7 +342,7 @@ def release_cached_buffers():
 class _Ctx:
     """What one forward keeps for its backward (upstream keeps geomBuffer/binningBuffer/imgBuffer the same way)."""
     __slots__ = ("prm", "tanx", "tany", "geom", "binning", "image", "scratch", "capacity", "num_rendered", "radii", "V", "P", "H",
-                 "W", "M", "opts", "f3d", "gauss_normals", "normal", "normal_wn", "median", "depth2", "median_pos", "__weakref__")
+                 "W", "M", "aa", "f3d", "gauss_normals", "normal", "normal_wn", "median", "depth2", "median_pos", "__weakref__")
 
 
 def _make_params(P, V, deg, M, H, W, mod, tanx, tany, prefiltered=False, debug=False, per_view_means=False, raw=False):
@@ -390,11 +361,12 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     antialiasing: the screen-space mip filter; filter_3d: the 3D smoothing filter's [P] variances (b200gs_render_opts).
     The state remembers both for the backward.
     contrib: None, or the contribution accumulators (weight_sum, weight_max, touches), [P] int64 / int32 / int32 device tensors
-    read as u64 / u32 / u32: b200gs_forward_contrib_opts then runs and folds this call's views into them.
-    normals=True: b200gs_forward_normals_opts runs; the state holds the normal image `normal` [V,3,H,W] and the per-(view,
-    Gaussian) normals `gauss_normals` [V,P,4] its backward reads.
-    geometry=True: b200gs_forward_geometry_opts runs (with the normals io when normals=True); the state holds the images
-    `median` and `depth2` [V,1,H,W] and the median positions `median_pos` [V,H,W] int32 its backward reads."""
+    read as u64 / u32 / u32: the forward then folds this call's views into them.
+    normals=True: the state holds the normal image `normal` [V,3,H,W] and the per-(view, Gaussian) normals `gauss_normals`
+    [V,P,4] its backward reads.
+    geometry=True: the state holds the images `median` and `depth2` [V,1,H,W] and the median positions `median_pos` [V,H,W]
+    int32 its backward reads.
+    Every option travels in b200gs_render_opts; with all of them off the plain b200gs_forward runs."""
     L = load_library()
     dev = means3D.device
     if dev.type != "cuda":
@@ -427,26 +399,18 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     cap = _cap_hint.get(key, max(1 << 16, 4 * P * V))
     n_out = C.c_int64(0)
     stream = torch.cuda.current_stream(dev).cuda_stream
-    opts = _render_opts(antialiasing, filter_3d) if (antialiasing or filter_3d is not None) else None
-    # with the defaults the plain entry point runs (b200gs_forward == b200gs_forward_opts with NULL options)
-    fwd = (lambda *a: L.b200gs_forward_opts(a[0], C.byref(opts), *a[1:])) if opts is not None else L.b200gs_forward
-    gauss_normals = normal = None
+    gauss_normals = normal = median = depth2 = median_pos = None
     if normals:
         gauss_normals = torch.empty(V, P, 4, dtype=torch.float32, device=dev)
         normal = torch.empty(V, 3, H, W, dtype=torch.float32, device=dev)
-        nio = _normals_io(gauss_normals, normal)
-        fwd = lambda *a: L.b200gs_forward_normals_opts(a[0], None if opts is None else C.byref(opts), C.byref(nio), *a[1:])
-    median = depth2 = median_pos = None
     if geometry:
         median = torch.empty(V, 1, H, W, dtype=torch.float32, device=dev)
         depth2 = torch.empty(V, 1, H, W, dtype=torch.float32, device=dev)
         median_pos = torch.empty(V, H, W, dtype=torch.int32, device=dev)
-        gio = _geometry_io(median_pos, median, depth2)
-        nio_p = C.byref(nio) if normals else None
-        fwd = lambda *a: L.b200gs_forward_geometry_opts(a[0], None if opts is None else C.byref(opts), nio_p, C.byref(gio), *a[1:])
-    if contrib is not None:
-        fwd = lambda *a: L.b200gs_forward_contrib_opts(a[0], None if opts is None else C.byref(opts), *a[1:-1],
-                                                       *[_ptr(t) for t in contrib], a[-1])
+    weight_sum, weight_max, touches = contrib if contrib is not None else (None, None, None)
+    fwd = _opts_or_plain(L.b200gs_forward, L.b200gs_forward_opts, antialiasing, filter_3d, gauss_normals=gauss_normals,
+                         out_normal=normal, median_pos=median_pos, out_median=median, out_depth2=depth2, weight_sum=weight_sum,
+                         weight_max=weight_max, touches=touches)
     with torch.cuda.device(dev):
         for _ in range(3):
             pkey = (key, stream, cap)
@@ -480,19 +444,19 @@ def _forward_impl(means3D, shs, colors_precomp, opacities, scales, rotations, co
     st.geom, st.binning, st.image, st.scratch, st.capacity, st.num_rendered = geom, binning, image, bufs["scratch"], call_cap, \
         int(n_out.value)
     st.radii, st.V, st.P, st.H, st.W, st.M = radii, V, P, H, W, M
-    st.opts, st.f3d = opts, filter_3d  # the backward reads the same variances (st keeps them alive)
+    st.aa, st.f3d = antialiasing, filter_3d  # the backward gets the same options (st keeps the variances alive)
     st.gauss_normals, st.normal, st.normal_wn = gauss_normals, normal, None
     st.median, st.depth2, st.median_pos = median, depth2, median_pos
     weakref.finalize(st, _pool.give, pkey, bufs)  # when the autograd graph drops the state, the buffers are parked for re-use
     return color, radii, depth, alpha, st
 
 
-def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_abs=None, nio=None, gio=None):
+def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, **buffers):
     """b200gs_backward_deterministic with the work buffer from _det_pool, sized by the partial-capacity hint; a call whose
-    partials do not fit is repeated with room for the count it reported (at most two retries).  d_means2D_abs: the absgrad
-    form, with its float2-per-partial array pooled beside the work buffer.  nio: the normals form (_NormalsIO with dL_dnormal),
-    with its float4-per-partial array pooled the same way.  gio: the geometry form (_GeometryIO with a geometry gradient),
-    which needs no buffer of its own."""
+    partials do not fit is repeated with room for the count it reported (at most two retries).  buffers: the backward's
+    option buffers (_backward_impl).  With dL_dmeans2D_abs the float2-per-partial array abs_partials, with dL_dnormal the
+    float4-per-partial array nrm_partials, are pooled beside the work buffer; geometry needs no buffer of its own."""
+    absgrad, nrm = buffers.get("dL_dmeans2D_abs") is not None, buffers.get("dL_dnormal") is not None
     P, V, H, W = st.P, st.V, st.H, st.W
     key = (dev.index, P, V, H, W)
     pcap = _partial_hint.get(key, max(1 << 16, 2 * st.num_rendered))
@@ -500,43 +464,18 @@ def _backward_deterministic(L, st: _Ctx, dev, args, det_state=None, d_means2D_ab
     stream = torch.cuda.current_stream(dev).cuda_stream
     for _ in range(3):
         # sized for the forward's instance capacity (>= its count), so the pool key stays the same from call to call
-        pkey = (dev.index, stream, st.capacity, pcap, P, V, d_means2D_abs is not None, nio is not None)
+        pkey = (dev.index, stream, st.capacity, pcap, P, V, absgrad, nrm)
         bufs = _det_pool.take(pkey)
         if bufs is None:
             bufs = dict(det=torch.empty(L.b200gs_deterministic_bytes(st.capacity, pcap, P, V), dtype=torch.uint8, device=dev))
-            if d_means2D_abs is not None:
+            if absgrad:
                 bufs["abs"] = torch.empty(max(8 * pcap, 16), dtype=torch.uint8, device=dev)
-            if nio is not None:
+            if nrm:
                 bufs["nrm"] = torch.empty(max(16 * pcap, 16), dtype=torch.uint8, device=dev)
         det = bufs["det"]
-        opts_p = C.byref(st.opts) if st.opts is not None else None
-        if nio is not None:
-            nio.nrm_partials, nio.nrm_partials_bytes = _ptr(bufs["nrm"]), bufs["nrm"].numel()
-        if gio is not None:
-            ab = bufs.get("abs")
-            rc = L.b200gs_backward_deterministic_geometry_opts(
-                args[0], opts_p, None if nio is None else C.byref(nio), C.byref(gio), *args[1:29], _ptr(d_means2D_abs), *args[29:],
-                _ptr(det), det.numel(), pcap, C.byref(n_out), _ptr(ab), 0 if ab is None else ab.numel(), C.c_void_p(stream))
-        elif nio is not None:
-            if d_means2D_abs is not None:
-                ab = bufs["abs"]
-                rc = L.b200gs_backward_deterministic_absgrad_normals_opts(
-                    args[0], opts_p, C.byref(nio), *args[1:29], _ptr(d_means2D_abs), *args[29:], _ptr(det), det.numel(), pcap,
-                    C.byref(n_out), _ptr(ab), ab.numel(), C.c_void_p(stream))
-            else:
-                rc = L.b200gs_backward_deterministic_normals_opts(args[0], opts_p, C.byref(nio), *args[1:], _ptr(det), det.numel(),
-                                                                  pcap, C.byref(n_out), C.c_void_p(stream))
-        elif d_means2D_abs is not None:
-            ab = bufs["abs"]
-            opts = C.byref(st.opts) if st.opts is not None else None
-            rc = L.b200gs_backward_deterministic_absgrad_opts(args[0], opts, *args[1:29], _ptr(d_means2D_abs), *args[29:], _ptr(det),
-                                                              det.numel(), pcap, C.byref(n_out), _ptr(ab), ab.numel(),
-                                                              C.c_void_p(stream))
-        elif st.opts is not None:
-            rc = L.b200gs_backward_deterministic_opts(args[0], C.byref(st.opts), *args[1:], _ptr(det), det.numel(), pcap,
-                                                      C.byref(n_out), C.c_void_p(stream))
-        else:
-            rc = L.b200gs_backward_deterministic(*args, _ptr(det), det.numel(), pcap, C.byref(n_out), C.c_void_p(stream))
+        bwd = _opts_or_plain(L.b200gs_backward_deterministic, L.b200gs_backward_deterministic_opts, st.aa, st.f3d, **buffers,
+                             abs_partials=bufs.get("abs"), nrm_partials=bufs.get("nrm"))
+        rc = bwd(*args, _ptr(det), det.numel(), pcap, C.byref(n_out), C.c_void_p(stream))
         if rc == OK and det_state is not None:
             det_state["patch_masks"] = det[:st.num_rendered].clone()
             det_state["n_partials"] = int(n_out.value)
@@ -557,16 +496,18 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
     """`out` (optional): dict of preallocated contiguous fp32 gradient buffers by name (means3D, sh, opacity, scales,
     rotations) -- the packed entry points them into one flat buffer so that B3 writes the all-reduce payload in place.
 
-    absgrad=True: the absgrad entry points run, and a ninth value is returned: dL_dmeans2D_abs [V,P,3], the per-pixel terms
-    of dL_dmeans2D summed in absolute value (include/b200gs.h).  Every other gradient is what absgrad=False gives.
+    absgrad=True: a ninth value is returned: dL_dmeans2D_abs [V,P,3], the per-pixel terms of dL_dmeans2D summed in absolute
+    value (include/b200gs.h).  Every other gradient is what absgrad=False gives.
 
-    g_normal [V,3,H,W] (a forward with normals=True): the normals entry points run, dL/dN reaches the opacities, means and
-    colours through the blend weights and the rotations through the normals; st.normal_wn then holds the [V,P,4] sums Wn.
-    None: the call without normals.
+    g_normal [V,3,H,W] (a forward with normals=True): dL/dN reaches the opacities, means and colours through the blend
+    weights and the rotations through the normals; st.normal_wn then holds the [V,P,4] sums Wn.  None: the call without
+    normals.
 
-    g_median, g_depth2 [V,1,H,W] (a forward with geometry=True; None = zero): the geometry entry points run.  dL/dM2 reaches
-    the opacities, means and colours through the blend weights and the means through the depth; dL/dmedian reaches the means
-    of each pixel's median Gaussian through its depth.  With both None the call is the one without geometry.
+    g_median, g_depth2 [V,1,H,W] (a forward with geometry=True; None = zero): dL/dM2 reaches the opacities, means and colours
+    through the blend weights and the means through the depth; dL/dmedian reaches the means of each pixel's median Gaussian
+    through its depth.  With both None the call is the one without geometry.
+
+    Every option travels in b200gs_render_opts; with all of them off the plain b200gs_backward[_deterministic] runs.
 
     Under torch.use_deterministic_algorithms(True) the backward is the library's deterministic one: the same gradients up
     to float rounding, bit-identical from run to run (one host wait per call, for its partial count).  `det_state`
@@ -595,34 +536,18 @@ def _backward_impl(st: _Ctx, means3D, shs, colors_precomp, opacities, scales, ro
             _ptr(st.binning), st.capacity, _ptr(st.image), st.num_rendered, _ptr(g_color), _ptr(g_depth), _ptr(g_alpha),
             _ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh), _ptr(d_col), _ptr(d_op), _ptr(d_sc), _ptr(d_rot), _ptr(d_cov),
             _ptr(scratch), scratch.numel())
-    nio = None
+    # the option buffers: the forward's filters and workspaces (from st) with the gradients that turn a feature on
+    buffers = dict(dL_dmeans2D_abs=d_abs)
     if g_normal is not None and st.gauss_normals is not None:
         st.normal_wn = torch.empty(V, P, 4, **f)
-        nio = _normals_io(st.gauss_normals, None, g_normal, st.normal_wn)
-    gio = None
+        buffers.update(gauss_normals=st.gauss_normals, dL_dnormal=g_normal, normal_wn=st.normal_wn)
     if (g_median is not None or g_depth2 is not None) and st.median_pos is not None:
-        gio = _geometry_io(st.median_pos, None, None, g_median, g_depth2)
+        buffers.update(median_pos=st.median_pos, dL_dmedian=g_median, dL_ddepth2=g_depth2)
     with torch.cuda.device(dev):
         if torch.are_deterministic_algorithms_enabled():
-            rc = _backward_deterministic(L, st, dev, args, det_state, d_abs, nio, gio)
-        elif gio is not None:
-            rc = L.b200gs_backward_geometry_opts(args[0], C.byref(st.opts) if st.opts is not None else None,
-                                                 None if nio is None else C.byref(nio), C.byref(gio), *args[1:29], _ptr(d_abs),
-                                                 *args[29:], _stream(dev))
-        elif nio is not None:
-            opts_p = C.byref(st.opts) if st.opts is not None else None
-            if absgrad:
-                rc = L.b200gs_backward_absgrad_normals_opts(args[0], opts_p, C.byref(nio), *args[1:29], _ptr(d_abs), *args[29:],
-                                                            _stream(dev))
-            else:
-                rc = L.b200gs_backward_normals_opts(args[0], opts_p, C.byref(nio), *args[1:], _stream(dev))
-        elif absgrad:
-            rc = L.b200gs_backward_absgrad_opts(args[0], C.byref(st.opts) if st.opts is not None else None, *args[1:29], _ptr(d_abs),
-                                                *args[29:], _stream(dev))
-        elif st.opts is not None:  # the backward gets the options its forward got
-            rc = L.b200gs_backward_opts(args[0], C.byref(st.opts), *args[1:], _stream(dev))
+            rc = _backward_deterministic(L, st, dev, args, det_state, **buffers)
         else:
-            rc = L.b200gs_backward(*args, _stream(dev))
+            rc = _opts_or_plain(L.b200gs_backward, L.b200gs_backward_opts, st.aa, st.f3d, **buffers)(*args, _stream(dev))
     _check(rc, "backward")
     return grads
 

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define B200GS_ABI_VERSION 4
+#define B200GS_ABI_VERSION 5
 #define B200GS_MAX_VIEWS 64 /* per call; callers chunk larger batches */
 
 typedef enum b200gs_status {
@@ -159,11 +159,13 @@ int b200gs_backward_deterministic(const b200gs_params *prm,
                                   void *scratch, size_t scratch_bytes,
                                   void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *stream);
 
-/* ---- render options (additive to ABI 4) -----------------------------------------------------------------------------
+/* ---- render options ---------------------------------------------------------------------------------------------------
  * The *_opts entry points take the argument list of their plain counterpart with `opts` after `prm`.  opts == NULL means the
- * defaults, which is exactly what b200gs_forward / b200gs_backward / b200gs_backward_deterministic do.  struct_bytes =
- * sizeof(b200gs_render_opts) of the caller's header; a value too small to hold the fields the library reads returns
- * B200GS_E_ARGS.  A backward call MUST get the same options as the forward call whose state buffers it reads.
+ * defaults, which is exactly what b200gs_forward / b200gs_backward / b200gs_backward_deterministic do.  A backward call MUST
+ * get the same options as the forward call whose state buffers it reads.
+ *   struct_bytes: sizeof(b200gs_render_opts) of the caller's header.  8 (a header before filter3d_var) reads antialiasing
+ *     only; 16 (a header that ends with filter3d_var) reads both; >= sizeof(b200gs_render_opts) reads every field; any other
+ *     value is B200GS_E_ARGS.
  *   antialiasing: 0 = off.  Non-zero = the screen-space mip filter: the covariance keeps its +0.3 px^2 dilation and the
  *     opacity is multiplied by rho = sqrt(det(S) / det(S + 0.3 I)), S the projected 2D covariance, floored at rho = 0.005,
  *     so that a Gaussian's integrated footprint does not depend on the pixel scale it is drawn at.  The backward then needs
@@ -173,12 +175,119 @@ int b200gs_backward_deterministic(const b200gs_params *prm,
  *     s'_i = sqrt(s_i^2 + v) and the opacity o * sqrt(prod_i s_i^2 / (s_i^2 + v)), so that its integrated 3D weight is kept;
  *     the backward's dL_dscales / dL_dopacity are w.r.t. the unfiltered parameters, and v gets no gradient.  With
  *     cov3D_precomp it is B200GS_E_ARGS; the backward needs opacities.  Only shape is checked, not the values (no sync).
- *   struct_bytes: 8 (a header before filter3d_var) reads antialiasing only; >= 16 reads both; any other value is
- *     B200GS_E_ARGS. */
+ * The other fields are NULL when their feature is off; each feature below says which fields turn it on.  A build of the
+ * library without a feature returns B200GS_E_UNSUPPORTED for a call that turns it on, before any other argument check: the
+ * classic comparator has none of the four, nor the deterministic backward; the bulk-copy build has no normals, geometry or
+ * contribution scores.  Contribution scores together with normals or geometry are B200GS_E_ARGS.
+ *
+ * Normal maps: each Gaussian's shortest-axis normal blended like its colour.  On in a forward iff gauss_normals is set; on
+ * in a backward iff gauss_normals and dL_dnormal are both set (dL_dnormal without gauss_normals is B200GS_E_ARGS).
+ * For view v and Gaussian g (DESIGN.md section 2):
+ *   axis    k = argmin of the activated scales s (after exp for raw parameters; before scale_modifier and the 3D filter,
+ *           which leave the argmin unchanged in exact arithmetic); on a tie the lowest index wins.
+ *   normal  n = column k of R(q), q the rotation as the covariance uses it (after the in-kernel normalise for raw), formed
+ *           with the covariance's own float operations; not renormalised.
+ *   flip    d = n . (campos_v - mean_{v,g}) as fmul, fma, fma over components 0, 1, 2 of fsub(campos, mean); if d < 0, n
+ *           becomes -n (it faces the camera).  mean is the per-view position with means3D_per_view.  A NaN d keeps the sign.
+ *   image   out_normal[v,c,p] = sum over the blends of pixel p of w n_c, accumulated as N_c = fma(n_c, w, N_c) with the
+ *           colour's w = alpha * T and order.  No background term: [V,3,H,W], world space, unnormalised, 0 where nothing
+ *           blends.
+ *   grads   dL/dN enters dL/dalpha as cg += n . dL/dN.  Wn = sum w dL/dN per (view, Gaussian) is dL/dn; times the flip sign,
+ *           through d(column k of R)/dq (and the normalise Jacobian for raw), it is ADDED to dL_drots.  Scales, means and
+ *           campos get no gradient through n (the argmin and the flip are piecewise constant), only the alpha-path terms.
+ * Colour, depth, alpha, radii and the state buffers are byte-identical to the call without normals, and the deterministic
+ * partial count is unchanged.  cov3D_precomp has no axis: B200GS_E_ARGS.
+ *   gauss_normals  [V*P] x 16 B device workspace, 16-byte aligned (else B200GS_E_BUFFER): the forward writes (sign n, sign)
+ *                  of every (view, Gaussian); the backward reads it, so it must survive from the forward to its backward
+ *                  like the state buffers
+ *   out_normal     [V,3,H,W] (forward output; NULL in a forward is B200GS_E_ARGS)
+ *   dL_dnormal     [V,3,H,W] (backward input); NULL = zero: the backward is then exactly the call without normals
+ *   normal_wn      [V*P] x 16 B device workspace, 16-byte aligned (backward with dL_dnormal; NULL is B200GS_E_ARGS, else
+ *                  B200GS_E_BUFFER): the Wn sums
+ *   nrm_partials   deterministic backward with dL_dnormal: nrm_partials_bytes >= 16 * partial_capacity bytes, 16-byte
+ *                  aligned, one float4 per partial at its slot (det_buf's layout and size do not change; NULL is
+ *                  B200GS_E_ARGS, too small or misaligned B200GS_E_BUFFER)
+ *
+ * Geometry outputs: median depth and depth second moment of the blend.  On in a forward iff median_pos is set; on in a
+ * backward iff dL_dmedian or dL_ddepth2 is set, and median_pos is then required.
+ * For view v and pixel p, over the blends of p in the colour's order, with the colour's alpha, T (before the blend),
+ * w = alpha * T and d the Gaussian's view-space depth (DESIGN.md section 2):
+ *   depth2   out_depth2[v,0,p] = M2 = sum w d^2, accumulated as M2 = fma(d * d, w, M2).  No background term; 0 where nothing
+ *            blends.  With alpha and depth: the depth distortion sum_{i<j} w_i w_j (d_i - d_j)^2 = A * M2 - M1^2.
+ *   median   out_median[v,0,p] = d of the LAST blend whose T is > 0.5 (strict, on the float32 T): the blend at which T
+ *            crosses 1/2, or the last blend if T never reaches it.  0 where nothing blends.  median_pos[v,p] = its 1-based
+ *            position in the tile's list (0 = none).
+ *   grads    dL/dM2 enters dL/dalpha as cg += d^2 dL/dM2, and adds sum_p w 2d dL/dM2 to the Gaussian's depth gradient.
+ *            dL/dmedian adds dL/dmedian_p to the depth gradient of p's median Gaussian only (the selection is piecewise
+ *            constant: no alpha-path term).  Both reach the means through the existing depth term.
+ * Colour, depth, alpha, normals, radii and the state buffers are byte-identical to the call without geometry, and the
+ * deterministic partial count is unchanged.  Combines with SH or precomputed colours, raw parameters, cov3D_precomp,
+ * antialiasing, the 3D filter, per-view means, normals, absgrad and the deterministic backward.
+ *   median_pos     [V,H,W] x u32 device workspace, 4-byte aligned (else B200GS_E_BUFFER): the forward writes it, the
+ *                  backward reads it, so it must survive from the forward to its backward like the state buffers
+ *   out_median     [V,1,H,W] (forward output; NULL in a forward is B200GS_E_ARGS)
+ *   out_depth2     [V,1,H,W] (forward output; NULL in a forward is B200GS_E_ARGS)
+ *   dL_dmedian     [V,1,H,W] (backward input); NULL = zero
+ *   dL_ddepth2     [V,1,H,W] (backward input); NULL = zero.  With both NULL the backward is exactly the call without geometry.
+ *
+ * Contribution scores: per-Gaussian blend weights of the forward blend.  On in a forward iff any of weight_sum, weight_max and
+ * touches is set, and then all three are required (else B200GS_E_ARGS); a backward does not read them.  The forward computes
+ * every output exactly as without them (images, radii, state buffers byte-identical), plus three per-Gaussian accumulators
+ * over every pixel of every view:
+ *   For pixel p and sorted tile-list entry k of p's tile the blend evaluates power, alpha and test_T = T (1 - alpha).
+ *   touch: power <= 0 and alpha >= 1/255 while the pixel is live (its T before the entry is > 0; out-of-image pixels never
+ *     are).  A touch either blends or is the single terminating hit at which T would drop below 1e-4 (it ends the pixel
+ *     without blending).
+ *   blend: a touch that blends, with weight w = fmul(alpha, T), the float the colour sum uses.
+ *   weight_sum [P] u64 (device, in/out): += sum over blends of q(w) = round-half-even(w * 2^24) (w <= 0.99, so q < 2^24).
+ *     weight_sum * 2^-24 is the sum of weights to within 2^-25 per blend.
+ *   weight_max [P] u32 (device, in/out): max(weight_max, bits of w) over blends (w > 0: unsigned order is float order;
+ *     0 = never blended).  Read it as a float.
+ *   touches [P] u32 (device, in/out): += number of touches.
+ * Integer adds and maxima: any camera set, in calls of any size and order, folds to the same bits, and two runs write
+ * identical bytes.  PRECONDITION: the total pixel count sum(V*H*W) folded into one set of accumulators stays below 2^32
+ * (each pixel adds at most 1 to touches and less than 2^24 to weight_sum, so neither can overflow).
+ * Removing every Gaussian with touches == 0 over a camera set, survivors kept in order, leaves those cameras' colour,
+ * depth and alpha byte-identical and the survivors' radii unchanged (DESIGN.md section 2).
+ * This forward always waits for the instance count before the blend: one that returns B200GS_E_BIN_TOO_SMALL or
+ * B200GS_E_INSTANCES has not touched the accumulators.
+ *
+ * Absolute screen-space gradients for densification.  On in a backward iff dL_dmeans2D_abs is set; a forward does not read
+ * them.  Every other output is exactly what the call without them computes.
+ *   dL_dmeans2D_abs [V,P,3] (device, overwritten): per (view, Gaussian), the per-pixel terms of dL_dmeans2D summed in
+ *     absolute value per component: ( sum_p |g_p.x|, sum_p |g_p.y|, 0 ), NDC units like dL_dmeans2D, where g_p = dL_p /
+ *     dmean2D is pixel p's term of the signed gradient.  The signed sum cancels where a Gaussian's pixels pull its centre in
+ *     opposite directions; this one does not (the "absgrad" / homodirectional densification statistic).  Zero where
+ *     radii == 0.  b200gs_densify_stats accepts it in place of dL_dmeans2D.
+ *   abs_partials (deterministic backward only): a caller-owned device array of abs_partials_bytes >= 8 * partial_capacity
+ *     bytes, 8-byte aligned (else B200GS_E_BUFFER; NULL is B200GS_E_ARGS): one float2 per partial, at the partial's slot.
+ *     It is separate from det_buf, whose layout and size (b200gs_deterministic_bytes) do not change.  The absolute sums are
+ *     then bit-reproducible like every other output. */
 typedef struct b200gs_render_opts {
-    int32_t struct_bytes;   /* sizeof(b200gs_render_opts) */
-    int32_t antialiasing;   /* 0 | 1 */
+    int32_t struct_bytes;      /* sizeof(b200gs_render_opts) */
+    int32_t antialiasing;      /* 0 | 1 */
     const float *filter3d_var; /* [P] or NULL */
+    /* normal maps */
+    float *gauss_normals;
+    float *out_normal;
+    const float *dL_dnormal;
+    float *normal_wn;
+    void *nrm_partials;
+    size_t nrm_partials_bytes;
+    /* geometry outputs */
+    uint32_t *median_pos;
+    float *out_median;
+    float *out_depth2;
+    const float *dL_dmedian;
+    const float *dL_ddepth2;
+    /* contribution scores (forward) */
+    uint64_t *weight_sum;
+    uint32_t *weight_max;
+    uint32_t *touches;
+    /* absolute screen-space gradients (backward) */
+    float *dL_dmeans2D_abs;
+    void *abs_partials;
+    size_t abs_partials_bytes;
 } b200gs_render_opts;
 int b200gs_forward_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
                         const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
@@ -212,245 +321,6 @@ int b200gs_backward_deterministic_opts(const b200gs_params *prm, const b200gs_re
                                        float *dL_dscales, float *dL_drots, float *dL_dcov3D,
                                        void *scratch, size_t scratch_bytes,
                                        void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials, void *stream);
-
-/* ---- absolute screen-space gradients for densification (additive to ABI 4) ------------------------------------------
- * The absgrad forms take the argument list of b200gs_backward_opts / b200gs_backward_deterministic_opts with one more output
- * after dL_dcov3D, and compute every other output exactly as those calls do.
- *   dL_dmeans2D_abs [V,P,3] (device, overwritten; NULL is B200GS_E_ARGS): per (view, Gaussian), the per-pixel terms of
- *     dL_dmeans2D summed in absolute value per component: ( sum_p |g_p.x|, sum_p |g_p.y|, 0 ), NDC units like dL_dmeans2D,
- *     where g_p = dL_p / dmean2D is pixel p's term of the signed gradient.  The signed sum cancels where a Gaussian's pixels
- *     pull its centre in opposite directions; this one does not (the "absgrad" / homodirectional densification statistic).
- *     Zero where radii == 0.  b200gs_densify_stats accepts it in place of dL_dmeans2D.
- *   abs_partials (deterministic form only): a caller-owned device array of abs_partials_bytes >= 8 * partial_capacity bytes,
- *     8-byte aligned (else B200GS_E_BUFFER; NULL is B200GS_E_ARGS): one float2 per partial, at the partial's slot.  It is
- *     separate from det_buf, whose layout and size (b200gs_deterministic_bytes) do not change.  The absolute sums are then
- *     bit-reproducible like every other output.
- * The classic comparator build returns B200GS_E_UNSUPPORTED. */
-int b200gs_backward_absgrad_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
-                                 const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
-                                 const float *scales, const float *rotations, const float *cov3D_precomp,
-                                 const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                                 const int32_t *radii,
-                                 const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                                 const void *image_buf, int64_t num_rendered,
-                                 const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                 float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
-                                 float *dL_dscales, float *dL_drots, float *dL_dcov3D, float *dL_dmeans2D_abs,
-                                 void *scratch, size_t scratch_bytes, void *stream);
-int b200gs_backward_deterministic_absgrad_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
-                                               const float *means3D, const float *shs, const float *colors_precomp,
-                                               const float *opacities, const float *scales, const float *rotations,
-                                               const float *cov3D_precomp, const float *bg, const float *viewmatrix,
-                                               const float *projmatrix, const float *campos, const int32_t *radii,
-                                               const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                                               const void *image_buf, int64_t num_rendered,
-                                               const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                               float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                                               float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                               float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes,
-                                               void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials,
-                                               void *abs_partials, size_t abs_partials_bytes, void *stream);
-
-/* ---- contribution scores: per-Gaussian blend weights of the forward blend (additive to ABI 4) -----------------------
- * b200gs_forward_contrib_opts takes b200gs_forward_opts's argument list and computes every output exactly as that call does
- * (images, radii, state buffers byte-identical), plus three per-Gaussian accumulators over every pixel of every view:
- *   For pixel p and sorted tile-list entry k of p's tile the blend evaluates power, alpha and test_T = T (1 - alpha).
- *   touch: power <= 0 and alpha >= 1/255 while the pixel is live (its T before the entry is > 0; out-of-image pixels never
- *     are).  A touch either blends or is the single terminating hit at which T would drop below 1e-4 (it ends the pixel
- *     without blending).
- *   blend: a touch that blends, with weight w = fmul(alpha, T), the float the colour sum uses.
- *   weight_sum [P] u64 (device, in/out): += sum over blends of q(w) = round-half-even(w * 2^24) (w <= 0.99, so q < 2^24).
- *     weight_sum * 2^-24 is the sum of weights to within 2^-25 per blend.
- *   weight_max [P] u32 (device, in/out): max(weight_max, bits of w) over blends (w > 0: unsigned order is float order;
- *     0 = never blended).  Read it as a float.
- *   touches [P] u32 (device, in/out): += number of touches.
- * Integer adds and maxima: any camera set, in calls of any size and order, folds to the same bits, and two runs write
- * identical bytes.  PRECONDITION: the total pixel count sum(V*H*W) folded into one set of accumulators stays below 2^32
- * (each pixel adds at most 1 to touches and less than 2^24 to weight_sum, so neither can overflow).
- * Removing every Gaussian with touches == 0 over a camera set, survivors kept in order, leaves those cameras' colour,
- * depth and alpha byte-identical and the survivors' radii unchanged (DESIGN.md section 2).
- * This call always waits for the instance count before the blend: one that returns B200GS_E_BIN_TOO_SMALL or
- * B200GS_E_INSTANCES has not touched the accumulators.  A NULL accumulator is B200GS_E_ARGS; the classic comparator build
- * returns B200GS_E_UNSUPPORTED. */
-int b200gs_forward_contrib_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
-                                const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
-                                const float *scales, const float *rotations, const float *cov3D_precomp,
-                                const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                                float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
-                                void *geom_buf, size_t geom_bytes,
-                                void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
-                                void *image_buf, size_t image_bytes,
-                                int64_t *num_rendered, uint64_t *weight_sum, uint32_t *weight_max, uint32_t *touches,
-                                void *stream);
-
-/* ---- normal maps: each Gaussian's shortest-axis normal blended like its colour (additive to ABI 4) ---------------------
- * For view v and Gaussian g (DESIGN.md section 2):
- *   axis    k = argmin of the activated scales s (after exp for raw parameters; before scale_modifier and the 3D filter,
- *           which leave the argmin unchanged in exact arithmetic); on a tie the lowest index wins.
- *   normal  n = column k of R(q), q the rotation as the covariance uses it (after the in-kernel normalise for raw), formed
- *           with the covariance's own float operations; not renormalised.
- *   flip    d = n . (campos_v - mean_{v,g}) as fmul, fma, fma over components 0, 1, 2 of fsub(campos, mean); if d < 0, n
- *           becomes -n (it faces the camera).  mean is the per-view position with means3D_per_view.  A NaN d keeps the sign.
- *   image   out_normal[v,c,p] = sum over the blends of pixel p of w n_c, accumulated as N_c = fma(n_c, w, N_c) with the
- *           colour's w = alpha * T and order.  No background term: [V,3,H,W], world space, unnormalised, 0 where nothing
- *           blends.
- *   grads   dL/dN enters dL/dalpha as cg += n . dL/dN.  Wn = sum w dL/dN per (view, Gaussian) is dL/dn; times the flip sign,
- *           through d(column k of R)/dq (and the normalise Jacobian for raw), it is ADDED to dL_drots.  Scales, means and
- *           campos get no gradient through n (the argmin and the flip are piecewise constant), only the alpha-path terms.
- * Colour, depth, alpha, radii and the state buffers are byte-identical to the call without normals, and the deterministic
- * partial count is unchanged.  cov3D_precomp has no axis: B200GS_E_ARGS.  The classic comparator and the bulk-copy build
- * return B200GS_E_UNSUPPORTED.
- *   struct_bytes   sizeof(b200gs_normals_io) (a smaller value is B200GS_E_ARGS)
- *   gauss_normals  [V*P] x 16 B device workspace, 16-byte aligned: the forward writes (sign n, sign) of every (view, Gaussian);
- *                  the backward reads it, so it must survive from the forward to its backward like the state buffers
- *   out_normal     [V,3,H,W] (forward output)
- *   dL_dnormal     [V,3,H,W] (backward input); NULL = zero: the backward is then exactly the call without normals
- *   normal_wn      [V*P] x 16 B device workspace, 16-byte aligned (backward with dL_dnormal): the Wn sums
- *   nrm_partials   deterministic backward with dL_dnormal: nrm_partials_bytes >= 16 * partial_capacity bytes, 16-byte
- *                  aligned, one float4 per partial at its slot (det_buf's layout and size do not change)
- * The backward forms take the argument lists of b200gs_backward_opts, b200gs_backward_deterministic_opts and the two absgrad
- * forms, with the io struct after opts. */
-typedef struct b200gs_normals_io {
-    int32_t struct_bytes;
-    float *gauss_normals;
-    float *out_normal;
-    const float *dL_dnormal;
-    float *normal_wn;
-    void *nrm_partials;
-    size_t nrm_partials_bytes;
-} b200gs_normals_io;
-int b200gs_forward_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-                                const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
-                                const float *scales, const float *rotations, const float *cov3D_precomp,
-                                const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                                float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
-                                void *geom_buf, size_t geom_bytes,
-                                void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
-                                void *image_buf, size_t image_bytes,
-                                int64_t *num_rendered, void *stream);
-int b200gs_backward_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-                                 const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
-                                 const float *scales, const float *rotations, const float *cov3D_precomp,
-                                 const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                                 const int32_t *radii,
-                                 const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                                 const void *image_buf, int64_t num_rendered,
-                                 const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                 float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
-                                 float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                 void *scratch, size_t scratch_bytes, void *stream);
-int b200gs_backward_deterministic_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
-                                               const b200gs_normals_io *nrm,
-                                               const float *means3D, const float *shs, const float *colors_precomp,
-                                               const float *opacities, const float *scales, const float *rotations,
-                                               const float *cov3D_precomp, const float *bg, const float *viewmatrix,
-                                               const float *projmatrix, const float *campos, const int32_t *radii,
-                                               const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                                               const void *image_buf, int64_t num_rendered,
-                                               const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                               float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                                               float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                               void *scratch, size_t scratch_bytes,
-                                               void *det_buf, size_t det_bytes, int64_t partial_capacity, int64_t *n_partials,
-                                               void *stream);
-int b200gs_backward_absgrad_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-                                         const float *means3D, const float *shs, const float *colors_precomp,
-                                         const float *opacities, const float *scales, const float *rotations,
-                                         const float *cov3D_precomp, const float *bg, const float *viewmatrix,
-                                         const float *projmatrix, const float *campos, const int32_t *radii,
-                                         const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                                         const void *image_buf, int64_t num_rendered,
-                                         const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                         float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                                         float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                         float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream);
-int b200gs_backward_deterministic_absgrad_normals_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
-                                                       const b200gs_normals_io *nrm,
-                                                       const float *means3D, const float *shs, const float *colors_precomp,
-                                                       const float *opacities, const float *scales, const float *rotations,
-                                                       const float *cov3D_precomp, const float *bg, const float *viewmatrix,
-                                                       const float *projmatrix, const float *campos, const int32_t *radii,
-                                                       const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                                                       const void *image_buf, int64_t num_rendered,
-                                                       const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                                       float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                                                       float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                                       float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes,
-                                                       void *det_buf, size_t det_bytes, int64_t partial_capacity,
-                                                       int64_t *n_partials, void *abs_partials, size_t abs_partials_bytes,
-                                                       void *stream);
-
-/* ---- geometry outputs: median depth and depth second moment of the blend (additive to ABI 4) ---------------------------
- * For view v and pixel p, over the blends of p in the colour's order, with the colour's alpha, T (before the blend),
- * w = alpha * T and d the Gaussian's view-space depth (DESIGN.md section 2):
- *   depth2   out_depth2[v,0,p] = M2 = sum w d^2, accumulated as M2 = fma(d * d, w, M2).  No background term; 0 where nothing
- *            blends.  With alpha and depth: the depth distortion sum_{i<j} w_i w_j (d_i - d_j)^2 = A * M2 - M1^2.
- *   median   out_median[v,0,p] = d of the LAST blend whose T is > 0.5 (strict, on the float32 T): the blend at which T
- *            crosses 1/2, or the last blend if T never reaches it.  0 where nothing blends.  median_pos[v,p] = its 1-based
- *            position in the tile's list (0 = none).
- *   grads    dL/dM2 enters dL/dalpha as cg += d^2 dL/dM2, and adds sum_p w 2d dL/dM2 to the Gaussian's depth gradient.
- *            dL/dmedian adds dL/dmedian_p to the depth gradient of p's median Gaussian only (the selection is piecewise
- *            constant: no alpha-path term).  Both reach the means through the existing depth term.
- * Colour, depth, alpha, normals, radii and the state buffers are byte-identical to the call without geometry, and the
- * deterministic partial count is unchanged.  Combines with SH or precomputed colours, raw parameters, cov3D_precomp,
- * antialiasing, the 3D filter, per-view means, normals, absgrad and the deterministic backward.  The classic comparator and
- * the bulk-copy build return B200GS_E_UNSUPPORTED; the contribution forward has no geometry form.
- *   struct_bytes   sizeof(b200gs_geometry_io) (a smaller value is B200GS_E_ARGS)
- *   out_median     [V,1,H,W] (forward output; NULL in a forward is B200GS_E_ARGS)
- *   out_depth2     [V,1,H,W] (forward output; NULL in a forward is B200GS_E_ARGS)
- *   median_pos     [V,H,W] x u32 device workspace, 4-byte aligned (else B200GS_E_BUFFER; NULL is B200GS_E_ARGS): the forward
- *                  writes it, the backward reads it, so it must survive from the forward to its backward like the state buffers
- *   dL_dmedian     [V,1,H,W] (backward input); NULL = zero
- *   dL_ddepth2     [V,1,H,W] (backward input); NULL = zero.  With both NULL the backward is exactly the call without geometry.
- * Each entry point takes a nullable b200gs_normals_io (NULL: no normals; otherwise as the normals forms, including its
- * errors) and the geometry io after opts.  The forward takes b200gs_forward_opts' arguments after them.  The backward forms
- * take the arguments of b200gs_backward_absgrad_opts and b200gs_backward_deterministic_absgrad_opts, with dL_dmeans2D_abs
- * nullable (NULL: no absolute gradients, and abs_partials is then not read).  A NULL geometry io is B200GS_E_ARGS. */
-typedef struct b200gs_geometry_io {
-    int32_t struct_bytes;
-    float *out_median;
-    float *out_depth2;
-    uint32_t *median_pos;
-    const float *dL_dmedian;
-    const float *dL_ddepth2;
-} b200gs_geometry_io;
-int b200gs_forward_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-                                 const b200gs_geometry_io *geo,
-                                 const float *means3D, const float *shs, const float *colors_precomp, const float *opacities,
-                                 const float *scales, const float *rotations, const float *cov3D_precomp,
-                                 const float *bg, const float *viewmatrix, const float *projmatrix, const float *campos,
-                                 float *out_color, float *out_depth, float *out_alpha, int32_t *radii,
-                                 void *geom_buf, size_t geom_bytes,
-                                 void *binning_buf, size_t binning_bytes, int64_t instance_capacity,
-                                 void *image_buf, size_t image_bytes,
-                                 int64_t *num_rendered, void *stream);
-int b200gs_backward_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts, const b200gs_normals_io *nrm,
-                                  const b200gs_geometry_io *geo,
-                                  const float *means3D, const float *shs, const float *colors_precomp,
-                                  const float *opacities, const float *scales, const float *rotations,
-                                  const float *cov3D_precomp, const float *bg, const float *viewmatrix,
-                                  const float *projmatrix, const float *campos, const int32_t *radii,
-                                  const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                                  const void *image_buf, int64_t num_rendered,
-                                  const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                  float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                                  float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                  float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes, void *stream);
-int b200gs_backward_deterministic_geometry_opts(const b200gs_params *prm, const b200gs_render_opts *opts,
-                                                const b200gs_normals_io *nrm, const b200gs_geometry_io *geo,
-                                                const float *means3D, const float *shs, const float *colors_precomp,
-                                                const float *opacities, const float *scales, const float *rotations,
-                                                const float *cov3D_precomp, const float *bg, const float *viewmatrix,
-                                                const float *projmatrix, const float *campos, const int32_t *radii,
-                                                const void *geom_buf, const void *binning_buf, int64_t instance_capacity,
-                                                const void *image_buf, int64_t num_rendered,
-                                                const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                                                float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors,
-                                                float *dL_dopacity, float *dL_dscales, float *dL_drots, float *dL_dcov3D,
-                                                float *dL_dmeans2D_abs, void *scratch, size_t scratch_bytes,
-                                                void *det_buf, size_t det_bytes, int64_t partial_capacity,
-                                                int64_t *n_partials, void *abs_partials, size_t abs_partials_bytes,
-                                                void *stream);
 
 /* ---- 3D smoothing filter: per-Gaussian maximal sampling rate over a camera set (Mip-Splatting's 3D filter) ------------
  * For each of the n_views cameras (viewmatrix [n_views,16] device, tanfovx / tanfovy host [n_views], shared H x W), with

@@ -29,8 +29,9 @@ def test_every_declared_symbol_is_exported(lib):
     assert set(rasterizer.EXPORTS) == declared
 
 
-def test_abi_version_4_and_size_queries_are_sane(lib):
-    """ABI 4: b200gs_state_view ends with the contributor-mask region.  The library, the header and the ctypes mirror agree."""
+def test_abi_version_5_and_size_queries_are_sane(lib):
+    """ABI 5: every optional render feature travels in b200gs_render_opts; b200gs_state_view ends with the contributor-mask
+    region.  The library, the header and the ctypes mirror agree."""
     sz, i32, i64 = ctypes.c_size_t, ctypes.c_int32, ctypes.c_int64
     lib.b200gs_geom_bytes.restype = sz; lib.b200gs_geom_bytes.argtypes = [i32, i32]
     lib.b200gs_image_bytes.restype = sz; lib.b200gs_image_bytes.argtypes = [i32, i32, i32]
@@ -38,8 +39,8 @@ def test_abi_version_4_and_size_queries_are_sane(lib):
     lib.b200gs_backward_scratch_bytes.restype = sz; lib.b200gs_backward_scratch_bytes.argtypes = [i32, i32]
     from humangaussian_b200 import rasterizer
     hdr = open(os.path.join(ROOT, "include", "b200gs.h")).read()
-    assert re.search(r"#define B200GS_ABI_VERSION 4\b", hdr)
-    assert lib.b200gs_abi_version() == 4 and rasterizer.ABI_VERSION == 4
+    assert re.search(r"#define B200GS_ABI_VERSION 5\b", hdr)
+    assert lib.b200gs_abi_version() == 5 and rasterizer.ABI_VERSION == 5
     assert [f[0] for f in rasterizer._StateView._fields_][-2:] == ["contributor_masks", "contributor_mask_words"]
     assert lib.b200gs_geom_bytes(1000, 1) >= 1000 * (48 + 4 + 4 + 8 + 1)
     assert lib.b200gs_geom_bytes(1000, 4) >= 4 * 1000 * 65
@@ -85,7 +86,8 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
     src = tmp_path / "layout.c"
     fields = {"b200gs_params": [f[0] for f in rasterizer._Params._fields_],
               "b200gs_densify_cfg": [f[0] for f in densify._Cfg._fields_],
-              "b200gs_state_view": [f[0] for f in rasterizer._StateView._fields_]}
+              "b200gs_state_view": [f[0] for f in rasterizer._StateView._fields_],
+              "b200gs_render_opts": [f[0] for f in rasterizer._RenderOpts._fields_]}
     body = ['#include <stdio.h>', '#include <stddef.h>', '#include "b200gs.h"', 'int main(void){']
     for s, fs in fields.items():
         body.append(f'printf("{s} %zu\\n", sizeof({s}));')
@@ -96,7 +98,8 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
     exe = tmp_path / "layout"
     subprocess.check_call(["/usr/bin/gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
     got = dict(line.split() for line in subprocess.check_output([str(exe)], text=True).splitlines())
-    mirrors = {"b200gs_params": rasterizer._Params, "b200gs_densify_cfg": densify._Cfg, "b200gs_state_view": rasterizer._StateView}
+    mirrors = {"b200gs_params": rasterizer._Params, "b200gs_densify_cfg": densify._Cfg, "b200gs_state_view": rasterizer._StateView,
+               "b200gs_render_opts": rasterizer._RenderOpts}
     for s, cls in mirrors.items():
         assert int(got[s]) == C.sizeof(cls), s
         for f in fields[s]:

@@ -88,35 +88,76 @@ def _lib(path):
     return C.CDLL(path)
 
 
-def _abs_call(L, det, m2d_abs=True, abs_partials=True, abs_bytes=8 * 16):
-    """one P = 0 call of the absgrad entry points: every device pointer is a host dummy (nothing is dereferenced for P = 0)"""
+def _abs_call(L, det, m2d_abs=True, abs_partials=True, abs_bytes=8 * 16, **fields):
+    """one P = 0 call of b200gs_backward_opts / b200gs_backward_deterministic_opts with the absolute gradients in the options
+    (and any other option fields given): every device pointer is a host dummy (nothing is dereferenced for P = 0)"""
     from humangaussian_b200 import rasterizer as R
     prm, _tx, _ty = R._make_params(0, 1, 0, 1, 8, 8, 1.0, [1.0], [1.0])
     buf = (C.c_float * 64)()
     d = C.cast(buf, C.c_void_p)
     n = C.c_int64(-1)
+    o = R._RenderOpts(C.sizeof(R._RenderOpts), 0, None)
+    o.dL_dmeans2D_abs = d if m2d_abs else None
+    if det:
+        o.abs_partials, o.abs_partials_bytes = (d if abs_partials else None), abs_bytes
+    for k, v in fields.items():
+        setattr(o, k, v)
     grads = [d] * 8  # dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors (NULL below), dL_dopacity, dL_dscales, dL_drots, dL_dcov3D
     grads[3], grads[7] = None, None
-    common = [C.byref(prm), None, d, d, None, d, d, d, None, d, d, d, d, d, d, d, C.c_int64(1), d, C.c_int64(0), None, None, None,
-              *grads, d if m2d_abs else None, d, C.c_size_t(256)]
+    common = [C.byref(prm), C.byref(o), d, d, None, d, d, d, None, d, d, d, d, d, d, d, C.c_int64(1), d, C.c_int64(0), None, None,
+              None, *grads, d, C.c_size_t(256)]
     if not det:
-        return L.b200gs_backward_absgrad_opts(*common, None)
-    return L.b200gs_backward_deterministic_absgrad_opts(*common, d, C.c_size_t(256), C.c_int64(16), C.byref(n),
-                                                        d if abs_partials else None, C.c_size_t(abs_bytes), None)
+        return L.b200gs_backward_opts(*common, None)
+    return L.b200gs_backward_deterministic_opts(*common, d, C.c_size_t(256), C.c_int64(16), C.byref(n), None)
 
 
-def test_abi_absgrad_entry_points_on_empty_scenes():
+def _fwd_call(L, **fields):
+    """one P = 0 b200gs_forward_opts call with the given option fields, for argument errors found before any device work"""
+    from humangaussian_b200 import rasterizer as R
+    prm, _tx, _ty = R._make_params(0, 1, 0, 1, 8, 8, 1.0, [1.0], [1.0])
+    buf = (C.c_float * 64)()
+    d = C.cast(buf, C.c_void_p)
+    n = C.c_int64(-1)
+    o = R._RenderOpts(C.sizeof(R._RenderOpts), 0, None)
+    for k, v in fields.items():
+        setattr(o, k, v)
+    ins = [d, d, None, d, d, d, None, d, d, d, d]  # means3D .. campos, as in _abs_call
+    return L.b200gs_forward_opts(C.byref(prm), C.byref(o), *ins, d, d, d, d, d, C.c_size_t(1 << 20), d, C.c_size_t(1 << 20),
+                                 C.c_int64(1 << 16), d, C.c_size_t(1 << 20), C.byref(n), None)
+
+
+def test_abi_absgrad_options_on_empty_scenes():
     from humangaussian_b200 import rasterizer as R
     L = _lib(os.path.join(ROOT, "humangaussian_b200", "libb200gs.so"))
     for det in (False, True):
         assert _abs_call(L, det) == R.OK
-        assert _abs_call(L, det, m2d_abs=False) == R.E_ARGS
+        assert _abs_call(L, det, m2d_abs=False) == R.OK  # no dL_dmeans2D_abs: the call without absolute gradients
     assert _abs_call(L, True, abs_partials=False) == R.E_ARGS
     assert _abs_call(L, True, abs_bytes=8 * 16 - 1) == R.E_BUFFER  # 8 bytes per partial of partial_capacity = 16
-    assert {"b200gs_backward_absgrad_opts", "b200gs_backward_deterministic_absgrad_opts"} <= set(R.EXPORTS)
+    assert _abs_call(L, True, m2d_abs=False, abs_partials=False) == R.OK  # abs_partials is read with dL_dmeans2D_abs only
 
 
-def test_abi_classic_comparator_reports_unsupported():
+def test_abi_option_combinations_on_empty_scenes():
+    """The rules of b200gs_render_opts that the C layer checks before any device work: contribution scores with normals or
+    geometry, dL_dnormal without gauss_normals, and a geometry gradient without median_pos are argument errors."""
+    from humangaussian_b200 import rasterizer as R
+    L = _lib(os.path.join(ROOT, "humangaussian_b200", "libb200gs.so"))
+    ws = (C.c_uint64 * 4)()
+    aligned = (C.c_float * 64)()  # 16-byte aligned host memory stands in for the device workspaces
+    p = C.cast(aligned, C.c_void_p)
+    contrib = dict(weight_sum=C.cast(ws, C.c_void_p), weight_max=p, touches=p)
+    assert _fwd_call(L, **contrib, gauss_normals=p, out_normal=p) == R.E_ARGS
+    assert _fwd_call(L, **contrib, median_pos=p, out_median=p, out_depth2=p) == R.E_ARGS
+    assert _fwd_call(L, weight_sum=C.cast(ws, C.c_void_p)) == R.E_ARGS  # an accumulator without the other two
+    for det in (False, True):
+        assert _abs_call(L, det, dL_dnormal=p) == R.E_ARGS
+        assert _abs_call(L, det, dL_dnormal=p, gauss_normals=p, normal_wn=p, nrm_partials=p, nrm_partials_bytes=1 << 20) == R.OK
+        for grad in ("dL_dmedian", "dL_ddepth2"):
+            assert _abs_call(L, det, **{grad: p}) == R.E_ARGS
+            assert _abs_call(L, det, **{grad: p}, median_pos=p) == R.OK
+
+
+def test_abi_classic_comparator_rejects_absgrad_options():
     from humangaussian_b200 import rasterizer as R
     L = _lib(os.path.join(ROOT, "baseline", "libb200gs_classic.so"))
     for det in (False, True):

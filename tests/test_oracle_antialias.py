@@ -202,7 +202,7 @@ def test_render_opts_layout_matches_the_header(tmp_path):
         assert int(got[f]) == getattr(_RenderOpts, f).offset, f
 
 
-def test_render_opts_struct_bytes_is_checked(lib):
+def test_render_opts_abi5_struct_bytes_is_checked(lib):
     """Too small a struct_bytes is an argument error on every *_opts entry; NULL and a full struct are accepted.  An empty
     scene (P = 0) returns from the backward before any device work, so this runs without a GPU."""
     from humangaussian_b200 import rasterizer as R
@@ -226,7 +226,8 @@ def test_render_opts_struct_bytes_is_checked(lib):
         o = R._RenderOpts(small, 1)
         assert bwd(C.byref(o)) == R.E_ARGS and fwd(C.byref(o)) == R.E_ARGS, small
         assert bwd(C.byref(o), det=True) == R.E_ARGS, small
-    for o in (None, C.byref(R._render_opts(True)), C.byref(R._render_opts(False)), C.byref(R._RenderOpts(64, 1))):
+    larger = R._RenderOpts(C.sizeof(R._RenderOpts) + 64, 1)  # a newer header's struct: the fields this library knows are read
+    for o in (None, C.byref(R._render_opts(True)), C.byref(R._render_opts(False)), C.byref(larger)):
         assert bwd(o) == R.OK
     # the filtered backward needs the opacities it multiplies (as raw parameters do)
     no_op = list(inputs)

@@ -227,14 +227,14 @@ def lib():
     return rasterizer._lib
 
 
-def test_render_opts_has_the_filter_pointer():
+def test_render_opts_keeps_the_filter_pointer_at_offset_8():
     from humangaussian_b200.rasterizer import _RenderOpts
-    assert C.sizeof(_RenderOpts) == 16 and _RenderOpts.filter3d_var.offset == 8
+    assert C.sizeof(_RenderOpts) == 152 and _RenderOpts.filter3d_var.offset == 8
 
 
-def test_render_opts_struct_bytes_rule(lib):
-    """struct_bytes 8 (a header before the filter pointer) and >= 16 are accepted; 0, 4 and 9..15 (a cut pointer) are
-    argument errors.  The filter with cov3D_precomp is an argument error; the filtered backward needs opacities.  P = 0:
+def test_render_opts_abi5_struct_bytes_rule(lib):
+    """struct_bytes 8 (a header before the filter pointer), 16 (a header that ends with it) and >= sizeof are accepted; 0, 4,
+    9..15 (a cut pointer) and the sizes between 16 and sizeof (a cut feature block) are argument errors.  The filter with cov3D_precomp is an argument error; the filtered backward needs opacities.  P = 0:
     every call returns before any device work, so this runs without a GPU."""
     from humangaussian_b200 import rasterizer as R
     prm, _, _ = R._make_params(0, 1, 0, 1, 16, 16, 1.0, [1.0], [1.0])
@@ -252,10 +252,11 @@ def test_render_opts_struct_bytes_rule(lib):
         return lib.b200gs_forward_opts(C.byref(prm), opts, *ins[:11], fake, fake, fake, fake, fake, 1, fake, 1, 1, fake, 1,
                                        C.byref(n), None)
 
-    for nbytes in (0, 4, *range(9, 16)):
+    full = C.sizeof(R._RenderOpts)
+    for nbytes in (0, 4, *range(9, 16), 17, 24, 64, full - 8, full - 1):
         o = R._RenderOpts(nbytes, 1, 256)
         assert fwd(C.byref(o)) == R.E_ARGS and bwd(C.byref(o)) == R.E_ARGS and bwd(C.byref(o), det=True) == R.E_ARGS, nbytes
-    for nbytes in (8, 16, 64):
+    for nbytes in (8, 16, full, full + 64):
         for ptr in (None, 256):
             assert bwd(C.byref(R._RenderOpts(nbytes, 1, ptr))) == R.OK, (nbytes, ptr)
     # cov3D_precomp + filter: an argument error from the forward and the backward; an old 8-byte header never reads the pointer
