@@ -746,6 +746,80 @@ int b200gs_adam_packed(const b200gs_adam_cfg *cfg, float *params, const float *g
     return B200GS_OK;
 }
 
+// ---- mesh export (mesh.cu) ----
+static int field_split(int32_t res, int32_t num_blocks)
+{   // chunk length per axis, or 0 when the blocks or the field CTAs (one per block and 512 voxels) outgrow 32-bit indices
+    if (res < 1 || num_blocks < 1 || res / num_blocks < 1) return 0;
+    const int64_t split = res / num_blocks, nch = (res + split - 1) / split;
+    if (nch * nch * nch * ((split * split * split + 511) / 512) > 0x7fffffffLL) return 0;
+    return (int)split;
+}
+
+size_t b200gs_density_field_scratch_bytes(int32_t P, int32_t resolution, int32_t num_blocks)
+{
+    const int split = field_split(resolution, num_blocks);
+    return split && P >= 0 ? density_field_scratch_bytes(P, resolution, split) : 0;
+}
+
+int b200gs_density_field(int32_t P, const float *means, const float *cov6, const float *opacities, int32_t resolution,
+                         int32_t num_blocks, const float *samples, float relax, float *field, void *scratch, size_t scratch_bytes,
+                         void *stream)
+{
+    if (P < 0 || !field || resolution < 1 || num_blocks < 1) return B200GS_E_ARGS;
+    const int split = field_split(resolution, num_blocks);
+    if (!split) return B200GS_E_RANGE;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (P == 0) {
+        CK(cudaMemsetAsync(field, 0, (size_t)resolution * resolution * resolution * 4, st), "density_field memset");
+        return B200GS_OK;
+    }
+    if (!means || !cov6 || !opacities || !samples || !scratch) return B200GS_E_ARGS;
+    if (scratch_bytes < density_field_scratch_bytes(P, resolution, split)) return B200GS_E_BUFFER;
+    int nl = 0;
+    if (launch_density_field(P, means, cov6, opacities, resolution, split, samples, relax, field, (char *)scratch, scratch_bytes, st, &nl))
+        return B200GS_E_RANGE;
+    g_launches += nl;
+    CK(cudaGetLastError(), "density_field launch");
+    return B200GS_OK;
+}
+
+static bool mc_dims_ok(int32_t X, int32_t Y, int32_t Z)
+{   // vertex ids are int32 and there is at most one vertex per grid edge, fewer than 3 per grid point
+    return X >= 2 && Y >= 2 && Z >= 2 && 3 * (int64_t)X * Y * Z <= 0x7fffffffLL;
+}
+
+size_t b200gs_marching_cubes_scratch_bytes(int32_t X, int32_t Y, int32_t Z)
+{
+    return mc_dims_ok(X, Y, Z) ? marching_cubes_scratch_bytes(X, Y, Z) : 0;
+}
+
+int b200gs_marching_cubes_count(int32_t X, int32_t Y, int32_t Z, const float *volume, float iso, void *scratch, size_t scratch_bytes,
+                                uint64_t *counts, void *stream)
+{
+    if (!volume || !scratch || !counts) return B200GS_E_ARGS;
+    if (!mc_dims_ok(X, Y, Z)) return B200GS_E_RANGE;
+    if (scratch_bytes < marching_cubes_scratch_bytes(X, Y, Z)) return B200GS_E_BUFFER;
+    int nl = 0;
+    if (launch_marching_cubes_count(X, Y, Z, volume, iso, (char *)scratch, scratch_bytes, counts, (cudaStream_t)stream, &nl))
+        return cuda_fail(cudaGetLastError(), "marching_cubes_count memset");
+    g_launches += nl;
+    CK(cudaGetLastError(), "marching_cubes_count launch");
+    return B200GS_OK;
+}
+
+int b200gs_marching_cubes_emit(int32_t X, int32_t Y, int32_t Z, const float *volume, float iso, const void *scratch,
+                               size_t scratch_bytes, float *vertices, int32_t *faces, void *stream)
+{
+    if (!volume || !scratch) return B200GS_E_ARGS;
+    if (!mc_dims_ok(X, Y, Z)) return B200GS_E_RANGE;
+    if (scratch_bytes < marching_cubes_scratch_bytes(X, Y, Z)) return B200GS_E_BUFFER;
+    int nl = 0;
+    launch_marching_cubes_emit(X, Y, Z, volume, iso, (const char *)scratch, scratch_bytes, vertices, faces, (cudaStream_t)stream, &nl);
+    g_launches += nl;
+    CK(cudaGetLastError(), "marching_cubes_emit launch");
+    return B200GS_OK;
+}
+
 int b200gs_test_sort_pairs(uint32_t *keys_a, uint32_t *keys_b, uint32_t *vals_a, uint32_t *vals_b, int64_t n, int32_t nbits,
                            void *scratch, size_t scratch_bytes, int32_t *result_in_b, void *stream)
 {

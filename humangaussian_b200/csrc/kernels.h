@@ -251,3 +251,14 @@ struct AdamArgs {
 };
 void launch_adam_packed(const AdamArgs &a, int64_t total, float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
                         cudaStream_t st);
+
+// mesh export (mesh.cu): density field over blocks of `split` samples per axis, and marching cubes.  Nonzero return:
+// scratch too small (-1) or a failed launch setup (-2).
+size_t density_field_scratch_bytes(int P, int res, int split);
+int launch_density_field(int P, const float *means, const float *cov6, const float *opac, int res, int split, const float *samples,
+                         float relax, float *field, char *scratch, size_t scratch_bytes, cudaStream_t st, int *n_launches);
+size_t marching_cubes_scratch_bytes(int X, int Y, int Z);
+int launch_marching_cubes_count(int X, int Y, int Z, const float *vol, float iso, char *scratch, size_t scratch_bytes, uint64_t *counts,
+                                cudaStream_t st, int *n_launches);
+int launch_marching_cubes_emit(int X, int Y, int Z, const float *vol, float iso, const char *scratch, size_t scratch_bytes, float *verts,
+                               int32_t *faces, cudaStream_t st, int *n_launches);

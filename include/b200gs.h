@@ -462,6 +462,36 @@ typedef struct b200gs_adam_cfg {
 int b200gs_adam_packed(const b200gs_adam_cfg *cfg, float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
                        void *stream);
 
+/* ---- mesh export (the reference's GaussianModel.extract_fields / extract_mesh, gs_renderer.py:241-361) -------------
+ * b200gs_density_field: field [res,res,res] (device, x-major: field[(x*res + y)*res + z]) of
+ *   sum over Gaussians g of block(x,y,z) of opacities[g] * exp(power),  power = -0.5 (d^T Sigma^-1 d) (0 where power > 0),
+ *   d = (samples[x], samples[y], samples[z]) - means[g], Sigma^-1 the closed-form inverse of cov6 [a,b,c,d,e,f] =
+ *   [xx,xy,xz,yy,yz,zz] with 1e-24 added to the determinant, every product and sum in the reference's order, rounded once.
+ *   Blocks are chunks of split = res / num_blocks samples per axis (the last may be short; there may be more than
+ *   num_blocks).  Gaussian g belongs to a block iff, on all three axes, min(chunk samples) - relax < mean < max(chunk
+ *   samples) + relax in float32.  The sum runs in a fixed order: the same bits on every call.
+ *     means [P,3], cov6 [P,6], opacities [P], samples [res] (device); relax = (2 / num_blocks) * relax_ratio as a float;
+ *     scratch of b200gs_density_field_scratch_bytes(P, res, num_blocks).  P = 0 zeroes the field.
+ *   B200GS_E_ARGS: P < 0, res < 1 or num_blocks < 1; B200GS_E_RANGE: res / num_blocks < 1, or the blocks or the field's
+ *   CTAs (one per block and 512 voxels) outgrow 32-bit indices. */
+size_t b200gs_density_field_scratch_bytes(int32_t P, int32_t resolution, int32_t num_blocks);
+int b200gs_density_field(int32_t P, const float *means, const float *cov6, const float *opacities, int32_t resolution,
+                         int32_t num_blocks, const float *samples, float relax, float *field, void *scratch, size_t scratch_bytes,
+                         void *stream);
+/* Marching cubes over volume [X,Y,Z] (device, z fastest) at `iso`: a corner is inside iff its value > iso; one vertex per
+ * grid edge whose ends differ, at p0 + t along the edge, t = (iso - v0) / (v1 - v0), in index coordinates; triangles wound
+ * with normals toward lower values.  Vertices are numbered in order of (grid point at the edge's low end, axis), triangles
+ * in order of (cell, table row); the table is generated by humangaussian_b200/mc_table.py.
+ *   b200gs_marching_cubes_count classifies and scans: counts [2] uint64 (device) = vertices, triangles.  The caller reads
+ *   them (the one host wait of an extraction) to size vertices [n_vertices,3] float and faces [n_triangles,3] int32, then
+ *   b200gs_marching_cubes_emit writes them from the same scratch (either output may be NULL to skip it).
+ *   X, Y, Z >= 2 and 3*X*Y*Z <= INT32_MAX (vertex ids are int32), else B200GS_E_RANGE. */
+size_t b200gs_marching_cubes_scratch_bytes(int32_t X, int32_t Y, int32_t Z);
+int b200gs_marching_cubes_count(int32_t X, int32_t Y, int32_t Z, const float *volume, float iso, void *scratch, size_t scratch_bytes,
+                                uint64_t *counts, void *stream);
+int b200gs_marching_cubes_emit(int32_t X, int32_t Y, int32_t Z, const float *volume, float iso, const void *scratch,
+                               size_t scratch_bytes, float *vertices, int32_t *faces, void *stream);
+
 /* ---- introspection of the state buffers, for parity tests (tile/sort indices must match bit-for-bit) ------- */
 typedef struct b200gs_state_view {
     const void *geom_records;     /* [V*P] x 48 B: px,py,hx,hy | conicA,conicB,conicC,opacity | r,g,b,depth */
