@@ -42,38 +42,69 @@ def _rect_colors(rect, ids):
     return colors
 
 
-def per_pixel_jacobian(inp, gimg, antialiasing=False, filter_3d=None):
-    """dense [P, 2, H*W] float64 array J with J[k, c, p] = dL_p / dmeans2D[k, c] (NDC units), for one view of `inp` (the
-    oracle's activated inputs) under the image gradients gimg = (gC [3,H,W], gD [1,H,W], gA [1,H,W]).  filter_3d: [P]
-    variances; the 3D filter's s', o' are formed as the kernels form them (filter3d_reference.filter_params)."""
+def pixel_losses(inp, gimg, antialiasing=False, filter_3d=None, gN=None, gM2=None):
+    """(losses, state, radii): losses(m2d) is the [H*W] float64 tensor of L_p for the NDC offsets m2d [P,3], one view of
+    `inp` (the oracle's activated inputs).  L_p = gC.c + gD d + gA a at p, plus with gN [3,H,W] the normal pass gN.N (n the
+    shortest-scale axis of the unfiltered scales, flipped to face the camera, bg = 0) and with gM2 [H,W] the depth second
+    moment gM2 M2 (colours (z^2, 0, 0), bg = 0).  filter_3d: [P] variances; the 3D filter's s', o' are formed as the kernels
+    form them (filter3d_reference.filter_params)."""
     from oracle.dense_ref import dense_render
+    t64 = lambda a: torch.tensor(np.asarray(a), dtype=torch.float64)
+    if gN is not None:  # the axis and the flip come from the unfiltered activated parameters
+        import normal_reference as NR
+        sign = NR.gauss_normals(inp["means3D"], inp["campos"], inp["scales"], inp["rotations"])[:, 3]
+        nrm = NR.normals_torch(t64(inp["rotations"]), NR.axis(inp["scales"]), sign)
     if filter_3d is not None:
         from filter3d_reference import filter_params
         sp, op, _ = filter_params(inp["scales"], inp["opacities"], filter_3d)
         inp = dict(inp, scales=sp, opacities=op)
     st, radii = _state(inp, antialiasing)
     H, W = inp["image_height"], inp["image_width"]
-    P = len(radii)
-    t64 = lambda a: torch.tensor(np.asarray(a), dtype=torch.float64)
     ids = np.nonzero(radii > 0)[0]
     order = ids[np.lexsort((ids, st["depths"][ids]))]
     kw = dict(means3D=t64(inp["means3D"]), opacities=t64(inp["opacities"]), viewmatrix=t64(inp["viewmatrix"]),
-              projmatrix=t64(inp["projmatrix"]), campos=t64(inp["campos"]), bg=t64(inp["bg"]), H=H, W=W, tanfovx=inp["tanfovx"],
-              tanfovy=inp["tanfovy"], radii=radii, rect=st["rect"], order=order, sh_degree=inp.get("sh_degree", 0),
-              scale_modifier=inp.get("scale_modifier", 1.0))
-    for k in ("shs", "colors_precomp", "scales", "rotations", "cov3D_precomp"):
+              projmatrix=t64(inp["projmatrix"]), campos=t64(inp["campos"]), H=H, W=W, tanfovx=inp["tanfovx"],
+              tanfovy=inp["tanfovy"], radii=radii, rect=st["rect"], order=order, scale_modifier=inp.get("scale_modifier", 1.0))
+    for k in ("scales", "rotations", "cov3D_precomp"):
         if inp.get(k) is not None:
             kw[k] = t64(inp[k])
+    colours = dict(bg=t64(inp["bg"]), sh_degree=inp.get("sh_degree", 0))
+    for k in ("shs", "colors_precomp"):
+        if inp.get(k) is not None:
+            colours[k] = t64(inp[k])
     if antialiasing:
         from aa_reference import dense_render_aa as render
     else:
         render = dense_render
     gC, gD, gA = (t64(g) for g in gimg)
+    zero = torch.zeros(3, dtype=torch.float64)
+    if gM2 is not None:
+        from geometry_reference import view_depth64
+        z = view_depth64(kw["means3D"], inp["viewmatrix"])
+        z2 = torch.stack([z * z, torch.zeros_like(z), torch.zeros_like(z)], 1)
 
     def losses(m2d):
-        c, d, a, _ = render(means2D=m2d, **kw)
-        return ((c * gC).sum(0) + (d * gD)[0] + (a * gA)[0]).reshape(-1)  # L_p, [H*W]
+        c, d, a, _ = render(means2D=m2d, **colours, **kw)
+        Lp = (c * gC).sum(0) + (d * gD)[0] + (a * gA)[0]
+        if gN is not None:
+            cn, _, _, _ = render(means2D=m2d, bg=zero, colors_precomp=nrm, **kw)
+            Lp = Lp + (cn * t64(gN)).sum(0)
+        if gM2 is not None:
+            cm, _, _, _ = render(means2D=m2d, bg=zero, colors_precomp=z2, **kw)
+            Lp = Lp + cm[0] * t64(gM2).reshape(H, W)
+        return Lp.reshape(-1)  # L_p, [H*W]
 
+    return losses, st, radii
+
+
+def per_pixel_jacobian(inp, gimg, antialiasing=False, filter_3d=None, gN=None, gM2=None):
+    """dense [P, 2, H*W] float64 array J with J[k, c, p] = dL_p / dmeans2D[k, c] (NDC units), for one view of `inp` (the
+    oracle's activated inputs) under the image gradients gimg = (gC [3,H,W], gD [1,H,W], gA [1,H,W]), and with gN / gM2 the
+    normal and depth-second-moment terms of L_p (pixel_losses; a median gradient is constant in means2D and adds nothing)."""
+    losses, st, radii = pixel_losses(inp, gimg, antialiasing, filter_3d, gN, gM2)
+    H, W = inp["image_height"], inp["image_width"]
+    P = len(radii)
+    ids = np.nonzero(radii > 0)[0]
     J = np.zeros((P, 2, H * W))
     rect = np.asarray(st["rect"]).reshape(P, 4)
     m0 = torch.zeros(P, 3, dtype=torch.float64)
@@ -91,9 +122,9 @@ def per_pixel_jacobian(inp, gimg, antialiasing=False, filter_3d=None):
     return J, radii
 
 
-def absgrad(inp, gimg, antialiasing=False, filter_3d=None):
+def absgrad(inp, gimg, antialiasing=False, filter_3d=None, gN=None, gM2=None):
     """(abs [P,3], signed [P,3], radii): sum_p |g_p| and sum_p g_p per component, z = 0 (float64)"""
-    J, radii = per_pixel_jacobian(inp, gimg, antialiasing, filter_3d)
+    J, radii = per_pixel_jacobian(inp, gimg, antialiasing, filter_3d, gN, gM2)
     P = J.shape[0]
     a, s = np.zeros((P, 3)), np.zeros((P, 3))
     a[:, :2] = np.abs(J).sum(2)
