@@ -32,24 +32,27 @@
 //     no BSSY/BSYNC/BRA inside the pair, about 96 per 32-entry chunk of bookkeeping.  Backward 64 registers, 13.1 KB smem,
 //     no spills; 107 per unrolled pair of hits (53.5 per hit; about 65 with a branch around the contributing-lane block
 //     and separate slot / hit counters), plus the flush.
-//   * Deterministic mode (torch.use_deterministic_algorithms): blend_bwd_det_kernel is the same body with a flush that stores
-//     each (instance, patch) partial into its own slot instead of the REDs; deterministic.cu plans the slots and adds each
-//     Gaussian's partials in a fixed order.  blend_bwd_kernel's SASS does not change.
-//   * Absolute screen-space gradients (densification statistic, DESIGN.md section 2): blend_bwd_abs_kernel and
-//     blend_bwd_det_abs_kernel are the same bodies with a flush that also sums |q (A dx + B dy)| and |q (B dx + C dy)| into
-//     ScreenGrad's padding (or a float2 per partial); absgrad_out_kernel scales them to dL_dmeans2D_abs.  The default
-//     kernels' SASS does not change.
-//   * Contribution scores (DESIGN.md section 2): blend_fwd_contrib_kernel is the forward body with each hit also folded into
-//     its Gaussian's weight_sum / weight_max / touches (warp reductions, then three atomics from lane 0).  blend_fwd_kernel is
-//     the same body's other instantiation.
-//   * Normal maps (DESIGN.md section 2): blend_fwd_nrm_kernel and the four B1 nrm kernels are the same bodies with an NRM flag:
-//     each hit's normal (normals.cu's gauss_normals) is staged next to its slab record, the forward keeps three more sums
-//     per pixel, the backward adds n . dL/dN to cg and the flush sums Wn = sum w dL/dN.  The default kernels' SASS does not
-//     change.
+//   * Two kernel templates: blend_fwd_kernel<CONTRIB, NRM, GEO> (five instantiations: contribution scores never come with
+//     normals or geometry) and blend_bwd_kernel<DET, ABS, NRM, GEO> (all sixteen).  A feature flag adds its code under an
+//     `if` on the flag, its per-warp shared arrays, and its kernel arguments as members of FwdFeatures / BwdFeatures; with
+//     every flag off the code is the default kernel's, so a feature does not change the default kernels' SASS.  The
+//     launchers map the option bits to an instantiation in one place each.
+//   * Deterministic mode (torch.use_deterministic_algorithms): DET selects a flush that stores each (instance, patch)
+//     partial into its own slot instead of the REDs; deterministic.cu plans the slots and adds each Gaussian's partials in
+//     a fixed order.
+//   * Absolute screen-space gradients (densification statistic, DESIGN.md section 2): with ABS the flush also sums
+//     |q (A dx + B dy)| and |q (B dx + C dy)| into ScreenGrad's padding (or a float2 per partial); absgrad_out_kernel scales
+//     them to dL_dmeans2D_abs.
+//   * Contribution scores (DESIGN.md section 2): with CONTRIB the forward also folds each hit into its Gaussian's
+//     weight_sum / weight_max / touches (warp reductions, then three atomics from lane 0).
+//   * Normal maps (DESIGN.md section 2): with NRM each hit's normal (normals.cu's gauss_normals) is staged next to its slab
+//     record, the forward keeps three more sums per pixel, the backward adds n . dL/dN to cg and the flush sums
+//     Wn = sum w dL/dN.
 //   * The compile-time switches below are the A/B experiments DESIGN.md section 5 lists: the
 //     product is BWD_T_DIV=1 and BWD_PARK=16, everything else 0.
 #include "common.cuh"
 #include "kernels.h"
+#include <type_traits>
 
 #define FULL 0xffffffffu
 #ifndef WARPS_PER_CTA
@@ -61,13 +64,14 @@
                           // 12 within noise, 20 blocks 2.5 % slower
 #endif
 #define CTAS_PER_TILE (8 / WARPS_PER_CTA)
-#ifndef FWD_BULK
-#define FWD_BULK 0 // 1: forward blend with cp.async.bulk + mbarrier staging of the id runs (A/B experiment; see DESIGN.md)
-#endif
 #ifndef FWD_MIN_BLOCKS
-// caps the forward kernel at 56 registers (36 warps/SM), no spills; left to itself ptxas takes 60.  The bulk-copy variant
-// spills at 56 and is capped at 64 (32 warps/SM).
-#define FWD_MIN_BLOCKS (FWD_BULK ? 16 : 18)
+#define FWD_MIN_BLOCKS 18 // caps the default forward kernel at 56 registers (36 warps/SM), no spills; left to itself ptxas takes 60
+#endif
+#ifndef FWD_FEATURE_MIN_BLOCKS
+// the forward kernels with a feature: at the default's cap of 56 registers the contribution variant spills 8 bytes in the hit
+// loop; 16 blocks (64 registers, 32 warps/SM, the backward's occupancy) removes the spill (DESIGN.md section 5 lists the
+// registers of every instantiation at this bound)
+#define FWD_FEATURE_MIN_BLOCKS 16
 #endif
 #ifndef BWD_PARK
 #define BWD_PARK 16 // backward: hits parked per flush (8 or 16); 32 / BWD_PARK lanes share a hit in the flush pass.  H100 80GB
@@ -117,6 +121,17 @@ struct FwdPixel {
     uint32_t last, used; // 1-based list position of the last blended entry; entries of the chunk this pixel blended
 };
 
+// The forward's feature arguments: one member per enabled feature, none for a disabled one (an empty base takes no space), so
+// an instantiation's parameters keep the layout (args, contribution outputs, normals, geometry outputs) of the features it has.
+// Code that reads a member sits under `if constexpr` on its flag.
+template <bool> struct FwdContribArg {};
+template <> struct FwdContribArg<true> { ContribOut co; };
+template <bool> struct FwdNrmArg {};
+template <> struct FwdNrmArg<true> { const float4 *gauss_normals; float *out_normal; }; // [V*P] (normals.cu), [V,3,H,W]
+template <bool> struct FwdGeoArg {};
+template <> struct FwdGeoArg<true> { GeoFwd geo; };
+template <bool CONTRIB, bool NRM, bool GEO> struct FwdFeatures : FwdContribArg<CONTRIB>, FwdNrmArg<NRM>, FwdGeoArg<GEO> {};
+
 // One slab hit s (three words) blended into pixel (fpx, fpy): the operation sequence of DESIGN.md section 2.  The three
 // outcomes -- skip (power > 0 or alpha < 1/255), done (T would fall below 1e-4) and blend -- are predicates, not branches:
 // 13.6 of 32 lanes blend per visit, so a branch would diverge and the warp would issue both sides anyway.  A lane that does
@@ -154,9 +169,9 @@ struct GeoPixel {
 // the colour's predicate.
 // GEO (geometry outputs, DESIGN.md section 2): M2 = fma(d*d, w, M2) under the colour's predicate, and a blend whose transmittance
 // before blending is > 0.5 becomes the median (the last such blend wins).
-template <bool CONTRIB, bool NRM = false, bool GEO = false>
-__device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float fpy, FwdPixel &p, uint32_t gid, const ContribOut &co,
-                                              const float4 *ns = nullptr, float *N = nullptr, GeoPixel *gp = nullptr)
+template <bool CONTRIB, bool NRM, bool GEO>
+__device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float fpy, FwdPixel &p, uint32_t gid, const float4 *ns,
+                                              float *N, GeoPixel &gp, const FwdFeatures<CONTRIB, NRM, GEO> &f)
 {
     const float4 g0 = s[0], q1 = s[1], q2 = s[2];
     const float dx = fsub(g0.x, fpx), dy = fsub(g0.y, fpy);
@@ -179,29 +194,28 @@ __device__ __forceinline__ void fwd_blend_hit(const float4 *s, float fpx, float 
         if (blend) { N[0] = ffma(n.x, w, N[0]); N[1] = ffma(n.y, w, N[1]); N[2] = ffma(n.z, w, N[2]); }
     }
     if (GEO) { // (p.T is still the transmittance before this hit; a finished pixel's is <= 0)
-        if (blend) gp->M2 = ffma(fmul(q2.w, q2.w), w, gp->M2);
-        if (blend & (p.T > 0.5f)) { gp->med = q2.w; gp->mpos = __float_as_uint(g0.z); }
+        if (blend) gp.M2 = ffma(fmul(q2.w, q2.w), w, gp.M2);
+        if (blend & (p.T > 0.5f)) { gp.med = q2.w; gp.mpos = __float_as_uint(g0.z); }
     }
     p.T = blend ? test_T : (hit ? -fabsf(p.T) : p.T);
-    if (CONTRIB) contrib_hit(hit & live, blend, w, gid, co);
+    if constexpr (CONTRIB) contrib_hit(hit & live, blend, w, gid, f.co);
 }
 
 // Blends the cnt hits staged in slab s, in order, two per iteration.  gids: the hits' Gaussian indices (CONTRIB only).
 // NRM: ns holds the hits' normals, N the pixel's three normal sums.  GEO: gp is the pixel's geometry state.
-template <bool CONTRIB, bool NRM = false, bool GEO = false>
+template <bool CONTRIB, bool NRM, bool GEO>
 __device__ __forceinline__ void fwd_blend_slab(const float4 *s, int cnt, float fpx, float fpy, FwdPixel &p, const uint32_t *gids,
-                                               const ContribOut &co, const float4 *ns = nullptr, float *N = nullptr,
-                                               GeoPixel *gp = nullptr)
+                                               const float4 *ns, float *N, GeoPixel &gp, const FwdFeatures<CONTRIB, NRM, GEO> &f)
 {
     const float4 *const end2 = s + 3 * (cnt & ~1);
 #pragma unroll 1
     for (; s != end2; s += 6) {
-        fwd_blend_hit<CONTRIB, NRM, GEO>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co, ns, N, gp);
-        fwd_blend_hit<CONTRIB, NRM, GEO>(s + 3, fpx, fpy, p, CONTRIB ? gids[1] : 0u, co, NRM ? ns + 1 : ns, N, gp);
+        fwd_blend_hit(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, ns, N, gp, f);
+        fwd_blend_hit(s + 3, fpx, fpy, p, CONTRIB ? gids[1] : 0u, NRM ? ns + 1 : ns, N, gp, f);
         if (CONTRIB) gids += 2;
         if (NRM) ns += 2;
     }
-    if (cnt & 1) fwd_blend_hit<CONTRIB, NRM, GEO>(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, co, ns, N, gp);
+    if (cnt & 1) fwd_blend_hit(s, fpx, fpy, p, CONTRIB ? gids[0] : 0u, ns, N, gp, f);
 }
 
 // Writes the pixel's outputs (out-of-image pixels write nothing).
@@ -220,19 +234,20 @@ __device__ __forceinline__ void fwd_store_pixel(const BlendArgs &a, int v, int p
     a.out_alpha[v * HW + pix] = p.Aa;
 }
 
-#if !FWD_BULK
-// The body of the F6 kernels.  CONTRIB (contribution scores, DESIGN.md section 2): compaction also writes each hit's Gaussian
-// index (record index - v*P) into the warp's 32-word gids array, and every hit is folded into co; everything else is the
+// The body of the F6 kernel.  CONTRIB (contribution scores, DESIGN.md section 2): compaction also writes each hit's Gaussian
+// index (record index - v*P) into the warp's 32-word gid_slabs row, and every hit is folded into f.co; everything else is the
 // same code.
 // NRM (normal maps, DESIGN.md section 2): hit lanes also gather gauss_normals[record index] into the warp's 32-entry nrm_slabs
 // row, the pixel keeps three normal sums, and the pixel writes them to out_normal [V,3,H,W].
 // GEO (geometry outputs, DESIGN.md section 2): the pixel keeps M2 and the median (GeoPixel) and writes them to geo's images and
 // median_pos.
-template <bool CONTRIB, bool NRM = false, bool GEO = false>
-__device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gid_slabs)[32], const ContribOut &co,
-                                               float4 (*nrm_slabs)[32] = nullptr, const float4 *gauss_normals = nullptr,
-                                               float *out_normal = nullptr, const GeoFwd *geo = nullptr)
+// A feature's shared arrays are declared in every instantiation; one that never touches them allocates no shared memory for
+// them.
+template <bool CONTRIB, bool NRM, bool GEO>
+__device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, const FwdFeatures<CONTRIB, NRM, GEO> &f)
 {
+    __shared__ uint32_t gid_slabs[WARPS_PER_CTA][32]; // CONTRIB
+    __shared__ float4 nrm_slabs[WARPS_PER_CTA][32];   // NRM
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
 
     const int ntiles = a.grid_x * a.grid_y;
@@ -279,7 +294,7 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
         if (hit) {
             g1 = __ldg(recs4 + 3 * (size_t)id_c + 1);
             g2 = __ldg(recs4 + 3 * (size_t)id_c + 2);
-            if (NRM) gn = __ldg(gauss_normals + id_c);
+            if constexpr (NRM) gn = __ldg(f.gauss_normals + id_c);
         }
         const float4 g0_h = g0_c;
         const uint32_t id_h = id_c;
@@ -295,12 +310,11 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
                 s[1] = make_float4(fmul(-0.5f, g1.x), -g1.y, fmul(-0.5f, g1.z), g1.w);
                 s[2] = g2;
                 if (CONTRIB) gid_slabs[warp][__popc(b & lt)] = id_h - (uint32_t)v * (uint32_t)a.P;
-                if (NRM) nrm_slabs[warp][__popc(b & lt)] = gn;
+                if constexpr (NRM) nrm_slabs[warp][__popc(b & lt)] = gn;
             }
             __syncwarp();
             p.used = 0u;
-            fwd_blend_slab<CONTRIB, NRM, GEO>(slab, __popc(b), fpx, fpy, p, CONTRIB ? gid_slabs[warp] : nullptr, co,
-                                              NRM ? nrm_slabs[warp] : nullptr, N, &gp);
+            fwd_blend_slab(slab, __popc(b), fpx, fpy, p, gid_slabs[warp], nrm_slabs[warp], N, gp, f);
             m = __reduce_or_sync(FULL, p.used);
             __syncwarp();
         }
@@ -308,238 +322,57 @@ __device__ __forceinline__ void blend_fwd_body(const BlendArgs &a, uint32_t (*gi
     }
     if (inside) {
         fwd_store_pixel(a, v, px, py, p);
-        if (NRM) {
+        if constexpr (NRM) {
             const size_t HW = (size_t)a.H * a.W, pix = (size_t)py * a.W + px;
-            float *on = out_normal + (size_t)v * 3 * HW + pix;
+            float *on = f.out_normal + (size_t)v * 3 * HW + pix;
             on[0] = N[0]; on[HW] = N[1]; on[2 * HW] = N[2];
         }
-        if (GEO) {
+        if constexpr (GEO) {
             const size_t i = (size_t)v * a.H * a.W + (size_t)py * a.W + px;
-            geo->out_median[i] = gp.med;
-            geo->out_depth2[i] = gp.M2;
-            geo->median_pos[i] = gp.mpos;
+            f.geo.out_median[i] = gp.med;
+            f.geo.out_depth2[i] = gp.M2;
+            f.geo.median_pos[i] = gp.mpos;
         }
     }
 }
 
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_kernel(BlendArgs a)
+// F6.  The body stays a function of its own, inlined here: the compiler then optimises it before it reaches the kernel, which
+// keeps ptxas's register assignment of the feature instantiations as DESIGN.md section 5 lists them (written as the kernel
+// itself, the NRM and GEO instantiations come out with some registers renamed).
+template <bool CONTRIB, bool NRM, bool GEO>
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, CONTRIB || NRM || GEO ? FWD_FEATURE_MIN_BLOCKS : FWD_MIN_BLOCKS)
+    blend_fwd_kernel(BlendArgs a, FwdFeatures<CONTRIB, NRM, GEO> f)
 {
-    blend_fwd_body<false>(a, nullptr, ContribOut{});
+    blend_fwd_body(a, f);
 }
 
-// F6 with the contribution scores.  At F6's cap of 56 registers it spills 8 bytes in the hit loop; 16 blocks (64 registers,
-// 32 warps/SM, the backward's occupancy) removes the spill (DESIGN.md section 5)
-#ifndef FWD_CONTRIB_MIN_BLOCKS
-#define FWD_CONTRIB_MIN_BLOCKS 16
-#endif
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_CONTRIB_MIN_BLOCKS) blend_fwd_contrib_kernel(BlendArgs a, ContribOut co)
-{
-    __shared__ uint32_t gids[WARPS_PER_CTA][32];
-    blend_fwd_body<true>(a, gids, co);
-}
-
-// F6 with the normal image (DESIGN.md section 5 lists its registers at this bound)
-#ifndef FWD_NRM_MIN_BLOCKS
-#define FWD_NRM_MIN_BLOCKS 16
-#endif
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_NRM_MIN_BLOCKS) blend_fwd_nrm_kernel(BlendArgs a, const float4 *gauss_normals,
-                                                                                             float *out_normal)
-{
-    __shared__ float4 nrm[WARPS_PER_CTA][32];
-    blend_fwd_body<false, true>(a, nullptr, ContribOut{}, nrm, gauss_normals, out_normal);
-}
-
-// F6 with the geometry outputs, without and with the normal image (DESIGN.md section 5 lists their registers at this bound)
-#ifndef FWD_GEO_MIN_BLOCKS
-#define FWD_GEO_MIN_BLOCKS 16
-#endif
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_GEO_MIN_BLOCKS) blend_fwd_geo_kernel(BlendArgs a, GeoFwd g)
-{
-    blend_fwd_body<false, false, true>(a, nullptr, ContribOut{}, nullptr, nullptr, nullptr, &g);
-}
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_GEO_MIN_BLOCKS) blend_fwd_nrm_geo_kernel(BlendArgs a, const float4 *gauss_normals,
-                                                                                                 float *out_normal, GeoFwd g)
-{
-    __shared__ float4 nrm[WARPS_PER_CTA][32];
-    blend_fwd_body<false, true, true>(a, nullptr, ContribOut{}, nrm, gauss_normals, out_normal, &g);
-}
-
-#endif // !FWD_BULK
-
-#if FWD_BULK
-// ------------------------------------------------------------------------------------------------
-// F6, bulk-copy variant (A/B experiment of round 2; DESIGN.md "Bulk-copy staging"): the tile's id run -- the one contiguous
-// stream of the blend -- is brought into shared memory by the async proxy (cp.async.bulk + mbarrier complete_tx, two 1 KB
-// stages per warp) instead of per-lane LDG prefetches; the 48-byte records are still gathered by id (they are scattered in
-// HBM: a bulk copy moves contiguous bytes only).  Chunks are aligned to the absolute 32-entry grid of point_list so that a
-// chunk never straddles two stages and every bulk copy starts on a 16-byte boundary; results are identical, and the
-// contributor masks are re-cut to the list-relative chunk grid the backward reads.
-// ------------------------------------------------------------------------------------------------
-#define BULK_CHUNKS 8                    // chunks (of 32 ids) per stage
-#define BULK_IDS (32 * BULK_CHUNKS)      // 256 ids = 1 KB per stage
-struct __align__(16) BulkStage {
-    uint32_t ids[2][BULK_IDS];
-    unsigned long long mbar[2];
-};
-__device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long *b, int count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(b)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t bytes, unsigned long long *b)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(b)), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(b)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long *b, uint32_t parity)
-{
-    uint32_t done = 0;
-    int spins = 0;
-    while (!done) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(smem_addr(b)), "r"(parity) : "memory");
-        if (!done && ++spins > (1 << 24)) __trap(); // a protocol error must fail loudly, never hang the GPU
-    }
-}
-
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, FWD_MIN_BLOCKS) blend_fwd_kernel(BlendArgs a)
-{
-    __shared__ WarpSlab slabs[WARPS_PER_CTA];
-    __shared__ BulkStage bulk[WARPS_PER_CTA];
-
-    const int ntiles = a.grid_x * a.grid_y;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t vt = a.tile_order[blockIdx.x / CTAS_PER_TILE];
-    const int v = (int)(vt / (uint32_t)ntiles), tile = (int)(vt % (uint32_t)ntiles);
-    const int patch = (blockIdx.x % CTAS_PER_TILE) * WARPS_PER_CTA + warp;
-    const int tile_x = tile % a.grid_x, tile_y = tile / a.grid_x;
-    const int x0 = tile_x * GS_TILE + (patch & 1) * 8, y0 = tile_y * GS_TILE + (patch >> 1) * 4;
-    const int px = x0 + (lane & 7), py = y0 + (lane >> 3);
-    const bool inside = px < a.W && py < a.H;
-    const float fpx = (float)px, fpy = (float)py, fx0 = (float)x0, fy0 = (float)y0;
-    WarpSlab &sl = slabs[warp];
-    BulkStage &bk = bulk[warp];
-
-    const uint2 range = a.ranges[(size_t)v * ntiles + tile];
-    const float4 *recs4 = reinterpret_cast<const float4 *>(a.recs);
-    const uint32_t lt = (1u << lane) - 1u;
-    // absolute chunk grid: chunk c covers point_list[a0 + 32 c + lane]
-    const uint32_t a0 = range.x & ~31u;
-    const int n_chunks = range.y > range.x ? (int)((range.y - a0 + 31u) >> 5) : 0;
-    const int n_stages = (n_chunks + BULK_CHUNKS - 1) / BULK_CHUNKS;
-    // contributor masks on the list-relative grid (as the main variant writes them): with r = range.x & 31, relative chunk k
-    // holds the entries r.. of absolute chunk k and the entries ..r-1 of absolute chunk k+1
-    uint32_t *const cmask = a.cmask + ((size_t)(range.x >> 5) + vt) * 8 + patch;
-    const uint32_t r = range.x & 31u;
-    const int n_rel = (int)((range.y - range.x + 31u) >> 5);
-    uint32_t carry = 0; // relative word c-1, its bits from absolute chunk c-1
-
-    FwdPixel p = {inside ? 1.0f : 0.0f, 0.f, 0.f, 0.f, 0.f, 0.f, 0u, 0u};
-
-    if (lane == 0) { mbar_init(&bk.mbar[0], 1); mbar_init(&bk.mbar[1], 1); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncwarp();
-    // stage s -> buffer s & 1, its (s >> 1)-th use: wait parity (s >> 1) & 1.  Bytes: whole stage, clipped to the 16-byte
-    // rounded end of the tile's run (inside the point_list allocation: its capacity is rounded up to 256 bytes).
-    auto issue = [&](int s) {
-        const uint32_t first = a0 + (uint32_t)s * BULK_IDS;
-        const uint32_t end = min(first + (uint32_t)BULK_IDS, (range.y + 3u) & ~3u);
-        bulk_load(bk.ids[s & 1], a.point_list + first, (end - first) * 4u, &bk.mbar[s & 1]);
-    };
-    int issued = 0, waited = 0; // stages issued / stages whose arrival has been observed (warp-uniform)
-    if (lane == 0) { if (n_stages > 0) issue(0); if (n_stages > 1) issue(1); }
-    issued = min(n_stages, 2);
-
-    uint32_t id_c = 0;
-    float4 g0_c = make_float4(0.f, 0.f, -1.f, -1.f);
-    bool valid_c = false;
-    if (n_chunks > 0) {
-        mbar_wait(&bk.mbar[0], 0);
-        waited = 1;
-        const uint32_t ab = a0 + lane;
-        valid_c = ab >= range.x && ab < range.y;
-        if (valid_c) { id_c = bk.ids[0][lane]; g0_c = __ldg(recs4 + 3 * (size_t)id_c); }
-    }
-    int c = 0;
-    for (; c < n_chunks; c++) {
-        // as in the main variant: the relative chunks the backward reads all end before this exit
-        if (__all_sync(FULL, !(p.T > 0.0f))) break;
-        const bool hit = box_hits_patch(g0_c, fx0, fy0, fx0 + 7.0f, fy0 + 3.0f);
-        const uint32_t b = __ballot_sync(FULL, hit);
-        float4 g1, g2;
-        if (hit) {
-            g1 = __ldg(recs4 + 3 * (size_t)id_c + 1);
-            g2 = __ldg(recs4 + 3 * (size_t)id_c + 2);
-        }
-        const float4 g0_h = g0_c;
-        const uint32_t pos_h = a0 + 32u * (uint32_t)c + lane - range.x + 1u; // 1-based list position
-        // next chunk: ids from the stage in shared memory (wait for it when the chunk opens a new stage), records by gather
-        g0_c = make_float4(0.f, 0.f, -1.f, -1.f);
-        if (c + 1 < n_chunks) {
-            const int sn = (c + 1) / BULK_CHUNKS;
-            if (sn == waited) { mbar_wait(&bk.mbar[sn & 1], (uint32_t)(sn >> 1) & 1u); waited = sn + 1; }
-            const uint32_t ab = a0 + 32u * (uint32_t)(c + 1) + lane;
-            if (ab >= range.x && ab < range.y) {
-                id_c = bk.ids[sn & 1][((c + 1) % BULK_CHUNKS) * 32 + lane];
-                g0_c = __ldg(recs4 + 3 * (size_t)id_c);
-            }
-            // the stage before `sn` was last read one iteration ago (the ballot above ordered those reads): refill its buffer
-            if ((c + 1) % BULK_CHUNKS == 0 && sn + 1 < n_stages && sn + 1 == issued) {
-                if (lane == 0) issue(sn + 1);
-                issued = sn + 2;
-            }
-        }
-        uint32_t m = 0u; // mask of this absolute chunk
-        if (b != 0u) {
-            if (hit) {
-                const int slot = __popc(b & lt);
-                sl.rec[3 * slot] = make_float4(g0_h.x, g0_h.y, __uint_as_float(pos_h), __uint_as_float(1u << lane));
-                sl.rec[3 * slot + 1] = make_float4(fmul(-0.5f, g1.x), -g1.y, fmul(-0.5f, g1.z), g1.w);
-                sl.rec[3 * slot + 2] = g2;
-            }
-            __syncwarp();
-            p.used = 0u;
-            fwd_blend_slab<false>(sl.rec, __popc(b), fpx, fpy, p, nullptr, ContribOut{});
-            m = __reduce_or_sync(FULL, p.used);
-            __syncwarp();
-        }
-        // bits below r complete relative chunk c-1; bits from r up start relative chunk c
-        const uint64_t sh = (uint64_t)m << (32u - r);
-        if (c >= 1 && lane == 0) cmask[(size_t)(c - 1) * 8] = carry | (uint32_t)sh;
-        carry = (uint32_t)(sh >> 32);
-    }
-    // relative chunk c-1: its entries from absolute chunk c (if any) were never processed, so they did not contribute
-    if (c >= 1 && c - 1 < n_rel && lane == 0) cmask[(size_t)(c - 1) * 8] = carry;
-    // a bulk copy still in flight targets this CTA's shared memory: observe every issued stage before the warp may exit
-    for (int s = waited; s < issued; s++) mbar_wait(&bk.mbar[s & 1], (uint32_t)(s >> 1) & 1u);
-    if (inside) fwd_store_pixel(a, v, px, py, p);
-}
-#endif // FWD_BULK
-
-#if !FWD_BULK
 int blend_caps()
 {
     return BLEND_CAP_CONTRIB | BLEND_CAP_NORMALS | BLEND_CAP_GEOMETRY | BLEND_CAP_ABSGRAD | BLEND_CAP_DETERMINISTIC;
 }
-#else
-// the contribution, normal and geometry variants exist for the default kernel only (the normals' and geometry's backward
-// kernels are then not launched either)
-int blend_caps() { return BLEND_CAP_ABSGRAD | BLEND_CAP_DETERMINISTIC; }
-#endif
+
+// Calls k(std::true_type{}) or k(std::false_type{}) as f is set: the launchers turn each option bit into a template argument
+// with it, so the instantiation an option set selects is spelled in one place.
+template <class K> static void with_flag(bool f, K &&k)
+{
+    if (f) k(std::true_type{});
+    else k(std::false_type{});
+}
 
 void launch_blend_fwd(const BlendArgs &a, const ContribOut *co, const float4 *gauss_normals, float *out_normal, const GeoFwd *g,
                       cudaStream_t st)
 {
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-#if !FWD_BULK
-    if (co) blend_fwd_contrib_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *co);
-    else if (g && gauss_normals) blend_fwd_nrm_geo_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal, *g);
-    else if (g) blend_fwd_geo_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *g);
-    else if (gauss_normals) blend_fwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, gauss_normals, out_normal);
-    else
-#endif
-        blend_fwd_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
+    auto launch = [&](auto C, auto N, auto G) {
+        FwdFeatures<C, N, G> f;
+        if constexpr (C) f.co = *co;
+        if constexpr (N) { f.gauss_normals = gauss_normals; f.out_normal = out_normal; }
+        if constexpr (G) f.geo = *g;
+        blend_fwd_kernel<C, N, G><<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, f);
+    };
+    // contribution scores never come with normals or geometry (read_opts refuses the combination)
+    if (co) launch(std::true_type{}, std::false_type{}, std::false_type{});
+    else with_flag(gauss_normals, [&](auto N) { with_flag(g, [&](auto G) { launch(std::false_type{}, N, G); }); });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -566,6 +399,16 @@ __device__ __forceinline__ void red_add_v2(float *p, float a, float b)
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
+// The backward's feature arguments, laid out as FwdFeatures: the deterministic flush's slots, normals, geometry gradients.
+// ABS has no argument of its own.
+template <bool> struct BwdDetArg {};
+template <> struct BwdDetArg<true> { DetFlush det; };
+template <bool> struct BwdNrmArg {};
+template <> struct BwdNrmArg<true> { NrmBwd nrm; };
+template <bool> struct BwdGeoArg {};
+template <> struct BwdGeoArg<true> { GeoBwd geo; };
+template <bool DET, bool NRM, bool GEO> struct BwdFeatures : BwdDetArg<DET>, BwdNrmArg<NRM>, BwdGeoArg<GEO> {};
+
 // Sums the first n park slots into ScreenGrad.  Lane l takes slot h = l % BWD_PARK over the pixels
 // [BWD_PARK*part, BWD_PARK*part + BWD_PARK), part = l / BWD_PARK: BWD_PARK / 8 rows of the 8x4 patch.  Within a row dy is
 // constant, so the row accumulates sum q, sum q*dx, sum q*dx^2 and folds dy in once per row; dx and dy are the hit loop's
@@ -581,16 +424,16 @@ __device__ __forceinline__ void red_add_v2(float *p, float a, float b)
 // load); B dy and C dy are folded once per row.  They go to ScreenGrad's padding (the third RED becomes a v4), or in
 // deterministic mode to the partial's own float2 of det.abs_partials.  The ten sums are formed exactly as without ABS.
 // NRM (normal maps, DESIGN.md section 2): the flush also sums Wn = sum w * dL/dN over the slot's pixels, dL/dN from the
-// warp's second pixel table npix (laid out as pk.pix).  Atomic mode adds (Wn, 0) to nb.wn[record] with one more v4 RED;
-// deterministic mode stores it to nb.partials[slot].  Everything else is formed exactly as without NRM.
+// warp's second pixel table npix (laid out as pk.pix).  Atomic mode adds (Wn, 0) to nrm.wn[record] with one more v4 RED;
+// deterministic mode stores it to nrm.partials[slot].  Everything else is formed exactly as without NRM.
 // GEO (geometry outputs, DESIGN.md section 2): the flush also sums Wm = sum w * dL/dM2 and Md = the dL/dmedian of the slot's
 // median pixels (the hit loop's ballot gmed[h], bit p = pixel p), both from the warp's pixel table gpix (laid out as pk.pix),
 // and each part adds 2d * Wm + Md to its W3 before the exchange, d the record's depth (word 11, an L1 hit as the conic is).
 // The depth gradient then reaches the mean through B2's existing depth term; everything else is formed exactly as without GEO.
-template <bool DET, bool ABS, bool NRM = false, bool GEO = false>
+template <bool ABS, bool DET, bool NRM, bool GEO>
 __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, float fx0, float fy_part, float *sgrad,
-                                           const BlendBwdArgs &a, const DetFlush &det, const float4 *npix = nullptr,
-                                           const NrmBwd *nb = nullptr, const float2 *gpix = nullptr, const uint32_t *gmed = nullptr)
+                                           const BlendBwdArgs &a, const BwdFeatures<DET, NRM, GEO> &f, const float4 *npix,
+                                           const float2 *gpix, const uint32_t *gmed)
 {
     __syncwarp();
     const int h = lane % BWD_PARK, part = lane / BWD_PARK;
@@ -657,21 +500,23 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
         if (ABS) { Ax += __shfl_xor_sync(FULL, Ax, o); Ay += __shfl_xor_sync(FULL, Ay, o); }
         if (NRM) { N0 += __shfl_xor_sync(FULL, N0, o); N1 += __shfl_xor_sync(FULL, N1, o); N2 += __shfl_xor_sync(FULL, N2, o); }
     }
-    if (DET) {
+    if constexpr (DET) {
         if (h < n) {
             // partial as S0, Sx | Sy, Sxx | Sxy, Syy | w.gC0, w.gC1 | w.gC2, w.gD: 40 bytes, 8-byte aligned
             const uint32_t range_x = __ldg(&a.ranges[__ldg(a.tile_order + blockIdx.x / CTAS_PER_TILE)].x);
             const int patch = (blockIdx.x % CTAS_PER_TILE) * WARPS_PER_CTA + (threadIdx.x >> 5);
             const uint32_t j = range_x + __float_as_uint(s.z);
-            const uint32_t slot = __ldg(det.base + j) - (uint32_t)__popc((uint32_t)__ldg(det.pm + j) >> patch);
-            float2 *rec = reinterpret_cast<float2 *>(det.partials + (size_t)slot * DET_PARTIAL_FLOATS);
+            const uint32_t slot = __ldg(f.det.base + j) - (uint32_t)__popc((uint32_t)__ldg(f.det.pm + j) >> patch);
+            float2 *rec = reinterpret_cast<float2 *>(f.det.partials + (size_t)slot * DET_PARTIAL_FLOATS);
             if (part == 0) { rec[0] = make_float2(S0, Sx); rec[1] = make_float2(Sy, Sxx); }
             if (part == 1) { rec[2] = make_float2(Sxy, Syy); rec[3] = make_float2(W0, W1); }
             if (part == (PARK_LANES > 2 ? 2 : 0)) {
                 rec[4] = make_float2(W2, W3);
-                if (ABS) det.abs_partials[slot] = make_float2(Ax, Ay);
+                if (ABS) f.det.abs_partials[slot] = make_float2(Ax, Ay);
             }
-            if (NRM && part == 1) nb->partials[slot] = make_float4(N0, N1, N2, 0.f);
+            if constexpr (NRM) {
+                if (part == 1) f.nrm.partials[slot] = make_float4(N0, N1, N2, 0.f);
+            }
         }
     } else if (h < n) {
         // ScreenGrad as moments: S0, Sx, Sy, Sxx | Sxy, Syy, w.gC0, w.gC1 | w.gC2, w.gD (| Ax, Ay in the padding with ABS)
@@ -684,23 +529,28 @@ __device__ __forceinline__ void park_flush(const WarpPark &pk, int n, int lane, 
             if (ABS) red_add_v4(rec + 8, W2, W3, Ax, Ay);
             else red_add_v2(rec + 8, W2, W3);
         }
-        if (NRM && part == 1) red_add_v4(reinterpret_cast<float *>(nb->wn + __float_as_uint(s.w)), N0, N1, N2, 0.f);
+        if constexpr (NRM) {
+            if (part == 1) red_add_v4(reinterpret_cast<float *>(f.nrm.wn + __float_as_uint(s.w)), N0, N1, N2, 0.f);
+        }
     }
     __syncwarp();
 }
 
-// The body of the B1 kernels: DET selects the flush (vector REDs into ScreenGrad, or stores of per-(instance, patch)
-// partials), ABS adds the absolute sums to it; everything else is the same code.
+// B1: DET selects the flush (vector REDs into ScreenGrad, or stores of per-(instance, patch) partials
+// into their slots of f.det), ABS adds the absolute sums to it; everything else is the same code.
 // NRM (normal maps): contributing lanes also stage gauss_normals[record] in the warp's nslab row, the pixel's dL/dN goes to
 // the second pixel table npix, cg gains n . dL/dN, and the flush sums Wn (park_flush).
-// GEO (geometry outputs): the pixel's (dL/dM2, dL/dmedian) go to the pixel table gpixs, cg gains d^2 * dL/dM2, every parked hit
-// ballots the lanes whose median it is into gmeds[slot], and the flush folds both depth terms into W3 (park_flush).
-template <bool DET, bool ABS, bool NRM = false, bool GEO = false>
-__device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetFlush &det, float4 (*nslabs)[32] = nullptr,
-                                               float4 (*npixs)[32 + PARK_LANES] = nullptr, const NrmBwd *nb = nullptr,
-                                               float2 (*gpixs)[32 + PARK_LANES] = nullptr, uint32_t (*gmeds)[BWD_PARK] = nullptr,
-                                               const GeoBwd *gb = nullptr)
+// GEO (geometry outputs): the pixel's (dL/dM2, dL/dmedian) go to the pixel table gpix, cg gains d^2 * dL/dM2, every parked hit
+// ballots the lanes whose median it is into gmed[slot], and the flush folds both depth terms into W3 (park_flush).
+// A feature's shared arrays are declared in every instantiation; one that never touches them allocates no shared memory for
+// them.
+template <bool DET, bool ABS, bool NRM, bool GEO>
+__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_kernel(BlendBwdArgs a, BwdFeatures<DET, NRM, GEO> f)
 {
+    __shared__ float2 gpix[WARPS_PER_CTA][32 + PARK_LANES]; // GEO
+    __shared__ uint32_t gmed[WARPS_PER_CTA][BWD_PARK];      // GEO
+    __shared__ float4 nslab[WARPS_PER_CTA][32];             // NRM
+    __shared__ float4 npix[WARPS_PER_CTA][32 + PARK_LANES]; // NRM
     __shared__ WarpSlab slabs[WARPS_PER_CTA];
     __shared__ WarpPark parks[WARPS_PER_CTA];
 
@@ -740,14 +590,14 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
         }
         if (a.dL_ddepth) gD = a.dL_ddepth[v * HW + pix];
         if (a.dL_dalpha) gA = a.dL_dalpha[v * HW + pix];
-        if (NRM) {
-            const float *g = nb->dL_dnormal + (size_t)v * 3 * HW;
+        if constexpr (NRM) {
+            const float *g = f.nrm.dL_dnormal + (size_t)v * 3 * HW;
             gN = make_float4(g[pix], g[HW + pix], g[2 * HW + pix], 0.f);
         }
-        if (GEO) {
-            if (gb->dL_ddepth2) gM2 = gb->dL_ddepth2[v * HW + pix];
-            if (gb->dL_dmedian) gMed = gb->dL_dmedian[v * HW + pix];
-            mpos = gb->median_pos[v * HW + pix];
+        if constexpr (GEO) {
+            if (f.geo.dL_ddepth2) gM2 = f.geo.dL_ddepth2[v * HW + pix];
+            if (f.geo.dL_dmedian) gMed = f.geo.dL_dmedian[v * HW + pix];
+            mpos = f.geo.median_pos[v * HW + pix];
         }
     }
     int wmax = last; // list positions at or beyond the patch's largest n_contrib cannot contribute here
@@ -760,8 +610,8 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
 
     const float bg_dot = a.bg[0] * gC0 + a.bg[1] * gC1 + a.bg[2] * gC2;
     pk.pix[lane + lane / BWD_PARK] = make_float4(gC0, gC1, gC2, gD); // read by the flushes, after their __syncwarp
-    if (NRM) npixs[warp][lane + lane / BWD_PARK] = gN;
-    if (GEO) gpixs[warp][lane + lane / BWD_PARK] = make_float2(gM2, gMed);
+    if (NRM) npix[warp][lane + lane / BWD_PARK] = gN;
+    if (GEO) gpix[warp][lane + lane / BWD_PARK] = make_float2(gM2, gMed);
     int np = 0;                                                      // park slots in use (warp-uniform)
     const float fx0 = (float)x0, fy_part = (float)(y0 + (lane / BWD_PARK) * (BWD_PARK / 8)); // the flush lane's first row
     float *const sgrad = reinterpret_cast<float *>(a.sgrad);
@@ -797,13 +647,13 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
             sl.rec[3 * s] = make_float4(g0.x, g0.y, __uint_as_float((uint32_t)(32 * c + 31 - lane)), __uint_as_float(id_h));
             sl.rec[3 * s + 1] = make_float4(fmul(-0.5f, g1.x), -g1.y, fmul(-0.5f, g1.z), g1.w);
             sl.rec[3 * s + 2] = g2;
-            if (NRM) nslabs[warp][s] = __ldg(nb->gauss_normals + id_h);
+            if constexpr (NRM) nslab[warp][s] = __ldg(f.nrm.gauss_normals + id_h);
         }
         __syncwarp();
         // The chunk's hits in runs that end at the next flush: one counter (np, the park slot) per hit, and the slab, park
         // and slot-table addresses advance as running pointers.
         const float4 *s = sl.rec;
-        const float4 *ns = NRM ? nslabs[warp] : nullptr;
+        const float4 *ns = nslab[warp];
         for (int left = __popc(mr); left > 0;) {
             const int run = min(left, BWD_PARK - np);
             left -= run;
@@ -848,118 +698,30 @@ __device__ __forceinline__ void blend_bwd_body(const BlendBwdArgs &a, const DetF
                 if (lane == 0) pk.hit[np] = g0;
                 if (GEO) { // the lanes whose median this hit is (pos is 0-based, mpos 1-based)
                     const uint32_t mb = __ballot_sync(FULL, contrib & ((uint32_t)pos + 1u == mpos));
-                    if (lane == 0) gmeds[warp][np] = mb;
+                    if (lane == 0) gmed[warp][np] = mb;
                 }
             }
             if (np == BWD_PARK) {
-                park_flush<DET, ABS, NRM, GEO>(pk, np, lane, fx0, fy_part, sgrad, a, det, NRM ? npixs[warp] : nullptr, nb,
-                                               GEO ? gpixs[warp] : nullptr, GEO ? gmeds[warp] : nullptr);
+                park_flush<ABS>(pk, np, lane, fx0, fy_part, sgrad, a, f, npix[warp], gpix[warp], gmed[warp]);
                 np = 0;
             }
         }
         __syncwarp();
     }
     if (np > 0)
-        park_flush<DET, ABS, NRM, GEO>(pk, np, lane, fx0, fy_part, sgrad, a, det, NRM ? npixs[warp] : nullptr, nb,
-                                       GEO ? gpixs[warp] : nullptr, GEO ? gmeds[warp] : nullptr);
-}
-
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_kernel(BlendBwdArgs a)
-{
-    blend_bwd_body<false, false>(a, DetFlush{});
-}
-
-// B1 of the deterministic backward: a.sgrad is not touched; every flushed (instance, patch) partial goes to its own slot
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_kernel(BlendBwdArgs a, DetFlush det)
-{
-    blend_bwd_body<true, false>(a, det);
-}
-
-// B1 with the absolute screen-space sums (Ax, Ay in ScreenGrad's padding)
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_abs_kernel(BlendBwdArgs a)
-{
-    blend_bwd_body<false, true>(a, DetFlush{});
-}
-
-// deterministic B1 with the absolute sums: (Ax, Ay) of partial `slot` go to det.abs_partials[slot]
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_abs_kernel(BlendBwdArgs a, DetFlush det)
-{
-    blend_bwd_body<true, true>(a, det);
-}
-
-// B1 with the normal term (NRM): atomic / deterministic, without and with the absolute sums.  Each stages the normals and
-// dL/dN in two more per-warp shared arrays.
-#define BWD_NRM_SHARED                                  \
-    __shared__ float4 nslab[WARPS_PER_CTA][32];         \
-    __shared__ float4 npix[WARPS_PER_CTA][32 + PARK_LANES]
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_nrm_kernel(BlendBwdArgs a, NrmBwd nb)
-{
-    BWD_NRM_SHARED;
-    blend_bwd_body<false, false, true>(a, DetFlush{}, nslab, npix, &nb);
-}
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_nrm_abs_kernel(BlendBwdArgs a, NrmBwd nb)
-{
-    BWD_NRM_SHARED;
-    blend_bwd_body<false, true, true>(a, DetFlush{}, nslab, npix, &nb);
-}
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_nrm_kernel(BlendBwdArgs a, DetFlush det, NrmBwd nb)
-{
-    BWD_NRM_SHARED;
-    blend_bwd_body<true, false, true>(a, det, nslab, npix, &nb);
-}
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_det_nrm_abs_kernel(BlendBwdArgs a, DetFlush det,
-                                                                                                  NrmBwd nb)
-{
-    BWD_NRM_SHARED;
-    blend_bwd_body<true, true, true>(a, det, nslab, npix, &nb);
-}
-
-// B1 with the geometry gradients (GEO): atomic / deterministic x absgrad off / on x normals off / on.  Each stages the pixels'
-// (dL/dM2, dL/dmedian) and the slots' median ballots in two more per-warp shared arrays (and the NRM forms the normals' two).
-template <bool DET, bool ABS, bool NRM>
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, BWD_MIN_BLOCKS) blend_bwd_geo_kernel(BlendBwdArgs a, DetFlush det, NrmBwd nb,
-                                                                                          GeoBwd gb)
-{
-    __shared__ float2 gpix[WARPS_PER_CTA][32 + PARK_LANES];
-    __shared__ uint32_t gmed[WARPS_PER_CTA][BWD_PARK];
-    if (NRM) {
-        BWD_NRM_SHARED;
-        blend_bwd_body<DET, ABS, true, true>(a, det, nslab, npix, &nb, gpix, gmed, &gb);
-    } else {
-        blend_bwd_body<DET, ABS, false, true>(a, det, nullptr, nullptr, nullptr, gpix, gmed, &gb);
-    }
+        park_flush<ABS>(pk, np, lane, fx0, fy_part, sgrad, a, f, npix[warp], gpix[warp], gmed[warp]);
 }
 
 void launch_blend_bwd(const BlendBwdArgs &a, const DetFlush *det, bool absgrad, const NrmBwd *n, const GeoBwd *g, cudaStream_t st)
 {
     const unsigned grid = (unsigned)(a.grid_x * a.grid_y * CTAS_PER_TILE * a.V);
-    if (g) {
-        const DetFlush d = det ? *det : DetFlush{};
-        const NrmBwd nb = n ? *n : NrmBwd{};
-        void (*k)(BlendBwdArgs, DetFlush, NrmBwd, GeoBwd);
-        if (det) {
-            if (n) k = absgrad ? blend_bwd_geo_kernel<true, true, true> : blend_bwd_geo_kernel<true, false, true>;
-            else k = absgrad ? blend_bwd_geo_kernel<true, true, false> : blend_bwd_geo_kernel<true, false, false>;
-        } else {
-            if (n) k = absgrad ? blend_bwd_geo_kernel<false, true, true> : blend_bwd_geo_kernel<false, false, true>;
-            else k = absgrad ? blend_bwd_geo_kernel<false, true, false> : blend_bwd_geo_kernel<false, false, false>;
-        }
-        k<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, d, nb, *g);
-    } else if (n) {
-        if (det) {
-            if (absgrad) blend_bwd_det_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det, *n);
-            else blend_bwd_det_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det, *n);
-        } else {
-            if (absgrad) blend_bwd_nrm_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *n);
-            else blend_bwd_nrm_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *n);
-        }
-    } else if (det) {
-        if (absgrad) blend_bwd_det_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det);
-        else blend_bwd_det_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, *det);
-    } else {
-        if (absgrad) blend_bwd_abs_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
-        else blend_bwd_kernel<<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a);
-    }
+    with_flag(det, [&](auto D) { with_flag(absgrad, [&](auto A) { with_flag(n, [&](auto N) { with_flag(g, [&](auto G) {
+        BwdFeatures<D, N, G> f;
+        if constexpr (D) f.det = *det;
+        if constexpr (N) f.nrm = *n;
+        if constexpr (G) f.geo = *g;
+        blend_bwd_kernel<D, A, N, G><<<grid, 32 * WARPS_PER_CTA, 0, st>>>(a, f);
+    }); }); }); });
 }
 
 // dL_dmeans2D_abs of every (view, Gaussian): the padding sums (Ax, Ay) times o * W/2 and o * H/2, o the record's opacity --

@@ -104,8 +104,8 @@ int launch_test_sort32(uint32_t *ka, uint32_t *kb, uint32_t *va, uint32_t *vb, i
                        int *result_in_b, cudaStream_t st);
 size_t test_sort32_scratch_bytes(int64_t n);
 
-// the optional features of the blend a build implements (blend_caps): all in blend.cu; the bulk-copy build lacks the
-// forward's CONTRIB, NORMALS and GEOMETRY; the classic comparator has none.  The host checks them before any launch.
+// the optional features of the blend a build implements (blend_caps): all in blend.cu; the classic comparator has none.  The
+// host checks them before any launch.
 enum { BLEND_CAP_CONTRIB = 1, BLEND_CAP_NORMALS = 2, BLEND_CAP_GEOMETRY = 4, BLEND_CAP_ABSGRAD = 8,
        BLEND_CAP_DETERMINISTIC = 16 };
 int blend_caps();

@@ -177,8 +177,8 @@ int b200gs_backward_deterministic(const b200gs_params *prm,
  *     cov3D_precomp it is B200GS_E_ARGS; the backward needs opacities.  Only shape is checked, not the values (no sync).
  * The other fields are NULL when their feature is off; each feature below says which fields turn it on.  A build of the
  * library without a feature returns B200GS_E_UNSUPPORTED for a call that turns it on, before any other argument check: the
- * classic comparator has none of the four, nor the deterministic backward; the bulk-copy build has no normals, geometry or
- * contribution scores.  Contribution scores together with normals or geometry are B200GS_E_ARGS.
+ * classic comparator has none of the four, nor the deterministic backward.  Contribution scores together with normals or
+ * geometry are B200GS_E_ARGS.
  *
  * Normal maps: each Gaussian's shortest-axis normal blended like its colour.  On in a forward iff gauss_normals is set; on
  * in a backward iff gauss_normals and dL_dnormal are both set (dL_dnormal without gauss_normals is B200GS_E_ARGS).

@@ -26,7 +26,7 @@ from humangaussian_b200 import dist as D  # noqa: E402
 from humangaussian_b200 import rasterizer as R  # noqa: E402
 
 PREPASS = ("det_start_kernel", "det_plan_kernel", "PopcLoad")
-B1 = ("blend_bwd_det_kernel",)
+B1 = ("blend_bwd_kernel<true, false, false, false>",)
 REDUCE = ("det_reduce_kernel",)
 
 
