@@ -69,8 +69,9 @@ __device__ __forceinline__ float gs_dot3(float a0, float a1, float a2, float b0,
 
 // torch.sigmoid in float32, as the densify plan and the MCMC kernels (densify.cu, mcmc.cu) evaluate it
 __device__ __forceinline__ float gs_sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }
-// F.normalize(dim=1) of a quaternion as torch's CUDA kernels evaluate it in float32: x / max(||x||, 1e-12) (preprocess.cu,
-// mcmc.cu); returns the clamped norm
+// F.normalize(dim=1) of a quaternion in float32: x / max(||x||, 1e-12), the squares summed pairwise without FMA (preprocess.cu,
+// mcmc.cu); returns the clamped norm.  torch's own F.normalize on the device may sum them in another order: on the benchmark's
+// scene under torch 2.11 its result differs in the last bit for about one quaternion in six (tests/test_gpu_bench_step.py)
 __device__ __forceinline__ float gs_normalize4(float *q)
 {
     const float n2 = fadd(fadd(fmul(q[0], q[0]), fmul(q[1], q[1])), fadd(fmul(q[2], q[2]), fmul(q[3], q[3])));

@@ -27,8 +27,8 @@ import numpy as np
 import pytest
 import torch
 
+import bench_step_reference as BS
 import contribution_reference as CR
-import normal_reference as NR
 import option_matrix_reference as OR
 from util import grad_images, grads_agree, screen_scene, small_scene
 
@@ -171,18 +171,13 @@ def _views(inp, cams, V):
 
 def _raw_of(inp):
     """raw parameters whose activations are inp's up to rounding, and inp re-activated from them as the kernels activate
-    (expf and 1 / (1 + expf(-x)) on the device, the normalisation in gs_normalize4's order), so the oracle sees the
-    kernels' activated values bit for bit"""
+    (bench_step_reference.activate on the device), so the oracle sees the kernels' activated values bit for bit"""
     o = np.asarray(inp["opacities"], np.float64)
     raw = dict(opacities=np.log(o / (1 - o)).astype(np.float32))
-    e = torch.exp(-torch.tensor(raw["opacities"], device=DEV)).cpu().numpy()
-    act = dict(opacities=(np.float32(1) / (np.float32(1) + e)).astype(np.float32))
     if inp.get("scales") is not None:
         raw.update(scales=np.log(inp["scales"].astype(np.float64)).astype(np.float32),
                    rotations=(inp["rotations"] * 1.3).astype(np.float32))
-        act["scales"] = torch.exp(torch.tensor(raw["scales"], device=DEV)).cpu().numpy()
-        act["rotations"] = NR.activate(raw["scales"], raw["rotations"], raw=True)[1]
-    return raw, dict(inp, **act)
+    return raw, dict(inp, **BS.activate(raw, DEV))
 
 
 def setup(case, scene=None):
