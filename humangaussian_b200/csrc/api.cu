@@ -783,6 +783,43 @@ int b200gs_density_field(int32_t P, const float *means, const float *cov6, const
     return B200GS_OK;
 }
 
+size_t b200gs_field_query_scratch_bytes(int32_t P, int32_t n_points, int32_t resolution, int32_t num_blocks, int32_t sh_degree)
+{
+    const int split = field_split(resolution, num_blocks);
+    return split && P >= 0 && n_points >= 0 && sh_degree >= 0 && sh_degree <= 3
+               ? field_query_scratch_bytes(P, n_points, resolution, split, sh_degree)
+               : 0;
+}
+
+int b200gs_field_query(int32_t P, const float *means, const float *cov6, const float *opacities, const float *shs, int32_t sh_coeffs,
+                       int32_t sh_degree, int32_t resolution, int32_t num_blocks, const float *samples, float relax, int32_t n_points,
+                       const float *points, float *density, float *normals, float *colors, void *scratch, size_t scratch_bytes,
+                       void *stream)
+{
+    if (P < 0 || n_points < 0 || resolution < 1 || num_blocks < 1 || sh_degree < 0 || sh_degree > 3) return B200GS_E_ARGS;
+    if (colors && !shs) return B200GS_E_ARGS;
+    if (shs && sh_coeffs < (sh_degree + 1) * (sh_degree + 1)) return B200GS_E_ARGS;
+    const int split = field_split(resolution, num_blocks);
+    if (!split) return B200GS_E_RANGE;
+    if (n_points == 0) return B200GS_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (P == 0) { // no Gaussian: every output is 0
+        if (density) CK(cudaMemsetAsync(density, 0, (size_t)n_points * 4, st), "field_query memset");
+        if (normals) CK(cudaMemsetAsync(normals, 0, (size_t)n_points * 12, st), "field_query memset");
+        if (colors) CK(cudaMemsetAsync(colors, 0, (size_t)n_points * 12, st), "field_query memset");
+        return B200GS_OK;
+    }
+    if (!means || !cov6 || !opacities || !samples || !points || !scratch) return B200GS_E_ARGS;
+    if (scratch_bytes < field_query_scratch_bytes(P, n_points, resolution, split, sh_degree)) return B200GS_E_BUFFER;
+    int nl = 0;
+    if (launch_field_query(P, means, cov6, opacities, shs, sh_coeffs, sh_degree, resolution, split, samples, relax, n_points, points,
+                           density, normals, colors, (char *)scratch, scratch_bytes, st, &nl))
+        return B200GS_E_RANGE;
+    g_launches += nl;
+    CK(cudaGetLastError(), "field_query launch");
+    return B200GS_OK;
+}
+
 static bool mc_dims_ok(int32_t X, int32_t Y, int32_t Z)
 {   // vertex ids are int32 and there is at most one vertex per grid edge, fewer than 3 per grid point
     return X >= 2 && Y >= 2 && Z >= 2 && 3 * (int64_t)X * Y * Z <= 0x7fffffffLL;

@@ -257,6 +257,11 @@ void launch_adam_packed(const AdamArgs &a, int64_t total, float *params, const f
 size_t density_field_scratch_bytes(int P, int res, int split);
 int launch_density_field(int P, const float *means, const float *cov6, const float *opac, int res, int split, const float *samples,
                          float relax, float *field, char *scratch, size_t scratch_bytes, cudaStream_t st, int *n_launches);
+// field query at n_points points of the field's frame (sh_degree 0-3; colours only when both shs and colors are given)
+size_t field_query_scratch_bytes(int P, int n_points, int res, int split, int sh_degree);
+int launch_field_query(int P, const float *means, const float *cov6, const float *opac, const float *shs, int sh_coeffs, int sh_degree,
+                       int res, int split, const float *samples, float relax, int n_points, const float *points, float *density,
+                       float *normals, float *colors, char *scratch, size_t scratch_bytes, cudaStream_t st, int *n_launches);
 size_t marching_cubes_scratch_bytes(int X, int Y, int Z);
 int launch_marching_cubes_count(int X, int Y, int Z, const float *vol, float iso, char *scratch, size_t scratch_bytes, uint64_t *counts,
                                 cudaStream_t st, int *n_launches);

@@ -13,10 +13,15 @@ summation order, so it is the same bits on every run.  `marching_cubes` is a GPU
 (mc_table.py): one welded vertex per crossing grid edge, triangles facing lower density.  `extract_mesh` chains the two
 and maps the vertices back to world space as the reference does.  The reference's clean_mesh / decimate_mesh
 (pymeshlab remeshing) are not part of this module: the output is the raw marching-cubes mesh.  There is no CPU path.
+
+`query_field` evaluates the same field at arbitrary world points (csrc/mesh.cu, b200gs_field_query): the density, the
+outward normal -grad / |grad|, and the SH colour of the opacity-weighted mean coefficients seen along -normal.
+`extract_colored_mesh` is `extract_mesh` with per-vertex normals and colours from it; `save_obj` and `save_ply_mesh`
+write them.
 """
 from __future__ import annotations
 
-from typing import NamedTuple
+from typing import NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -70,6 +75,58 @@ def _covariance(stds, rotations):
     return torch.stack([cov(0, 0), cov(0, 1), cov(0, 2), cov(1, 1), cov(1, 2), cov(2, 2)], dim=1).contiguous()
 
 
+class _Kept(NamedTuple):
+    """The Gaussians extract_fields counts, in the field's normalised frame."""
+    xyz: torch.Tensor    # [n,3] normalised centres
+    cov6: torch.Tensor   # [n,6] normalised covariances
+    opac: torch.Tensor   # [n] activated opacities
+    keep: torch.Tensor   # bool [P]
+    center: torch.Tensor
+    scale: float
+
+
+def _unwrap(fn, means3D, opacities, scales, rotations, raw, shs=None, sh_degree=None):
+    """A GaussianParams -> its raw tensors, shs = cat(features_dc, features_rest) and its sh_degree."""
+    if isinstance(means3D, GaussianParams):
+        if opacities is not None or scales is not None or rotations is not None or shs is not None:
+            raise ValueError(f"b200gs: {fn}: pass either a GaussianParams or the tensors")
+        g = means3D
+        shs = torch.cat([g.features_dc, g.features_rest], 1)
+        return g.xyz, g.opacity, g.scaling, g.rotation, True, shs, g.sh_degree if sh_degree is None else sh_degree
+    return means3D, opacities, scales, rotations, raw, shs, sh_degree
+
+
+def _kept(fn, means3D, opacities, scales, rotations, raw, resolution, num_blocks):
+    """extract_fields' checks, kept set, bounding-box normalisation and covariances."""
+    dev = means3D.device if isinstance(means3D, torch.Tensor) else None
+    if dev is None or dev.type != "cuda":
+        raise RuntimeError("b200gs: tensors must live on a CUDA device (there is no CPU path)")
+    resolution, num_blocks = _check_grid(resolution, num_blocks)
+    P = means3D.shape[0] if means3D.dim() == 2 else -1
+    means3D = _f32_cuda(means3D, "means3D", lambda t: t.dim() == 2 and t.shape[1] == 3)
+    opacities = _f32_cuda(opacities, "opacities", lambda t: tuple(t.shape) in ((P,), (P, 1)), dev).reshape(P)
+    scales = _f32_cuda(scales, "scales", lambda t: tuple(t.shape) == (P, 3), dev)
+    rotations = _f32_cuda(rotations, "rotations", lambda t: tuple(t.shape) == (P, 4), dev)
+
+    opac = torch.sigmoid(opacities) if raw else opacities
+    keep = opac > OPACITY_MIN
+    xyz = means3D[keep]
+    if xyz.shape[0] == 0:
+        raise ValueError(f"b200gs: {fn}: no Gaussian has opacity > {OPACITY_MIN}")
+    if not bool(torch.isfinite(xyz).all()):
+        raise ValueError(f"b200gs: {fn}: a kept Gaussian has a non-finite position")
+    stds = torch.exp(scales[keep]) if raw else scales[keep]
+    mn, mx = xyz.amin(0), xyz.amax(0)
+    center = (mn + mx) / 2
+    extent = (mx - mn).amax().item()
+    if extent == 0:
+        raise ValueError(f"b200gs: {fn}: the kept Gaussians' centres are a single point")
+    scale = 1.8 / extent
+    xyz = ((xyz - center) * scale).contiguous()
+    cov6 = _covariance(stds * scale, rotations[keep])
+    return _Kept(xyz, cov6, opac[keep].contiguous(), keep, center, scale), resolution, num_blocks
+
+
 @torch.no_grad()
 def extract_fields(means3D, opacities=None, scales=None, rotations=None, *, raw=False, resolution=128, num_blocks=16,
                    relax_ratio=1.5) -> Fields:
@@ -85,40 +142,19 @@ def extract_fields(means3D, opacities=None, scales=None, rotations=None, *, raw=
         if opacities is not None or scales is not None or rotations is not None:
             raise ValueError("b200gs: extract_fields: pass either a GaussianParams or the four tensors")
         means3D, opacities, scales, rotations, raw = means3D.xyz, means3D.opacity, means3D.scaling, means3D.rotation, True
-    dev = means3D.device if isinstance(means3D, torch.Tensor) else None
-    if dev is None or dev.type != "cuda":
-        raise RuntimeError("b200gs: tensors must live on a CUDA device (there is no CPU path)")
-    resolution, num_blocks = _check_grid(resolution, num_blocks)
-    P = means3D.shape[0] if means3D.dim() == 2 else -1
-    means3D = _f32_cuda(means3D, "means3D", lambda t: t.dim() == 2 and t.shape[1] == 3)
-    opacities = _f32_cuda(opacities, "opacities", lambda t: tuple(t.shape) in ((P,), (P, 1)), dev).reshape(P)
-    scales = _f32_cuda(scales, "scales", lambda t: tuple(t.shape) == (P, 3), dev)
-    rotations = _f32_cuda(rotations, "rotations", lambda t: tuple(t.shape) == (P, 4), dev)
+    k, resolution, num_blocks = _kept("extract_fields", means3D, opacities, scales, rotations, raw, resolution, num_blocks)
+    return Fields(_density_field(k.xyz, k.cov6, k.opac, resolution, num_blocks, relax_ratio), k.center, k.scale)
 
-    opac = torch.sigmoid(opacities) if raw else opacities
-    keep = opac > OPACITY_MIN
-    xyz = means3D[keep]
-    if xyz.shape[0] == 0:
-        raise ValueError(f"b200gs: extract_fields: no Gaussian has opacity > {OPACITY_MIN}")
-    if not bool(torch.isfinite(xyz).all()):
-        raise ValueError("b200gs: extract_fields: a kept Gaussian has a non-finite position")
-    stds = torch.exp(scales[keep]) if raw else scales[keep]
-    mn, mx = xyz.amin(0), xyz.amax(0)
-    center = (mn + mx) / 2
-    extent = (mx - mn).amax().item()
-    if extent == 0:
-        raise ValueError("b200gs: extract_fields: the kept Gaussians' centres are a single point")
-    scale = 1.8 / extent
-    xyz = ((xyz - center) * scale).contiguous()
-    cov6 = _covariance(stds * scale, rotations[keep])
-    return Fields(_density_field(xyz, cov6, opac[keep].contiguous(), resolution, num_blocks, relax_ratio), center, scale)
+
+def _samples_relax(dev, resolution, num_blocks, relax_ratio):
+    samples = torch.linspace(-1, 1, resolution).to(dev)  # built on the CPU, as the reference builds it
+    return samples, float(np.float32((2 / num_blocks) * relax_ratio))
 
 
 def _density_field(xyz, cov6, opac, resolution, num_blocks, relax_ratio):
     """b200gs_density_field on normalised centres [n,3], covariances [n,6] and opacities [n] (all kept)."""
     dev, n = xyz.device, xyz.shape[0]
-    samples = torch.linspace(-1, 1, resolution).to(dev)  # built on the CPU, as the reference builds it
-    relax = float(np.float32((2 / num_blocks) * relax_ratio))
+    samples, relax = _samples_relax(dev, resolution, num_blocks, relax_ratio)
     occ = torch.empty((resolution,) * 3, dtype=torch.float32, device=dev)
     L = R.load_library()
     with torch.cuda.device(dev):
@@ -166,26 +202,185 @@ class Mesh(NamedTuple):
     faces: torch.Tensor     # int32 [F,3]
 
 
+def _mesh(k, resolution, num_blocks, relax_ratio, density_thresh):
+    """-> (index-space vertices, faces, world vertices) of extract_mesh from the kept set k."""
+    occ = _density_field(k.xyz, k.cov6, k.opac, resolution, num_blocks, relax_ratio)
+    v, faces = marching_cubes(occ, density_thresh)
+    w = (v.double() / (resolution - 1.0) * 2 - 1) / k.scale + k.center.double()
+    return v, faces, w.float()
+
+
 @torch.no_grad()
 def extract_mesh(means3D, opacities=None, scales=None, rotations=None, *, raw=False, density_thresh=1.0, resolution=128,
                  num_blocks=16, relax_ratio=1.5) -> Mesh:
     """The reference's extract_mesh up to its remeshing: extract_fields, marching cubes at density_thresh, and the vertices
     mapped back to world space as v / (resolution - 1) * 2 - 1, then / scale + center (in float64, stored as float32)."""
-    f = extract_fields(means3D, opacities, scales, rotations, raw=raw, resolution=resolution, num_blocks=num_blocks,
-                       relax_ratio=relax_ratio)
-    v, faces = marching_cubes(f.occ, density_thresh)
-    w = (v.double() / (resolution - 1.0) * 2 - 1) / f.scale + f.center.double()
-    return Mesh(w.float(), faces)
+    if isinstance(means3D, GaussianParams):
+        if opacities is not None or scales is not None or rotations is not None:
+            raise ValueError("b200gs: extract_fields: pass either a GaussianParams or the four tensors")
+        means3D, opacities, scales, rotations, raw = means3D.xyz, means3D.opacity, means3D.scaling, means3D.rotation, True
+    k, resolution, num_blocks = _kept("extract_fields", means3D, opacities, scales, rotations, raw, resolution, num_blocks)
+    _, faces, w = _mesh(k, resolution, num_blocks, relax_ratio, density_thresh)
+    return Mesh(w, faces)
 
 
-def save_obj(path, vertices, faces):
-    """Wavefront OBJ: `v x y z` lines, then `f a b c` with 1-based indices."""
-    v = np.asarray(vertices.detach().cpu() if isinstance(vertices, torch.Tensor) else vertices, dtype=np.float64).reshape(-1, 3)
-    f = np.asarray(faces.detach().cpu() if isinstance(faces, torch.Tensor) else faces, dtype=np.int64).reshape(-1, 3)
+# ---- field query: normals and colours ------------------------------------------------------------------------------------
+class FieldQuery(NamedTuple):
+    density: torch.Tensor            # float32 [n]: the field at each point
+    normals: torch.Tensor            # float32 [n,3]: -grad / |grad| (outward, towards lower density); 0 where grad = 0
+    colors: Optional[torch.Tensor]   # float32 [n,3] >= 0 (not clamped above), or None without SH
+
+
+class ColoredMesh(NamedTuple):
+    vertices: torch.Tensor          # float32 [V,3], world space (extract_mesh's bytes)
+    faces: torch.Tensor             # int32 [F,3] (extract_mesh's bytes)
+    normals: torch.Tensor           # float32 [V,3], unit or 0
+    colors: Optional[torch.Tensor]  # float32 [V,3], or None without SH
+
+
+def _check_shs(fn, shs, keep, sh_degree, view_dependent, dev):
+    """-> (kept SH rows [n,K,3] contiguous, K, the degree the kernel evaluates), or (None, 0, 0) without SH."""
+    if shs is None:
+        if sh_degree is not None:
+            raise ValueError(f"b200gs: {fn}: sh_degree without shs")
+        return None, 0, 0
+    P = keep.shape[0]
+    shs = _f32_cuda(shs, "shs", lambda t: t.dim() == 3 and t.shape[0] == P and t.shape[1] >= 1 and t.shape[2] == 3, dev)
+    K = int(shs.shape[1])
+    if sh_degree is None:
+        sh_degree = min(3, int(np.sqrt(K)) - 1)
+    if not isinstance(sh_degree, (int, np.integer)) or not 0 <= sh_degree <= 3 or (sh_degree + 1) ** 2 > K:
+        raise ValueError(f"b200gs: {fn}: sh_degree must be 0..3 with (sh_degree + 1)^2 <= {K} coefficients (got {sh_degree!r})")
+    return shs[keep].contiguous(), K, int(sh_degree) if view_dependent else 0
+
+
+def _query(k, shs, K, deg, q, resolution, num_blocks, relax_ratio) -> FieldQuery:
+    """b200gs_field_query at normalised points q [n,3] (contiguous float32) for the kept set k."""
+    dev, n, P = q.device, q.shape[0], k.xyz.shape[0]
+    if n > 0x7FFFFFFF:
+        raise ValueError(f"b200gs: query_field: {n} points do not fit int32 point ids")
+    density = torch.empty(n, dtype=torch.float32, device=dev)
+    normals = torch.empty(n, 3, dtype=torch.float32, device=dev)
+    colors = torch.empty(n, 3, dtype=torch.float32, device=dev) if shs is not None else None
+    if n == 0:
+        return FieldQuery(density, normals, colors)
+    samples, relax = _samples_relax(dev, resolution, num_blocks, relax_ratio)
+    L = R.load_library()
+    with torch.cuda.device(dev):
+        scratch = torch.empty(L.b200gs_field_query_scratch_bytes(P, n, resolution, num_blocks, deg), dtype=torch.uint8, device=dev)
+        R._check(L.b200gs_field_query(P, R._ptr(k.xyz), R._ptr(k.cov6), R._ptr(k.opac), R._ptr(shs), K, deg, resolution, num_blocks,
+                                      R._ptr(samples), relax, n, R._ptr(q), R._ptr(density), R._ptr(normals), R._ptr(colors),
+                                      R._ptr(scratch), scratch.numel(), R._stream(dev)), "field_query")
+    return FieldQuery(density, normals, colors)
+
+
+@torch.no_grad()
+def query_field(points, means3D, opacities=None, scales=None, rotations=None, shs=None, *, raw=False, sh_degree=None,
+                view_dependent=True, resolution=128, num_blocks=16, relax_ratio=1.5) -> FieldQuery:
+    """extract_fields' density at world points [n,3], with the outward normal and an SH colour (DESIGN.md section 2).
+
+    The Gaussians come in any form extract_fields takes (activated tensors, raw=True, views of the packed buffer, or a
+    GaussianParams as means3D, whose SH are cat(features_dc, features_rest) at its sh_degree); shs [P,K,3] are the SH
+    coefficients of the same Gaussians, sh_degree (default: the largest that K holds, at most 3) the degree evaluated.
+    The points are mapped into the field's frame as (p - center) * scale in float32; there each point sees the members of
+    the block it falls in, so at a grid sample the density is the field's voxel bit for bit.  colour =
+    max(SH(S / D, -normal) + 0.5, 0) with S / D the opacity-weighted mean coefficients; view_dependent=False (or a zero
+    normal) keeps the DC term alone.  Where the density is 0 every output is 0.  Use it to colour a mesh that was
+    remeshed or decimated elsewhere.  Raises ValueError for a non-finite point, and as extract_fields does."""
+    means3D, opacities, scales, rotations, raw, shs, sh_degree = _unwrap("query_field", means3D, opacities, scales, rotations, raw, shs,
+                                                                         sh_degree)
+    k, resolution, num_blocks = _kept("query_field", means3D, opacities, scales, rotations, raw, resolution, num_blocks)
+    dev = k.xyz.device
+    pts = _f32_cuda(points, "points", lambda t: t.dim() == 2 and t.shape[1] == 3, dev)
+    if not bool(torch.isfinite(pts).all()):
+        raise ValueError("b200gs: query_field: a point is not finite")
+    shs, K, deg = _check_shs("query_field", shs, k.keep, sh_degree, view_dependent, dev)
+    q = ((pts - k.center) * k.scale).contiguous()
+    return _query(k, shs, K, deg, q, resolution, num_blocks, relax_ratio)
+
+
+@torch.no_grad()
+def extract_colored_mesh(means3D, opacities=None, scales=None, rotations=None, shs=None, *, raw=False, sh_degree=None,
+                         view_dependent=True, density_thresh=1.0, resolution=128, num_blocks=16, relax_ratio=1.5) -> ColoredMesh:
+    """extract_mesh (the same vertex and face bytes) with per-vertex normals and colours from the field query, evaluated at
+    the vertices' normalised positions v / (resolution - 1) * 2 - 1 (float32).  Arguments as extract_mesh and
+    query_field; without SH (tensors and shs=None) colors is None."""
+    means3D, opacities, scales, rotations, raw, shs, sh_degree = _unwrap("extract_colored_mesh", means3D, opacities, scales, rotations,
+                                                                         raw, shs, sh_degree)
+    k, resolution, num_blocks = _kept("extract_colored_mesh", means3D, opacities, scales, rotations, raw, resolution, num_blocks)
+    shs, K, deg = _check_shs("extract_colored_mesh", shs, k.keep, sh_degree, view_dependent, k.xyz.device)
+    v, faces, w = _mesh(k, resolution, num_blocks, relax_ratio, density_thresh)
+    q = (v / (resolution - 1) * 2 - 1).contiguous()
+    fq = _query(k, shs, K, deg, q, resolution, num_blocks, relax_ratio)
+    return ColoredMesh(w, faces, fq.normals, fq.colors)
+
+
+# ---- files ---------------------------------------------------------------------------------------------------------------
+def _np(a, dtype):
+    return np.asarray(a.detach().cpu() if isinstance(a, torch.Tensor) else a, dtype=dtype)
+
+
+def _mesh_arrays(fn, vertices, faces, normals, colors):
+    v = _np(vertices, np.float64).reshape(-1, 3)
+    f = _np(faces, np.int64).reshape(-1, 3)
     if f.size and (f.min() < 0 or f.max() >= len(v)):
-        raise ValueError("b200gs: save_obj: a face refers to a vertex that does not exist")
+        raise ValueError(f"b200gs: {fn}: a face refers to a vertex that does not exist")
+    out = []
+    for name, a in (("normals", normals), ("colors", colors)):
+        if a is not None:
+            a = _np(a, np.float32)
+            if a.shape != (len(v), 3):
+                raise ValueError(f"b200gs: {fn}: {name} must be [{len(v)}, 3] (got {list(a.shape)})")
+        out.append(a)
+    return v, f, out[0], out[1]
+
+
+def save_obj(path, vertices, faces, *, normals=None, colors=None):
+    """Wavefront OBJ: `v x y z` lines (`v x y z r g b` with colours, clamped to [0, 1]), `vn x y z` lines with normals,
+    then `f a b c` with 1-based indices (`f a//a b//b c//c` with normals)."""
+    v, f, n, c = _mesh_arrays("save_obj", vertices, faces, normals, colors)
     with open(path, "w") as fh:
         if len(v):
-            fh.write("\n".join("v %.9g %.9g %.9g" % tuple(r) for r in v) + "\n")
+            if c is None:
+                fh.write("\n".join("v %.9g %.9g %.9g" % tuple(r) for r in v) + "\n")
+            else:
+                vc = np.concatenate([v, np.clip(c, 0, 1).astype(np.float64)], 1)
+                fh.write("\n".join("v %.9g %.9g %.9g %.9g %.9g %.9g" % tuple(r) for r in vc) + "\n")
+            if n is not None:
+                fh.write("\n".join("vn %.9g %.9g %.9g" % tuple(r) for r in n.astype(np.float64)) + "\n")
         if len(f):
-            fh.write("\n".join("f %d %d %d" % tuple(r) for r in f + 1) + "\n")
+            if n is None:
+                fh.write("\n".join("f %d %d %d" % tuple(r) for r in f + 1) + "\n")
+            else:
+                fh.write("\n".join("f %d//%d %d//%d %d//%d" % tuple(r) for r in np.repeat(f + 1, 2, 1)) + "\n")
+
+
+def save_ply_mesh(path, vertices, faces, normals=None, colors=None):
+    """Binary little-endian PLY: vertex properties `x y z` (float), `nx ny nz` (float) with normals, `red green blue`
+    (uchar, clamp(c, 0, 1) * 255 truncated, as the frame pack does) with colours; faces as `list uchar int`."""
+    v, f, n, c = _mesh_arrays("save_ply_mesh", vertices, faces, normals, colors)
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if n is not None:
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+    if c is not None:
+        fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    vert = np.empty(len(v), dtype=np.dtype(fields))
+    for i, ax in enumerate("xyz"):
+        vert[ax] = v[:, i]
+    if n is not None:
+        for i, ax in enumerate(("nx", "ny", "nz")):
+            vert[ax] = n[:, i]
+    if c is not None:
+        u8 = (np.clip(c, np.float32(0), np.float32(1)) * np.float32(255)).astype(np.uint8)
+        for i, ax in enumerate(("red", "green", "blue")):
+            vert[ax] = u8[:, i]
+    face = np.empty(len(f), dtype=np.dtype([("n", "u1"), ("i", "<i4", (3,))]))
+    face["n"] = 3
+    face["i"] = f
+    head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}"]
+    head += [f"property {'float' if t == '<f4' else 'uchar'} {name}" for name, t in fields]
+    head += [f"element face {len(f)}", "property list uchar int vertex_indices", "end_header"]
+    with open(path, "wb") as fh:
+        fh.write(("\n".join(head) + "\n").encode("ascii"))
+        fh.write(vert.tobytes())
+        fh.write(face.tobytes())

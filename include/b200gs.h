@@ -478,6 +478,32 @@ size_t b200gs_density_field_scratch_bytes(int32_t P, int32_t resolution, int32_t
 int b200gs_density_field(int32_t P, const float *means, const float *cov6, const float *opacities, int32_t resolution,
                          int32_t num_blocks, const float *samples, float relax, float *field, void *scratch, size_t scratch_bytes,
                          void *stream);
+/* b200gs_field_query: the field of b200gs_density_field (same Gaussians, resolution, num_blocks, samples, relax) at
+ * n_points arbitrary points q [n,3] of the same normalised frame, with its gradient and an SH colour.
+ *   Members: per axis h(q_a) = the largest chunk c with c == 0 or samples[c*split] <= q_a; the members of q are the
+ *   Gaussians the field counts for block (h(qx), h(qy), h(qz)) -- at a grid sample, exactly its voxel's members.
+ *   Weights w_g = opacities[g] * exp(p_g(q)), p_g in the field's float32 operations and order, with its cut-offs (p > 0
+ *   and p <= -104 add nothing).  Sums run over the members in the field's order, so every run writes the same bits and
+ *   a point's result does not depend on the other points.
+ *     density [n]   D = sum w_g; at a grid sample the same bits as the field's voxel.
+ *     normals [n,3] n = -G / |G| with G = sum w_g (-Sigma_g^-1 (q - mean_g)) (Sigma^-1 the field's inverse): outward,
+ *                   toward lower density, as marching cubes winds its triangles; 0 where |G| = 0.  The world mapping
+ *                   is a uniform scale and a translation, so n is also the world normal.
+ *     colors [n,3]  max(SH(S / D, -n) + 0.5, 0) per channel, S = sum w_g sh_g over the first (sh_degree+1)^2
+ *                   coefficients of shs [P,sh_coeffs,3], SH the render preprocess's basis; the DC term alone where n = 0
+ *                   (pass sh_degree 0 for a view-independent colour).  The SH of the opacity-weighted mean
+ *                   coefficients, not the mean of clamped per-Gaussian colours: the two differ only where one
+ *                   Gaussian's colour would clamp at 0.
+ *   Where D == 0 every output is 0; a non-finite point does not fault, but its outputs may be non-finite.  Any output
+ *   may be NULL to skip it; shs may be NULL when colors is.  scratch of b200gs_field_query_scratch_bytes(P, n_points,
+ *   res, num_blocks, sh_degree); n_points = 0 does nothing; P = 0 zeroes the outputs.
+ *   B200GS_E_ARGS: as b200gs_density_field, and n_points < 0, sh_degree outside 0..3, colors without shs, or
+ *   sh_coeffs < (sh_degree+1)^2 with shs; B200GS_E_RANGE as b200gs_density_field. */
+size_t b200gs_field_query_scratch_bytes(int32_t P, int32_t n_points, int32_t resolution, int32_t num_blocks, int32_t sh_degree);
+int b200gs_field_query(int32_t P, const float *means, const float *cov6, const float *opacities, const float *shs, int32_t sh_coeffs,
+                       int32_t sh_degree, int32_t resolution, int32_t num_blocks, const float *samples, float relax, int32_t n_points,
+                       const float *points, float *density, float *normals, float *colors, void *scratch, size_t scratch_bytes,
+                       void *stream);
 /* Marching cubes over volume [X,Y,Z] (device, z fastest) at `iso`: a corner is inside iff its value > iso; one vertex per
  * grid edge whose ends differ, at p0 + t along the edge, t = (iso - v0) / (v1 - v0), in index coordinates; triangles wound
  * with normals toward lower values.  Vertices are numbered in order of (grid point at the edge's low end, axis), triangles
