@@ -857,6 +857,59 @@ int b200gs_marching_cubes_emit(int32_t X, int32_t Y, int32_t Z, const float *vol
     return B200GS_OK;
 }
 
+static int pose_check(int32_t style, int32_t V, int32_t H, int32_t W, const void *scratch, size_t scratch_bytes)
+{
+    if ((style != 0 && style != 1) || V < 1 || H < 1 || W < 1 || !scratch) return B200GS_E_ARGS;
+    if (H > 16384 || W > 16384 || (style == 0 && H < 103)) return B200GS_E_RANGE; // HumanSD lines need thickness >= 2
+    if (scratch_bytes < pose_scratch_bytes(style, V, H) || (((uintptr_t)scratch) & 15)) return B200GS_E_BUFFER;
+    return B200GS_OK;
+}
+
+size_t b200gs_pose_scratch_bytes(int32_t style, int32_t n_views, int32_t height, int32_t width)
+{
+    if ((style != 0 && style != 1) || n_views < 1 || height < 1 || width < 1 || height > 16384 || width > 16384) return 0;
+    return pose_scratch_bytes(style, n_views, height);
+}
+
+int b200gs_pose_keypoints(int32_t style, int32_t n_views, int32_t n_keypoints, int32_t height, int32_t width, const float *points,
+                          const float *mvp, const uint8_t *occlusion, const int32_t *limbs, float *kp, void *scratch,
+                          size_t scratch_bytes, void *stream)
+{
+    if (const int rc = pose_check(style, n_views, height, width, scratch, scratch_bytes)) return rc;
+    if (n_keypoints != pose_keypoints(style) || !points || !mvp || !occlusion || !limbs || !kp) return B200GS_E_ARGS;
+    if ((((uintptr_t)points) & 15) || (((uintptr_t)kp) & 7)) return B200GS_E_BUFFER; // float4 loads, float2 stores
+    PoseArgs a{};
+    a.style = style; a.V = n_views; a.H = height; a.W = width;
+    a.points = points; a.mvp = mvp; a.occlusion = occlusion; a.kp = kp;
+    for (int l = 0; l < pose_limbs(style); ++l)
+        for (int j = 0; j < 2; ++j) {
+            if (limbs[2 * l + j] < 0 || limbs[2 * l + j] >= n_keypoints) return B200GS_E_ARGS;
+            a.limbs[l][j] = (int8_t)limbs[2 * l + j];
+        }
+    pose_layout(a, (char *)scratch);
+    launch_pose_setup(a, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "pose_keypoints launch");
+    return B200GS_OK;
+}
+
+int b200gs_pose_draw(int32_t style, int32_t n_views, int32_t height, int32_t width, const uint8_t *colors, const void *scratch,
+                     size_t scratch_bytes, float *out, void *stream)
+{
+    if (const int rc = pose_check(style, n_views, height, width, scratch, scratch_bytes)) return rc;
+    if (!colors || !out) return B200GS_E_ARGS;
+    if (((uintptr_t)out) & 15) return B200GS_E_BUFFER;
+    PoseArgs a{};
+    a.style = style; a.V = n_views; a.H = height; a.W = width; a.out = out;
+    for (int s = 0; s < pose_shapes(style); ++s)
+        for (int c = 0; c < 3; ++c) a.colors[s][c] = colors[3 * s + c];
+    pose_layout(a, (char *)scratch);
+    launch_pose_draw(a, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "pose_draw launch");
+    return B200GS_OK;
+}
+
 int b200gs_test_sort_pairs(uint32_t *keys_a, uint32_t *keys_b, uint32_t *vals_a, uint32_t *vals_b, int64_t n, int32_t nbits,
                            void *scratch, size_t scratch_bytes, int32_t *result_in_b, void *stream)
 {

@@ -267,3 +267,24 @@ int launch_marching_cubes_count(int X, int Y, int Z, const float *vol, float iso
                                 cudaStream_t st, int *n_launches);
 int launch_marching_cubes_emit(int X, int Y, int Z, const float *vol, float iso, const char *scratch, size_t scratch_bytes, float *verts,
                                int32_t *faces, cudaStream_t st, int *n_launches);
+
+// pose maps (pose.cu): style 0 HumanSD (17 keypoints, 16 limbs), 1 OpenPose (18 keypoints, 18 circles + 17 limbs)
+struct PoseArgs {
+    int style, V, H, W;
+    const float *points;       // [K,4]
+    const float *mvp;          // [V,4,4] row-major
+    const uint8_t *occlusion;  // [V]
+    float *kp;                 // [V,K,2] out
+    int2 *hulls;               // scratch [V][S][H][4]: each shape's disjoint runs [lo, hi] per row (empty: lo > hi)
+    int2 *polys;               // scratch [V][17][361]: OpenPose ellipse polygons
+    float *out;                // [V,H,W,3]
+    int8_t limbs[17][2];       // keypoint pairs in draw order
+    uint8_t colors[35][3];     // per shape in draw order (OpenPose: the 18 circles, then the 17 limbs)
+};
+int pose_shapes(int style);
+int pose_limbs(int style);
+int pose_keypoints(int style);
+size_t pose_scratch_bytes(int style, int V, int H);
+void pose_layout(PoseArgs &a, char *scratch);
+void launch_pose_setup(const PoseArgs &a, cudaStream_t st);
+void launch_pose_draw(const PoseArgs &a, cudaStream_t st);

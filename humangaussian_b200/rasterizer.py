@@ -116,7 +116,8 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_backward_deterministic_opts", "b200gs_sampling_rate", "b200gs_prune_plan", "b200gs_mcmc_noise",
            "b200gs_mcmc_ratio", "b200gs_mcmc_move", "b200gs_density_field_scratch_bytes", "b200gs_density_field",
            "b200gs_field_query_scratch_bytes", "b200gs_field_query",
-           "b200gs_marching_cubes_scratch_bytes", "b200gs_marching_cubes_count", "b200gs_marching_cubes_emit"]
+           "b200gs_marching_cubes_scratch_bytes", "b200gs_marching_cubes_count", "b200gs_marching_cubes_emit",
+           "b200gs_pose_scratch_bytes", "b200gs_pose_keypoints", "b200gs_pose_draw"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -194,6 +195,11 @@ def load_library():
     L.b200gs_field_query_scratch_bytes.restype = sz; L.b200gs_field_query_scratch_bytes.argtypes = [i32, i32, i32, i32, i32]
     L.b200gs_field_query.restype = C.c_int
     L.b200gs_field_query.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, C.c_float, i32, vp, vp, vp, vp, vp, sz, vp]
+    L.b200gs_pose_scratch_bytes.restype = sz; L.b200gs_pose_scratch_bytes.argtypes = [i32, i32, i32, i32]
+    L.b200gs_pose_keypoints.restype = C.c_int
+    L.b200gs_pose_keypoints.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, sz, vp]
+    L.b200gs_pose_draw.restype = C.c_int
+    L.b200gs_pose_draw.argtypes = [i32, i32, i32, i32, vp, vp, sz, vp, vp]
     L.b200gs_marching_cubes_scratch_bytes.restype = sz; L.b200gs_marching_cubes_scratch_bytes.argtypes = [i32, i32, i32]
     L.b200gs_marching_cubes_count.restype = C.c_int
     L.b200gs_marching_cubes_count.argtypes = [i32, i32, i32, vp, C.c_float, vp, sz, vp, vp]

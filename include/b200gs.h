@@ -550,6 +550,28 @@ size_t b200gs_test_sort_scratch_bytes(int64_t n);
 /* The deterministic exp used by the blend kernels, evaluated on the device for n floats (parity pin vs oracle). */
 int b200gs_test_exp(const float *x, float *y, int64_t n, void *stream);
 
+/* ---- pose maps (humangaussian_b200/pose.py) ----------------------------------------------------------------------
+ * The reference's skeleton images for n_views mvp matrices, in two launches on `stream` with no host wait:
+ * b200gs_pose_keypoints projects the keypoints and rasterises every shape of every view into scratch, b200gs_pose_draw
+ * writes the images from it.  style 0 is HumanSD (17 keypoints, 16 limbs, line thickness 10 * height / 512, so height
+ * >= 103), style 1 OpenPose (18 keypoints, 17 limbs).
+ *   points     device [n_keypoints, 4] float32, 16-byte aligned (the reference's Skeleton.points3D)
+ *   mvp        device [n_views, 4, 4] float32 row-major;  occlusion: device [n_views] uint8 (0 / 1)
+ *   limbs      HOST [limbs][2] int32 keypoint pairs in draw order (16 or 17 limbs)
+ *   kp         device [n_views, n_keypoints, 2] float32 out, 8-byte aligned: (x, y) pixel coordinates before truncation
+ *   colors     HOST [shapes][3] uint8 in draw order: HumanSD one per limb; OpenPose the 18 keypoint circles, then the
+ *              17 limbs
+ *   out        device [n_views, height, width, 3] float32, 16-byte aligned
+ * scratch: b200gs_pose_scratch_bytes(style, n_views, height, width) bytes, 16-byte aligned, kept between the two
+ * calls.  Returns B200GS_E_ARGS for a bad style, count, limb index or NULL pointer, B200GS_E_RANGE for sizes outside
+ * 1..16384 (or a HumanSD height below 103), B200GS_E_BUFFER for a small or misaligned buffer. */
+size_t b200gs_pose_scratch_bytes(int32_t style, int32_t n_views, int32_t height, int32_t width);
+int b200gs_pose_keypoints(int32_t style, int32_t n_views, int32_t n_keypoints, int32_t height, int32_t width, const float *points,
+                          const float *mvp, const uint8_t *occlusion, const int32_t *limbs, float *kp, void *scratch,
+                          size_t scratch_bytes, void *stream);
+int b200gs_pose_draw(int32_t style, int32_t n_views, int32_t height, int32_t width, const uint8_t *colors, const void *scratch,
+                     size_t scratch_bytes, float *out, void *stream);
+
 /* ---- per-stage device timing (CUDA events recorded on the launch stream around each stage) -----------------
  * enable, run any number of forward/backward calls, then read: accumulated milliseconds and call counts per stage
  * since the last read.  b200gs_profile_read synchronises on the recorded events. */
