@@ -72,10 +72,13 @@ __device__ __forceinline__ float gs_sigmoidf(float x) { return 1.0f / (1.0f + ex
 // F.normalize(dim=1) of a quaternion in float32: x / max(||x||, 1e-12), the squares summed pairwise without FMA (preprocess.cu,
 // mcmc.cu); returns the clamped norm.  torch's own F.normalize on the device may sum them in another order: on the benchmark's
 // scene under torch 2.11 its result differs in the last bit for about one quaternion in six (tests/test_gpu_bench_step.py)
-__device__ __forceinline__ float gs_normalize4(float *q)
+// len (optional) receives ||x|| before the clamp: F.normalize's Jacobian is (I - q^ q^T) / ||x|| where ||x|| >= 1e-12, and
+// I / 1e-12 below, where the divisor is the constant
+__device__ __forceinline__ float gs_normalize4(float *q, float *len = nullptr)
 {
-    const float n2 = fadd(fadd(fmul(q[0], q[0]), fmul(q[1], q[1])), fadd(fmul(q[2], q[2]), fmul(q[3], q[3])));
-    const float n = fmaxf(fsqrt(n2), 1e-12f);
+    const float l = fsqrt(fadd(fadd(fmul(q[0], q[0]), fmul(q[1], q[1])), fadd(fmul(q[2], q[2]), fmul(q[3], q[3]))));
+    if (len) *len = l;
+    const float n = fmaxf(l, 1e-12f);
 #pragma unroll
     for (int k = 0; k < 4; k++) q[k] = fdiv(q[k], n);
     return n;

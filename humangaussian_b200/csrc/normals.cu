@@ -12,8 +12,8 @@
 
 // the rotation and the axis as F1 holds them: q after the in-kernel normalise (raw), k from the activated scales before
 // scale_modifier and the 3D filter (both leave the argmin unchanged in exact arithmetic; this pins the float ties).
-// Returns ||q|| before the normalise (1 for post-activation inputs).
-__device__ __forceinline__ float normal_axis(const NormalArgs &a, int i, float *q, int *k)
+// Returns max(||q||, 1e-12), the normalise's divisor (1 for post-activation inputs); *qlen gets ||q|| itself.
+__device__ __forceinline__ float normal_axis(const NormalArgs &a, int i, float *q, int *k, float *qlen = nullptr)
 {
     float s[3];
 #pragma unroll
@@ -23,11 +23,7 @@ __device__ __forceinline__ float normal_axis(const NormalArgs &a, int i, float *
     float qn = 1.0f;
     if (a.raw) {
         s[0] = expf(s[0]); s[1] = expf(s[1]); s[2] = expf(s[2]);
-        // torch's F.normalize in float32, as preprocess.cu's gs_normalize4
-        const float n2 = fadd(fadd(fmul(q[0], q[0]), fmul(q[1], q[1])), fadd(fmul(q[2], q[2]), fmul(q[3], q[3])));
-        qn = fmaxf(fsqrt(n2), 1e-12f);
-#pragma unroll
-        for (int c = 0; c < 4; c++) q[c] = fdiv(q[c], qn);
+        qn = gs_normalize4(q, qlen); // torch's F.normalize in float32, as F1 applies it
     }
     // strict comparisons: the lowest index wins a tie
     int kk = 0;
@@ -93,10 +89,11 @@ __global__ void __launch_bounds__(256) normal_bwd_kernel(const NormalArgs a, con
     if (!any) return;
     float q[4];
     int k;
-    const float qn = normal_axis(a, i, q, &k);
+    float ql = 1.0f;
+    const float qn = normal_axis(a, i, q, &k, &ql);
     float4 dq = dcol_dq(k, q, g0, g1, g2);
-    if (a.raw) { // F.normalize's Jacobian, as the preprocess backward applies it
-        const float dot = q[0] * dq.x + q[1] * dq.y + q[2] * dq.z + q[3] * dq.w;
+    if (a.raw) { // F.normalize's Jacobian, as the preprocess backward applies it (no projection below ||q|| = 1e-12)
+        const float dot = ql >= 1e-12f ? q[0] * dq.x + q[1] * dq.y + q[2] * dq.z + q[3] * dq.w : 0.f;
         const float inv = 1.0f / qn;
         dq.x = (dq.x - q[0] * dot) * inv; dq.y = (dq.y - q[1] * dot) * inv; dq.z = (dq.z - q[2] * dot) * inv;
         dq.w = (dq.w - q[3] * dot) * inv;

@@ -30,6 +30,42 @@ __device__ __forceinline__ void build_cov3d(const float *s3, float mod, const fl
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(hi, max(lo, v)); }
 
+// F1's screen-space covariance of a Gaussian (3D covariance S) in view V (A.2 step 3), in its pinned operations: ca0, cb, cc0
+// before the 0.3 px^2 dilation.  The preprocess backward re-runs it for antialiasing, so that its rho is F1's bit for bit.
+__device__ __forceinline__ void gs_cov2d(const float *V, const float S[3][3], float tx, float ty, float tz, float fx, float fy,
+                                         float tanx, float tany, float &ca0, float &cb, float &cc0)
+{
+    const float limx = fmul(1.3f, tanx), limy = fmul(1.3f, tany);
+    const float txtz = fdiv(tx, tz), tytz = fdiv(ty, tz);
+    const float cx = fmul(fminf(limx, fmaxf(-limx, txtz)), tz);
+    const float cy = fmul(fminf(limy, fmaxf(-limy, tytz)), tz);
+    const float J00 = fdiv(fx, tz), J11 = fdiv(fy, tz);
+    const float tz2 = fmul(tz, tz);
+    const float J02 = fdiv(-fmul(fx, cx), tz2), J12 = fdiv(-fmul(fy, cy), tz2);
+    float M0[3], M1[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        M0[k] = ffma(J02, V[4 * k + 2], fmul(J00, V[4 * k + 0]));
+        M1[k] = ffma(J12, V[4 * k + 2], fmul(J11, V[4 * k + 1]));
+    }
+    float N0[3], N1[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        N0[k] = gs_dot3(M0[0], M0[1], M0[2], S[0][k], S[1][k], S[2][k]);
+        N1[k] = gs_dot3(M1[0], M1[1], M1[2], S[0][k], S[1][k], S[2][k]);
+    }
+    ca0 = gs_dot3(N0[0], N0[1], N0[2], M0[0], M0[1], M0[2]);
+    cb = gs_dot3(N0[0], N0[1], N0[2], M1[0], M1[1], M1[2]);
+    cc0 = gs_dot3(N1[0], N1[1], N1[2], M1[0], M1[1], M1[2]);
+}
+
+// antialiasing's det0 / det of F1's covariance (its floor: rho = sqrt(max(2.5e-5, ratio)))
+__device__ __forceinline__ float gs_aa_ratio(float ca0, float cb, float cc0)
+{
+    const float det = ffma(fadd(ca0, GS_DILATE), fadd(cc0, GS_DILATE), -fmul(cb, cb));
+    return fdiv(ffma(ca0, cc0, -fmul(cb, cb)), det);
+}
+
 // The 3D smoothing filter (DESIGN.md section 2) on one Gaussian's activated scales s (before scale_modifier) and variance
 // v: t_i = s_i^2 + v, s'_i = sqrt(t_i), r_i = s_i^2 / t_i (1 where t_i = 0); returns coef = sqrt(r_0 r_1 r_2), the factor
 // that keeps o * sqrt(det Sigma) when the opacity becomes o' = o * coef.  IEEE float32, no contraction.
@@ -146,30 +182,9 @@ __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(Pr
             const float ndcx = fmul(hx, pw), ndcy = fmul(hy, pw);
 
             const float tanx = a.tanfovx[v], tany = a.tanfovy[v];
-            const float fx = gs_focal(a.W, tanx), fy = gs_focal(a.H, tany);
-            const float limx = fmul(1.3f, tanx), limy = fmul(1.3f, tany);
-            const float txtz = fdiv(tx, tz), tytz = fdiv(ty, tz);
-            const float cx = fmul(fminf(limx, fmaxf(-limx, txtz)), tz);
-            const float cy = fmul(fminf(limy, fmaxf(-limy, tytz)), tz);
-            const float J00 = fdiv(fx, tz), J11 = fdiv(fy, tz);
-            const float tz2 = fmul(tz, tz);
-            const float J02 = fdiv(-fmul(fx, cx), tz2), J12 = fdiv(-fmul(fy, cy), tz2);
-            float M0[3], M1[3];
-#pragma unroll
-            for (int k = 0; k < 3; k++) {
-                M0[k] = ffma(J02, V[4 * k + 2], fmul(J00, V[4 * k + 0]));
-                M1[k] = ffma(J12, V[4 * k + 2], fmul(J11, V[4 * k + 1]));
-            }
-            float N0[3], N1[3];
-#pragma unroll
-            for (int k = 0; k < 3; k++) {
-                N0[k] = gs_dot3(M0[0], M0[1], M0[2], S[0][k], S[1][k], S[2][k]);
-                N1[k] = gs_dot3(M1[0], M1[1], M1[2], S[0][k], S[1][k], S[2][k]);
-            }
-            const float ca0 = gs_dot3(N0[0], N0[1], N0[2], M0[0], M0[1], M0[2]);
+            float ca0, cb, cc0;
+            gs_cov2d(V, S, tx, ty, tz, gs_focal(a.W, tanx), gs_focal(a.H, tany), tanx, tany, ca0, cb, cc0);
             const float ca = fadd(ca0, GS_DILATE);
-            const float cb = gs_dot3(N0[0], N0[1], N0[2], M1[0], M1[1], M1[2]);
-            const float cc0 = gs_dot3(N1[0], N1[1], N1[2], M1[0], M1[1], M1[2]);
             const float cc = fadd(cc0, GS_DILATE);
             const float det = ffma(ca, cc, -fmul(cb, cb));
             if (det == 0.0f) break;
@@ -216,8 +231,7 @@ __global__ void __launch_bounds__(256, PFWD_MIN_BLOCKS) preprocess_fwd_kernel(Pr
             float oe = op; // the record's opacity
             if (AA) {
                 // floor rho >= 0.005: a degenerate footprint (det0 <= 0) lands on it
-                const float det0 = ffma(ca0, cc0, -fmul(cb, cb));
-                oe = fmul(op, fsqrt(fmaxf(2.5e-5f, fdiv(det0, det))));
+                oe = fmul(op, fsqrt(fmaxf(2.5e-5f, gs_aa_ratio(ca0, cb, cc0))));
             }
             radius = rad;
             tiles = (uint32_t)area;
@@ -311,6 +325,7 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
 
     float c6[6];
     float R[3][3], s[3] = {0, 0, 0}, q[4] = {0, 0, 0, 0}, qnorm = 1.0f;
+    bool qproj = true; // F.normalize's Jacobian projects (||q|| >= 1e-12)
     float coef = 1.0f; // F3D: o' = o * coef
     if (a.cov_pre) {
         for (int k = 0; k < 6; k++) c6[k] = a.cov_pre[6 * (size_t)i + k];
@@ -319,7 +334,9 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
         for (int k = 0; k < 4; k++) q[k] = a.rots[4 * (size_t)i + k];
         if (a.raw) { // the same activations F1 applied
             s3[0] = expf(s3[0]); s3[1] = expf(s3[1]); s3[2] = expf(s3[2]);
-            qnorm = gs_normalize4(q);
+            float qlen;
+            qnorm = gs_normalize4(q, &qlen);
+            qproj = qlen >= 1e-12f;
         }
         if (F3D) { // the same filter F1 applied: s3 becomes s'
             float t[3], r[3];
@@ -440,8 +457,12 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
             // rho = sqrt(det0 / det), det = det0 + d (ca0 + cc0 + d), d = 0.3: the derivatives in a cancellation-free form
             //   drho/da = d (cc0 cc + b^2) / (2 rho det^2),  drho/dc = d (ca0 ca + b^2) / (2 rho det^2),
             //   drho/db = -d b (ca + cc0) / (rho det^2);  zero where the floor holds
-            const float ratio = (ca0 * cc0 - cb * cb) / denom;
-            const float rho = sqrtf(fmaxf(2.5e-5f, ratio));
+            // rho and its floor's branch are F1's, recomputed in F1's operations: det0 is a cancellation for a needle, so a
+            // ratio of this view's own rounding can land on the other side of 2.5e-5, and its rho can be off by more than itself
+            float fa0, fb, fc0;
+            gs_cov2d(V, S, tx, ty, tz, gs_focal(a.W, tanx), gs_focal(a.H, tany), tanx, tany, fa0, fb, fc0);
+            const float ratio = gs_aa_ratio(fa0, fb, fc0);
+            const float rho = fsqrt(fmaxf(2.5e-5f, ratio));
             dop += rho * gO;
             if (ratio > 2.5e-5f) {
                 // the opacity before the filter (after the sigmoid for raw parameters), re-read per view (an L1 hit) rather
@@ -627,8 +648,8 @@ __global__ void __launch_bounds__(128, PBWD_MIN_BLOCKS) preprocess_bwd_kernel(Pr
         dq.y = 2.f * y * (dR[0][1] + dR[1][0]) + 2.f * z * (dR[0][2] + dR[2][0]) + 2.f * r * (dR[2][1] - dR[1][2]) - 4.f * x * (dR[1][1] + dR[2][2]);
         dq.z = 2.f * x * (dR[0][1] + dR[1][0]) + 2.f * r * (dR[0][2] - dR[2][0]) + 2.f * z * (dR[1][2] + dR[2][1]) - 4.f * y * (dR[0][0] + dR[2][2]);
         dq.w = 2.f * r * (dR[1][0] - dR[0][1]) + 2.f * x * (dR[0][2] + dR[2][0]) + 2.f * y * (dR[1][2] + dR[2][1]) - 4.f * z * (dR[0][0] + dR[1][1]);
-        if (a.raw) { // Jacobian of x / max(||x||, eps): (dq - q_hat (q_hat . dq)) / ||x||   (F.normalize's autograd)
-            const float dot = r * dq.x + x * dq.y + y * dq.z + z * dq.w;
+        if (a.raw) { // Jacobian of x / max(||x||, eps): (dq - q_hat (q_hat . dq)) / ||x||, dq / eps below eps (F.normalize's autograd)
+            const float dot = qproj ? r * dq.x + x * dq.y + y * dq.z + z * dq.w : 0.f;
             const float inv = 1.0f / qnorm;
             dq.x = (dq.x - r * dot) * inv; dq.y = (dq.y - x * dot) * inv; dq.z = (dq.z - y * dot) * inv; dq.w = (dq.w - z * dot) * inv;
         }

@@ -943,7 +943,8 @@ def forward_backward_with_state(g_color, g_depth, g_alpha, g_normal=None, g_medi
     normals=True: the normal image is a fifth output after alpha, and g_normal [V,3,H,W] (None: no normal gradient) its
     gradient; with g_normal, `state` also holds "normal_wn" [V,P,4], the sums Wn = sum w * dL/dN (DESIGN.md section 2).
     geometry=True: the median and depth2 images follow (after the normal image, if any), and g_median / g_depth2 [V,1,H,W]
-    (None: zero) are their gradients; `state` holds "median_pos"."""
+    (None: zero) are their gradients; `state` holds "median_pos".  `state["grads"]` is the gradient tuple of that backward
+    (d_means3D, d_means2D, d_sh, d_colors, d_opacity, d_scales, d_rotations, d_cov3D; None where the input was absent)."""
     outs = forward_with_state(**kw)
     images = outs[:-2]
     state, st = outs[-2:]
@@ -952,13 +953,14 @@ def forward_backward_with_state(g_color, g_depth, g_alpha, g_normal=None, g_medi
     t = lambda k: _f32c(kw.get(k), dev)
     g = [_f32c(x, dev).reshape(V, c, st.H, st.W) for x, c in ((g_color, 3), (g_depth, 1), (g_alpha, 1))]
     det_state = {}
-    _backward_impl(st, t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"),
+    grads = _backward_impl(st, t("means3D"), t("shs"), t("colors_precomp"), t("opacities"), t("scales"), t("rotations"),
                    t("cov3D_precomp"), _f32c(kw["bg"], dev), t("viewmatrix").reshape(V, 4, 4), t("projmatrix").reshape(V, 4, 4),
                    t("campos").reshape(V, 3), *g, det_state=det_state,
                    g_normal=None if g_normal is None else _f32c(g_normal, dev).reshape(V, 3, st.H, st.W),
                    g_median=None if g_median is None else _f32c(g_median, dev).reshape(V, 1, st.H, st.W),
                    g_depth2=None if g_depth2 is None else _f32c(g_depth2, dev).reshape(V, 1, st.H, st.W))
     state.update(det_state)
+    state["grads"] = grads
     if st.normal_wn is not None:
         state["normal_wn"] = st.normal_wn.clone()
     nbytes = V * P * 48
