@@ -910,6 +910,115 @@ int b200gs_pose_draw(int32_t style, int32_t n_views, int32_t height, int32_t wid
     return B200GS_OK;
 }
 
+#define MESH_MAX_FACES (1 << 24) // triangle + 1 is exact in float32 below 2^24
+static bool misaligned(const void *p, uintptr_t a) { return ((uintptr_t)p) & (a - 1); }
+
+static int mesh_image_check(int32_t V, int32_t H, int32_t W, int32_t Nv, int32_t Nf)
+{
+    if (V < 1 || V > B200GS_MAX_VIEWS || H < 1 || W < 1 || H > 16384 || W > 16384 || Nf >= MESH_MAX_FACES) return B200GS_E_RANGE;
+    if (Nv < 0 || Nf < 0) return B200GS_E_ARGS;
+    return B200GS_OK;
+}
+
+size_t b200gs_mesh_raster_scratch_bytes(int32_t n_views, int32_t n_faces, int32_t height, int32_t width)
+{
+    if (mesh_image_check(n_views, height, width, 0, n_faces)) return 0;
+    return mesh_raster_scratch_bytes(n_views, n_faces, height, width);
+}
+
+int b200gs_mesh_raster_count(int32_t n_views, int32_t n_verts, int32_t n_faces, int32_t height, int32_t width, const float *pos,
+                             const int32_t *tri, void *scratch, size_t scratch_bytes, uint64_t *count, void *stream)
+{
+    if (const int rc = mesh_image_check(n_views, height, width, n_verts, n_faces)) return rc;
+    if (!pos || !tri || !scratch || !count) return B200GS_E_ARGS;
+    if (scratch_bytes < mesh_raster_scratch_bytes(n_views, n_faces, height, width) || misaligned(scratch, 16) || misaligned(pos, 16) ||
+        misaligned(tri, 4) || misaligned(count, 8))
+        return B200GS_E_BUFFER;
+    int nl = 0;
+    if (launch_mesh_raster_count(n_views, n_verts, n_faces, height, width, pos, tri, (char *)scratch, count, (cudaStream_t)stream, &nl))
+        return cuda_fail(cudaGetLastError(), "mesh_raster_count memset");
+    g_launches += nl;
+    CK(cudaGetLastError(), "mesh_raster_count launch");
+    return B200GS_OK;
+}
+
+int b200gs_mesh_raster_emit(int32_t n_views, int32_t n_verts, int32_t n_faces, int32_t height, int32_t width, void *scratch,
+                            size_t scratch_bytes, int32_t *pairs, size_t pairs_bytes, float *rast, void *stream)
+{
+    if (const int rc = mesh_image_check(n_views, height, width, n_verts, n_faces)) return rc;
+    if (!scratch || !rast || (!pairs && pairs_bytes)) return B200GS_E_ARGS;
+    if (scratch_bytes < mesh_raster_scratch_bytes(n_views, n_faces, height, width) || misaligned(scratch, 16) || misaligned(pairs, 16) ||
+        misaligned(rast, 16))
+        return B200GS_E_BUFFER;
+    int nl = 0;
+    if (launch_mesh_raster_emit(n_views, n_faces, height, width, (char *)scratch, pairs, pairs ? pairs_bytes / 4 : 0, rast,
+                                (cudaStream_t)stream, &nl))
+        return cuda_fail(cudaGetLastError(), "mesh_raster_emit memset");
+    g_launches += nl;
+    CK(cudaGetLastError(), "mesh_raster_emit launch");
+    return B200GS_OK;
+}
+
+int b200gs_mesh_interpolate(int32_t n_views, int32_t height, int32_t width, int32_t n_verts, int32_t n_faces, int32_t channels,
+                            const float *attr, int32_t attr_per_view, const float *rast, const int32_t *tri, float *out, void *stream)
+{
+    if (const int rc = mesh_image_check(n_views, height, width, n_verts, n_faces)) return rc;
+    if (channels < 1 || (attr_per_view != 0 && attr_per_view != 1) || !attr || !rast || !tri || !out) return B200GS_E_ARGS;
+    if (misaligned(rast, 16) || misaligned(attr, 4) || misaligned(tri, 4) || misaligned(out, 4)) return B200GS_E_BUFFER;
+    launch_mesh_interpolate(n_views, height, width, n_verts, n_faces, channels, attr, attr_per_view, rast, tri, out, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "mesh_interpolate launch");
+    return B200GS_OK;
+}
+
+size_t b200gs_mesh_incidence_bytes(int32_t n_verts, int32_t n_faces)
+{
+    if (n_verts < 0 || n_faces < 0 || n_faces >= MESH_MAX_FACES || n_verts == 0x7fffffff) return 0;
+    return mesh_incidence_bytes(n_verts, n_faces);
+}
+
+int b200gs_mesh_incidence(int32_t n_verts, int32_t n_faces, const int32_t *faces, void *incidence, size_t incidence_bytes, void *stream)
+{
+    if (n_verts < 0 || n_faces < 0) return B200GS_E_ARGS;
+    if (n_faces >= MESH_MAX_FACES || n_verts == 0x7fffffff) return B200GS_E_RANGE; // key n_verts marks an invalid face
+    if (!faces || !incidence) return B200GS_E_ARGS;
+    if (incidence_bytes < mesh_incidence_bytes(n_verts, n_faces) || misaligned(incidence, 16) || misaligned(faces, 4)) return B200GS_E_BUFFER;
+    int nl = 0;
+    const int rc = launch_mesh_incidence(n_verts, n_faces, faces, (char *)incidence, incidence_bytes, (cudaStream_t)stream, &nl);
+    if (rc == -1) return cuda_fail(cudaGetLastError(), "mesh_incidence memset");
+    if (rc) return B200GS_E_RANGE;
+    g_launches += nl;
+    CK(cudaGetLastError(), "mesh_incidence launch");
+    return B200GS_OK;
+}
+
+int b200gs_mesh_vertex_normals(int32_t n_frames, int32_t n_verts, int32_t n_faces, const float *vertices, const int32_t *faces,
+                               const void *incidence, size_t incidence_bytes, float *normals, void *stream)
+{
+    if (n_frames < 1 || n_frames > B200GS_MAX_VIEWS || n_faces >= MESH_MAX_FACES || n_verts == 0x7fffffff) return B200GS_E_RANGE;
+    if (n_verts < 0 || n_faces < 0 || !vertices || !faces || !incidence || !normals) return B200GS_E_ARGS;
+    if (incidence_bytes < mesh_incidence_bytes(n_verts, n_faces) || misaligned(incidence, 16) || misaligned(vertices, 4) ||
+        misaligned(faces, 4) || misaligned(normals, 4))
+        return B200GS_E_BUFFER;
+    if (n_verts == 0) return B200GS_OK;
+    launch_mesh_vertex_normals(n_frames, n_verts, n_faces, vertices, faces, (const char *)incidence, normals, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "mesh_vertex_normals launch");
+    return B200GS_OK;
+}
+
+int b200gs_mesh_normal_image(int32_t n_views, int32_t height, int32_t width, int32_t n_verts, int32_t n_faces, const float *normals,
+                             int32_t normals_per_view, const float *rast, const int32_t *tri, float *out, void *stream)
+{
+    if (const int rc = mesh_image_check(n_views, height, width, n_verts, n_faces)) return rc;
+    if ((normals_per_view != 0 && normals_per_view != 1) || !normals || !rast || !tri || !out) return B200GS_E_ARGS;
+    if (misaligned(rast, 16) || misaligned(normals, 4) || misaligned(tri, 4) || misaligned(out, 4)) return B200GS_E_BUFFER;
+    launch_mesh_normal_image(n_views, height, width, n_verts, n_faces, normals, normals_per_view, rast, tri, out, (cudaStream_t)stream);
+    g_launches += 1;
+    CK(cudaGetLastError(), "mesh_normal_image launch");
+    return B200GS_OK;
+}
+
 int b200gs_test_sort_pairs(uint32_t *keys_a, uint32_t *keys_b, uint32_t *vals_a, uint32_t *vals_b, int64_t n, int32_t nbits,
                            void *scratch, size_t scratch_bytes, int32_t *result_in_b, void *stream)
 {

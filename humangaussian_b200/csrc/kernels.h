@@ -288,3 +288,20 @@ size_t pose_scratch_bytes(int style, int V, int H);
 void pose_layout(PoseArgs &a, char *scratch);
 void launch_pose_setup(const PoseArgs &a, cudaStream_t st);
 void launch_pose_draw(const PoseArgs &a, cudaStream_t st);
+
+// mesh rendering (meshraster.cu).  Rasterisation: count (setup, per-tile counts, scan; the exact pair total lands at *count)
+// then emit from the same scratch.  Nonzero return: a failed memset.
+size_t mesh_raster_scratch_bytes(int V, int Nf, int H, int W);
+int launch_mesh_raster_count(int V, int Nv, int Nf, int H, int W, const float *pos, const int *tri, char *scratch, uint64_t *count,
+                             cudaStream_t st, int *n_launches);
+int launch_mesh_raster_emit(int V, int Nf, int H, int W, char *scratch, int *pairs, uint64_t cap, float *rast, cudaStream_t st,
+                            int *n_launches);
+void launch_mesh_interpolate(int V, int H, int W, int Nv, int Nf, int C, const float *attr, int per_view, const float *rast, const int *tri,
+                             float *out, cudaStream_t st);
+void launch_mesh_normal_image(int V, int H, int W, int Nv, int Nf, const float *vn, int per_view, const float *rast, const int *tri,
+                              float *out, cudaStream_t st);
+// per-vertex incidence lists in (corner, face) order; the vertex normals read the buffer the incidence call wrote
+size_t mesh_incidence_bytes(int Nv, int Nf);
+int launch_mesh_incidence(int Nv, int Nf, const int *faces, char *buf, size_t bytes, cudaStream_t st, int *n_launches);
+void launch_mesh_vertex_normals(int F, int Nv, int Nf, const float *verts, const int *faces, const char *incidence, float *out,
+                                cudaStream_t st);

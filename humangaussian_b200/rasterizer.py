@@ -117,7 +117,9 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_mcmc_ratio", "b200gs_mcmc_move", "b200gs_density_field_scratch_bytes", "b200gs_density_field",
            "b200gs_field_query_scratch_bytes", "b200gs_field_query",
            "b200gs_marching_cubes_scratch_bytes", "b200gs_marching_cubes_count", "b200gs_marching_cubes_emit",
-           "b200gs_pose_scratch_bytes", "b200gs_pose_keypoints", "b200gs_pose_draw"]
+           "b200gs_pose_scratch_bytes", "b200gs_pose_keypoints", "b200gs_pose_draw",
+           "b200gs_mesh_raster_scratch_bytes", "b200gs_mesh_raster_count", "b200gs_mesh_raster_emit", "b200gs_mesh_interpolate",
+           "b200gs_mesh_incidence_bytes", "b200gs_mesh_incidence", "b200gs_mesh_vertex_normals", "b200gs_mesh_normal_image"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -205,6 +207,20 @@ def load_library():
     L.b200gs_marching_cubes_count.argtypes = [i32, i32, i32, vp, C.c_float, vp, sz, vp, vp]
     L.b200gs_marching_cubes_emit.restype = C.c_int
     L.b200gs_marching_cubes_emit.argtypes = [i32, i32, i32, vp, C.c_float, vp, sz, vp, vp, vp]
+    L.b200gs_mesh_raster_scratch_bytes.restype = sz; L.b200gs_mesh_raster_scratch_bytes.argtypes = [i32, i32, i32, i32]
+    L.b200gs_mesh_raster_count.restype = C.c_int
+    L.b200gs_mesh_raster_count.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, sz, vp, vp]
+    L.b200gs_mesh_raster_emit.restype = C.c_int
+    L.b200gs_mesh_raster_emit.argtypes = [i32, i32, i32, i32, i32, vp, sz, vp, sz, vp, vp]
+    L.b200gs_mesh_interpolate.restype = C.c_int
+    L.b200gs_mesh_interpolate.argtypes = [i32, i32, i32, i32, i32, i32, vp, i32, vp, vp, vp, vp]
+    L.b200gs_mesh_incidence_bytes.restype = sz; L.b200gs_mesh_incidence_bytes.argtypes = [i32, i32]
+    L.b200gs_mesh_incidence.restype = C.c_int
+    L.b200gs_mesh_incidence.argtypes = [i32, i32, vp, vp, sz, vp]
+    L.b200gs_mesh_vertex_normals.restype = C.c_int
+    L.b200gs_mesh_vertex_normals.argtypes = [i32, i32, i32, vp, vp, vp, sz, vp, vp]
+    L.b200gs_mesh_normal_image.restype = C.c_int
+    L.b200gs_mesh_normal_image.argtypes = [i32, i32, i32, i32, i32, vp, i32, vp, vp, vp, vp]
     L.b200gs_last_cuda_error.restype = C.c_char_p
     L.b200gs_launch_count.restype = i64
     L.b200gs_profile_enable.restype = None; L.b200gs_profile_enable.argtypes = [C.c_int]

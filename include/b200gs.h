@@ -572,6 +572,50 @@ int b200gs_pose_keypoints(int32_t style, int32_t n_views, int32_t n_keypoints, i
 int b200gs_pose_draw(int32_t style, int32_t n_views, int32_t height, int32_t width, const uint8_t *colors, const void *scratch,
                      size_t scratch_bytes, float *out, void *stream);
 
+/* ---- mesh rendering (humangaussian_b200/meshrender.py; DESIGN.md section 2 is the specification) ------------------
+ * Forward-only triangle rasterisation in nvdiffrast's instance mode (one topology, a batch of clip-space vertex sets),
+ * attribute interpolation, and the reference's vertex normals and normal image (animation.py:558-601).  Every call
+ * enqueues on `stream`; the results are the same bytes on every run.  n_views / n_frames must be 1..B200GS_MAX_VIEWS,
+ * height and width 1..16384, n_faces 0..2^24 - 1 (triangle + 1 must be exact in float32), else B200GS_E_RANGE.  A NULL
+ * pointer is B200GS_E_ARGS; a buffer smaller than its *_bytes query, or a pos / rast / scratch / pairs / incidence
+ * pointer that is not 16-byte aligned (other arrays: 4-byte), is B200GS_E_BUFFER.
+ *   pos    device [n_views, n_verts, 4] float32 clip coordinates (X, Y, Z, W)
+ *   tri    device [n_faces, 3] int32; a triangle with an index outside [0, n_verts), a non-finite coordinate, or W <= 0
+ *          at all three vertices is not drawn (and never dereferenced)
+ *   rast   device [n_views, height, width, 4] float32: (u, v, z/w, triangle + 1) of the nearest covering triangle, all 0
+ *          where none covers the pixel centre.  Row 0 is clip y = -1.  A triangle covers no pixel outside its pixel
+ *          rectangle (its projected bounding box widened by one pixel, where every W > 0), so one whose edge functions
+ *          are rounding noise (point-sized) draws at most there.
+ * b200gs_mesh_raster_count sets up every (view, triangle), bins them into 16 x 16-pixel tiles and writes the exact number
+ * of (tile, triangle) pairs to count (device, uint64[1]).  The caller reads it (the one host wait of a rasterisation) to
+ * size pairs (>= 4 * count bytes) and calls b200gs_mesh_raster_emit with the same arguments and scratch, which fills the
+ * tile lists and writes rast.  With a pairs buffer smaller than that the output is unspecified, but every access stays
+ * inside the buffers. */
+size_t b200gs_mesh_raster_scratch_bytes(int32_t n_views, int32_t n_faces, int32_t height, int32_t width);
+int b200gs_mesh_raster_count(int32_t n_views, int32_t n_verts, int32_t n_faces, int32_t height, int32_t width, const float *pos,
+                             const int32_t *tri, void *scratch, size_t scratch_bytes, uint64_t *count, void *stream);
+int b200gs_mesh_raster_emit(int32_t n_views, int32_t n_verts, int32_t n_faces, int32_t height, int32_t width, void *scratch,
+                            size_t scratch_bytes, int32_t *pairs, size_t pairs_bytes, float *rast, void *stream);
+/* out [n_views, height, width, channels] = a0 u + a1 v + a2 ((1 - u) - v) of the rasterised triangle's vertex attributes,
+ * 0 where rast.w is not a triangle id in 1..n_faces (or the triangle has an index outside [0, n_verts)).
+ *   attr device [n_views, n_verts, channels] (attr_per_view = 1) or [n_verts, channels] shared by every view (0); channels >= 1 */
+int b200gs_mesh_interpolate(int32_t n_views, int32_t height, int32_t width, int32_t n_verts, int32_t n_faces, int32_t channels,
+                            const float *attr, int32_t attr_per_view, const float *rast, const int32_t *tri, float *out, void *stream);
+/* The per-vertex face lists of one topology, built once for any number of frames: for every vertex its faces where it
+ * is corner 0 in ascending face order, then corner 1, then corner 2.  A face with an index outside [0, n_verts) is in no
+ * list.  incidence: b200gs_mesh_incidence_bytes(n_verts, n_faces) bytes, 16-byte aligned, kept for the normals calls. */
+size_t b200gs_mesh_incidence_bytes(int32_t n_verts, int32_t n_faces);
+int b200gs_mesh_incidence(int32_t n_verts, int32_t n_faces, const int32_t *faces, void *incidence, size_t incidence_bytes, void *stream);
+/* normals [n_frames, n_verts, 3] of vertices [n_frames, n_verts, 3]: the sum of the unnormalised face normals
+ * cross(v1 - v0, v2 - v0) in the incidence order, (0, 0, 1) where its dot is not > 1e-20, then safe_normalize.  faces
+ * and incidence must be the ones b200gs_mesh_incidence was given and wrote. */
+int b200gs_mesh_vertex_normals(int32_t n_frames, int32_t n_verts, int32_t n_faces, const float *vertices, const int32_t *faces,
+                               const void *incidence, size_t incidence_bytes, float *normals, void *stream);
+/* The reference's normal image: out [n_views, height, width, 3] = (safe_normalize(interpolated normals) + 1) / 2 where rast
+ * holds a triangle (as b200gs_mesh_interpolate decides), 1.0 elsewhere.  normals as attr above with channels = 3. */
+int b200gs_mesh_normal_image(int32_t n_views, int32_t height, int32_t width, int32_t n_verts, int32_t n_faces, const float *normals,
+                             int32_t normals_per_view, const float *rast, const int32_t *tri, float *out, void *stream);
+
 /* ---- per-stage device timing (CUDA events recorded on the launch stream around each stage) -----------------
  * enable, run any number of forward/backward calls, then read: accumulated milliseconds and call counts per stage
  * since the last read.  b200gs_profile_read synchronises on the recorded events. */
