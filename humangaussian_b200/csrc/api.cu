@@ -1007,6 +1007,70 @@ int b200gs_mesh_vertex_normals(int32_t n_frames, int32_t n_verts, int32_t n_face
     return B200GS_OK;
 }
 
+// ---- mesh cleanup and decimation (meshclean.cu) ----
+static int mesh_edit_check(int32_t Nv, int32_t Nf, const float *vertices, const int32_t *faces, void *scratch, float *out_vertices,
+                           int32_t *out_faces, int64_t *counts, int32_t *rounds)
+{
+    if (Nv < 0 || Nf < 0 || !counts || !rounds) return B200GS_E_ARGS;
+    if (Nv >= 0x7fffffff || Nf >= MESH_MAX_FACES) return B200GS_E_RANGE;
+    if ((Nv && (!vertices || !out_vertices)) || (Nf && (!faces || !out_faces || !scratch))) return B200GS_E_ARGS;
+    if (misaligned(scratch, 16) || misaligned(vertices, 4) || misaligned(faces, 4) || misaligned(out_vertices, 4) || misaligned(out_faces, 4))
+        return B200GS_E_BUFFER;
+    return B200GS_OK;
+}
+
+static int mesh_edit_status(int rc, const char *where)
+{
+    if (rc == -2) return B200GS_E_ARGS;
+    if (rc == -3) { snprintf(g_err, sizeof(g_err), "%s: the face count after a round is not the planned one", where); return B200GS_E_CUDA; }
+    return cuda_fail(cudaGetLastError(), where);
+}
+
+size_t b200gs_mesh_clean_scratch_bytes(int32_t n_verts, int32_t n_faces)
+{
+    if (n_verts < 0 || n_faces < 0 || n_verts >= 0x7fffffff || n_faces >= MESH_MAX_FACES) return 0;
+    return mesh_clean_scratch_bytes(n_verts, n_faces);
+}
+
+int b200gs_mesh_clean(int32_t n_verts, int32_t n_faces, const float *vertices, const int32_t *faces, int32_t min_faces, double min_diameter,
+                      void *scratch, size_t scratch_bytes, float *out_vertices, int32_t *out_faces, int64_t *counts, int32_t *rounds,
+                      void *stream)
+{
+    if (const int rc = mesh_edit_check(n_verts, n_faces, vertices, faces, scratch, out_vertices, out_faces, counts, rounds)) return rc;
+    if (min_faces < 0 || !(min_diameter >= 0.0) || !(min_diameter < 1e300)) return B200GS_E_ARGS;
+    if (n_faces && scratch_bytes < mesh_clean_scratch_bytes(n_verts, n_faces)) return B200GS_E_BUFFER;
+    int nl = 0, r = 0;
+    const int rc = launch_mesh_clean(n_verts, n_faces, vertices, faces, min_faces, min_diameter, (char *)scratch, out_vertices, out_faces,
+                                     counts, &r, (cudaStream_t)stream, &nl);
+    *rounds = r;
+    if (rc) return mesh_edit_status(rc, "mesh_clean");
+    g_launches += nl;
+    CK(cudaGetLastError(), "mesh_clean launch");
+    return B200GS_OK;
+}
+
+size_t b200gs_mesh_decimate_scratch_bytes(int32_t n_verts, int32_t n_faces)
+{
+    if (n_verts < 0 || n_faces < 0 || n_verts >= 0x7fffffff || n_faces >= MESH_MAX_FACES) return 0;
+    return mesh_decimate_scratch_bytes(n_verts, n_faces);
+}
+
+int b200gs_mesh_decimate(int32_t n_verts, int32_t n_faces, const float *vertices, const int32_t *faces, int32_t target, void *scratch,
+                         size_t scratch_bytes, float *out_vertices, int32_t *out_faces, int64_t *counts, int32_t *rounds, void *stream)
+{
+    if (const int rc = mesh_edit_check(n_verts, n_faces, vertices, faces, scratch, out_vertices, out_faces, counts, rounds)) return rc;
+    if (target < 4) return B200GS_E_ARGS;
+    if (n_faces && scratch_bytes < mesh_decimate_scratch_bytes(n_verts, n_faces)) return B200GS_E_BUFFER;
+    int nl = 0, r = 0;
+    const int rc = launch_mesh_decimate(n_verts, n_faces, vertices, faces, target, (char *)scratch, out_vertices, out_faces, counts, &r,
+                                        (cudaStream_t)stream, &nl);
+    *rounds = r;
+    if (rc) return mesh_edit_status(rc, "mesh_decimate");
+    g_launches += nl;
+    CK(cudaGetLastError(), "mesh_decimate launch");
+    return B200GS_OK;
+}
+
 int b200gs_mesh_normal_image(int32_t n_views, int32_t height, int32_t width, int32_t n_verts, int32_t n_faces, const float *normals,
                              int32_t normals_per_view, const float *rast, const int32_t *tri, float *out, void *stream)
 {

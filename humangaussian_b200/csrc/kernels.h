@@ -305,3 +305,15 @@ size_t mesh_incidence_bytes(int Nv, int Nf);
 int launch_mesh_incidence(int Nv, int Nf, const int *faces, char *buf, size_t bytes, cudaStream_t st, int *n_launches);
 void launch_mesh_vertex_normals(int F, int Nv, int Nf, const float *verts, const int *faces, const char *incidence, float *out,
                                 cudaStream_t st);
+// the start [Nv + 1] and list arrays inside an incidence buffer of (Nv, Nf)
+void mesh_incidence_lists(int Nv, int Nf, const char *buf, const uint32_t **start, const uint32_t **list);
+
+// mesh cleanup and decimation (meshclean.cu).  Both wait on the host (clean: once per labelling round and once for the
+// counts; decimate: once for the index check, once per round and once for the counts).  counts = vertices, faces.
+// Nonzero return: -1 a CUDA call failed, -2 a face index outside [0, Nv), -3 (decimate) an internal face-count mismatch
+size_t mesh_clean_scratch_bytes(int Nv, int Nf);
+int launch_mesh_clean(int Nv, int Nf, const float *verts, const int *faces, int min_faces, double min_diameter, char *scratch,
+                      float *out_verts, int *out_faces, int64_t *counts, int *rounds, cudaStream_t st, int *n_launches);
+size_t mesh_decimate_scratch_bytes(int Nv, int Nf);
+int launch_mesh_decimate(int Nv, int Nf, const float *verts, const int *faces, int target, char *scratch, float *out_verts,
+                         int *out_faces, int64_t *counts, int *rounds, cudaStream_t st, int *n_launches);

@@ -489,6 +489,13 @@ void launch_mesh_normal_image(int V, int H, int W, int Nv, int Nf, const float *
 
 size_t mesh_incidence_bytes(int Nv, int Nf) { return IncidenceLayout(Nv, Nf).total; }
 
+void mesh_incidence_lists(int Nv, int Nf, const char *buf, const uint32_t **start, const uint32_t **list)
+{
+    const IncidenceLayout L(Nv, Nf);
+    *start = (const uint32_t *)(buf + L.start);
+    *list = (const uint32_t *)(buf + L.list);
+}
+
 int launch_mesh_incidence(int Nv, int Nf, const int *faces, char *buf, size_t bytes, cudaStream_t st, int *n_launches)
 {
     const IncidenceLayout L(Nv, Nf);

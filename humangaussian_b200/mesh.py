@@ -11,8 +11,10 @@ quirks included (DESIGN.md section 2):
 Those P-sized steps are the reference's own torch ops; the field itself is one CUDA pipeline (csrc/mesh.cu) with a fixed
 summation order, so it is the same bits on every run.  `marching_cubes` is a GPU marching cubes with a generated table
 (mc_table.py): one welded vertex per crossing grid edge, triangles facing lower density.  `extract_mesh` chains the two
-and maps the vertices back to world space as the reference does.  The reference's clean_mesh / decimate_mesh
-(pymeshlab remeshing) are not part of this module: the output is the raw marching-cubes mesh.  There is no CPU path.
+and maps the vertices back to world space as the reference does; by default the output is the raw marching-cubes mesh.
+`clean_mesh` (floater removal by connected component) and `decimate_mesh` (quadric edge collapse to a face budget) are
+the GPU counterparts of the reference's pymeshlab clean_mesh / decimate_mesh (csrc/meshclean.cu), and extract_mesh runs
+them on request.  Isotropic remeshing is not done.  There is no CPU path.
 
 `query_field` evaluates the same field at arbitrary world points (csrc/mesh.cu, b200gs_field_query): the density, the
 outward normal -grad / |grad|, and the SH colour of the opacity-weighted mean coefficients seen along -normal.
@@ -202,25 +204,116 @@ class Mesh(NamedTuple):
     faces: torch.Tensor     # int32 [F,3]
 
 
-def _mesh(k, resolution, num_blocks, relax_ratio, density_thresh):
-    """-> (index-space vertices, faces, world vertices) of extract_mesh from the kept set k."""
+def _edit_args(fn, vertices, faces):
+    v = _f32_cuda(vertices, "vertices", lambda t: t.dim() == 2 and t.shape[1] == 3)
+    if not isinstance(faces, torch.Tensor) or faces.dtype != torch.int32 or faces.device != v.device or faces.dim() != 2 or \
+            faces.shape[1] != 3:
+        desc = f"{tuple(faces.shape)} {faces.dtype} on {faces.device}" if isinstance(faces, torch.Tensor) else type(faces).__name__
+        raise ValueError(f"b200gs: {fn}: faces must be int32 [F,3] on the vertices' device ({desc})")
+    Nv, Nf = int(v.shape[0]), int(faces.shape[0])
+    if Nv >= 0x7FFFFFFF or Nf >= 1 << 24:
+        raise ValueError(f"b200gs: {fn}: {Nv} vertices / {Nf} faces exceed 2^31 - 1 / 2^24")
+    return v.contiguous(), faces.detach().contiguous(), Nv, Nf
+
+
+def _edit(fn, vertices, faces, call, scratch_bytes):
+    """Runs b200gs_mesh_clean / _decimate -> (Mesh in the input's frame, rounds)."""
+    import ctypes as C
+    v, f, Nv, Nf = _edit_args(fn, vertices, faces)
+    dev = v.device
+    L = R.load_library()
+    with torch.cuda.device(dev):
+        scratch = torch.empty(max(1, scratch_bytes(L, Nv, Nf)), dtype=torch.uint8, device=dev)
+        ov = torch.empty(Nv, 3, dtype=torch.float32, device=dev)
+        of = torch.empty(Nf, 3, dtype=torch.int32, device=dev)
+        counts, rounds = (C.c_int64 * 2)(), C.c_int32(0)
+        rc = call(L, Nv, Nf, R._ptr(v), R._ptr(f), R._ptr(scratch), scratch.numel(), R._ptr(ov), R._ptr(of), counts, C.byref(rounds),
+                  R._stream(dev))
+    if rc == R.E_ARGS:
+        raise ValueError(f"b200gs: {fn}: a face index lies outside [0, {Nv})")
+    R._check(rc, fn)
+    return Mesh(ov[:counts[0]], of[:counts[1]]), int(rounds.value)
+
+
+@torch.no_grad()
+def clean_mesh(vertices, faces, *, min_faces=64, min_diameter=0.2) -> Mesh:
+    """Floater removal (DESIGN.md section 2) on a float32 [V,3] / int32 [F,3] CUDA mesh: drops faces that repeat a
+    vertex index and faces whose vertex set repeats an earlier face's, then every connected component (faces sharing a
+    vertex) with fewer than min_faces faces or whose bounding-box diagonal is below min_diameter times the whole mesh's,
+    then unreferenced vertices.  Surviving vertices and faces keep their order, and vertex bytes are unchanged; every run
+    gives the same bytes.  The defaults are recalled from kiui's clean_mesh (min_f=64, min_d=20 %), which the reference
+    calls; they have not been checked against its source.  pymeshlab's other cleanup steps are left out: marching cubes
+    already welds one vertex per grid edge, its table gives closed 2-manifolds, and remeshing is out of scope.
+    Raises ValueError for bad arguments or a face index outside [0, V)."""
+    if not isinstance(min_faces, (int, np.integer)) or min_faces < 0 or not np.isfinite(min_diameter) or min_diameter < 0:
+        raise ValueError(f"b200gs: clean_mesh: min_faces must be an integer >= 0 and min_diameter finite and >= 0 "
+                         f"(got {min_faces!r}, {min_diameter!r})")
+    return _edit("clean_mesh", vertices, faces,
+                 lambda L, Nv, Nf, *a: L.b200gs_mesh_clean(Nv, Nf, a[0], a[1], int(min_faces), float(min_diameter), *a[2:]),
+                 lambda L, Nv, Nf: L.b200gs_mesh_clean_scratch_bytes(Nv, Nf))[0]
+
+
+def _decimate(vertices, faces, target):
+    if not isinstance(target, (int, np.integer)) or target < 4:
+        raise ValueError(f"b200gs: decimate_mesh: target must be an integer >= 4 (got {target!r})")
+    target = min(int(target), 0x7FFFFFFF)
+    return _edit("decimate_mesh", vertices, faces,
+                 lambda L, Nv, Nf, *a: L.b200gs_mesh_decimate(Nv, Nf, a[0], a[1], target, *a[2:]),
+                 lambda L, Nv, Nf: L.b200gs_mesh_decimate_scratch_bytes(Nv, Nf))
+
+
+@torch.no_grad()
+def decimate_mesh(vertices, faces, target) -> Mesh:
+    """Quadric edge collapse (Garland-Heckbert) of a float32 [V,3] / int32 [F,3] CUDA mesh to at most `target` faces, in
+    parallel rounds on the GPU (DESIGN.md section 2 is the definition): area-weighted plane quadrics in float64, the
+    optimal position where the 3x3 system is well conditioned, else the cheapest of the two ends and the midpoint;
+    boundary and non-manifold vertices stay, every collapse keeps the link condition and flips no face.  A closed
+    manifold ends at target or target - 1 faces.  When no valid collapse is left above `target`, the mesh at that point
+    is returned with a warning.  Vertex attributes are not carried; query the field at the new vertices
+    (extract_colored_mesh does).  Surviving faces keep their order; every run gives the same bytes."""
+    m, _ = _decimate(vertices, faces, target)
+    if m.faces.shape[0] > target:
+        import warnings
+        warnings.warn(f"b200gs: decimate_mesh: stopped at {m.faces.shape[0]} faces, above the target {target}: no valid collapse "
+                      f"is left (boundary, non-manifold or topology-changing edges)", RuntimeWarning, stacklevel=2)
+    return m
+
+
+def _check_edit(clean, min_faces, min_diameter, decimate_target):
+    if not isinstance(decimate_target, (int, np.integer)) or (decimate_target != 0 and decimate_target < 4):
+        raise ValueError(f"b200gs: extract_mesh: decimate_target must be 0 (off) or an integer >= 4 (got {decimate_target!r})")
+    if clean and (not isinstance(min_faces, (int, np.integer)) or min_faces < 0 or not np.isfinite(min_diameter) or min_diameter < 0):
+        raise ValueError(f"b200gs: extract_mesh: min_faces must be an integer >= 0 and min_diameter finite and >= 0 "
+                         f"(got {min_faces!r}, {min_diameter!r})")
+
+
+def _mesh(k, resolution, num_blocks, relax_ratio, density_thresh, clean=False, min_faces=64, min_diameter=0.2, decimate_target=0):
+    """-> (index-space vertices, faces, world vertices) of extract_mesh from the kept set k; cleanup and decimation run
+    on the index-space mesh (grid pitch 1)."""
     occ = _density_field(k.xyz, k.cov6, k.opac, resolution, num_blocks, relax_ratio)
     v, faces = marching_cubes(occ, density_thresh)
+    if clean:
+        v, faces = clean_mesh(v, faces, min_faces=min_faces, min_diameter=min_diameter)
+    if decimate_target:
+        v, faces = decimate_mesh(v, faces, decimate_target)
     w = (v.double() / (resolution - 1.0) * 2 - 1) / k.scale + k.center.double()
     return v, faces, w.float()
 
 
 @torch.no_grad()
 def extract_mesh(means3D, opacities=None, scales=None, rotations=None, *, raw=False, density_thresh=1.0, resolution=128,
-                 num_blocks=16, relax_ratio=1.5) -> Mesh:
+                 num_blocks=16, relax_ratio=1.5, clean=False, min_faces=64, min_diameter=0.2, decimate_target=0) -> Mesh:
     """The reference's extract_mesh up to its remeshing: extract_fields, marching cubes at density_thresh, and the vertices
-    mapped back to world space as v / (resolution - 1) * 2 - 1, then / scale + center (in float64, stored as float32)."""
+    mapped back to world space as v / (resolution - 1) * 2 - 1, then / scale + center (in float64, stored as float32).
+    clean=True runs clean_mesh(min_faces, min_diameter) and decimate_target > 0 runs decimate_mesh to that many faces,
+    in that order, on the index-space mesh before the world mapping; the defaults give the raw marching-cubes mesh."""
+    _check_edit(clean, min_faces, min_diameter, decimate_target)
     if isinstance(means3D, GaussianParams):
         if opacities is not None or scales is not None or rotations is not None:
             raise ValueError("b200gs: extract_fields: pass either a GaussianParams or the four tensors")
         means3D, opacities, scales, rotations, raw = means3D.xyz, means3D.opacity, means3D.scaling, means3D.rotation, True
     k, resolution, num_blocks = _kept("extract_fields", means3D, opacities, scales, rotations, raw, resolution, num_blocks)
-    _, faces, w = _mesh(k, resolution, num_blocks, relax_ratio, density_thresh)
+    _, faces, w = _mesh(k, resolution, num_blocks, relax_ratio, density_thresh, clean, min_faces, min_diameter, decimate_target)
     return Mesh(w, faces)
 
 
@@ -286,7 +379,7 @@ def query_field(points, means3D, opacities=None, scales=None, rotations=None, sh
     the block it falls in, so at a grid sample the density is the field's voxel bit for bit.  colour =
     max(SH(S / D, -normal) + 0.5, 0) with S / D the opacity-weighted mean coefficients; view_dependent=False (or a zero
     normal) keeps the DC term alone.  Where the density is 0 every output is 0.  Use it to colour a mesh that was
-    remeshed or decimated elsewhere.  Raises ValueError for a non-finite point, and as extract_fields does."""
+    remeshed elsewhere (extract_colored_mesh already colours cleaned and decimated meshes).  Raises ValueError for a non-finite point, and as extract_fields does."""
     means3D, opacities, scales, rotations, raw, shs, sh_degree = _unwrap("query_field", means3D, opacities, scales, rotations, raw, shs,
                                                                          sh_degree)
     k, resolution, num_blocks = _kept("query_field", means3D, opacities, scales, rotations, raw, resolution, num_blocks)
@@ -301,15 +394,18 @@ def query_field(points, means3D, opacities=None, scales=None, rotations=None, sh
 
 @torch.no_grad()
 def extract_colored_mesh(means3D, opacities=None, scales=None, rotations=None, shs=None, *, raw=False, sh_degree=None,
-                         view_dependent=True, density_thresh=1.0, resolution=128, num_blocks=16, relax_ratio=1.5) -> ColoredMesh:
+                         view_dependent=True, density_thresh=1.0, resolution=128, num_blocks=16, relax_ratio=1.5, clean=False,
+                         min_faces=64, min_diameter=0.2, decimate_target=0) -> ColoredMesh:
     """extract_mesh (the same vertex and face bytes) with per-vertex normals and colours from the field query, evaluated at
-    the vertices' normalised positions v / (resolution - 1) * 2 - 1 (float32).  Arguments as extract_mesh and
-    query_field; without SH (tensors and shs=None) colors is None."""
+    the vertices' normalised positions v / (resolution - 1) * 2 - 1 (float32) -- after cleanup and decimation when they
+    are on, so a decimated mesh gets them at its final vertices.  Arguments as extract_mesh and query_field; without SH
+    (tensors and shs=None) colors is None."""
+    _check_edit(clean, min_faces, min_diameter, decimate_target)
     means3D, opacities, scales, rotations, raw, shs, sh_degree = _unwrap("extract_colored_mesh", means3D, opacities, scales, rotations,
                                                                          raw, shs, sh_degree)
     k, resolution, num_blocks = _kept("extract_colored_mesh", means3D, opacities, scales, rotations, raw, resolution, num_blocks)
     shs, K, deg = _check_shs("extract_colored_mesh", shs, k.keep, sh_degree, view_dependent, k.xyz.device)
-    v, faces, w = _mesh(k, resolution, num_blocks, relax_ratio, density_thresh)
+    v, faces, w = _mesh(k, resolution, num_blocks, relax_ratio, density_thresh, clean, min_faces, min_diameter, decimate_target)
     q = (v / (resolution - 1) * 2 - 1).contiguous()
     fq = _query(k, shs, K, deg, q, resolution, num_blocks, relax_ratio)
     return ColoredMesh(w, faces, fq.normals, fq.colors)

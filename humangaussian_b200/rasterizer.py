@@ -119,7 +119,8 @@ EXPORTS = ["b200gs_forward", "b200gs_backward", "b200gs_mark_visible", "b200gs_d
            "b200gs_marching_cubes_scratch_bytes", "b200gs_marching_cubes_count", "b200gs_marching_cubes_emit",
            "b200gs_pose_scratch_bytes", "b200gs_pose_keypoints", "b200gs_pose_draw",
            "b200gs_mesh_raster_scratch_bytes", "b200gs_mesh_raster_count", "b200gs_mesh_raster_emit", "b200gs_mesh_interpolate",
-           "b200gs_mesh_incidence_bytes", "b200gs_mesh_incidence", "b200gs_mesh_vertex_normals", "b200gs_mesh_normal_image"]
+           "b200gs_mesh_incidence_bytes", "b200gs_mesh_incidence", "b200gs_mesh_vertex_normals", "b200gs_mesh_normal_image",
+           "b200gs_mesh_clean_scratch_bytes", "b200gs_mesh_clean", "b200gs_mesh_decimate_scratch_bytes", "b200gs_mesh_decimate"]
 STAGES = ["preprocess_fwd", "scan", "binning", "blend_fwd", "blend_bwd", "preprocess_bwd"]
 
 
@@ -221,6 +222,12 @@ def load_library():
     L.b200gs_mesh_vertex_normals.argtypes = [i32, i32, i32, vp, vp, vp, sz, vp, vp]
     L.b200gs_mesh_normal_image.restype = C.c_int
     L.b200gs_mesh_normal_image.argtypes = [i32, i32, i32, i32, i32, vp, i32, vp, vp, vp, vp]
+    L.b200gs_mesh_clean_scratch_bytes.restype = sz; L.b200gs_mesh_clean_scratch_bytes.argtypes = [i32, i32]
+    L.b200gs_mesh_clean.restype = C.c_int
+    L.b200gs_mesh_clean.argtypes = [i32, i32, vp, vp, i32, C.c_double, vp, sz, vp, vp, C.POINTER(i64), C.POINTER(i32), vp]
+    L.b200gs_mesh_decimate_scratch_bytes.restype = sz; L.b200gs_mesh_decimate_scratch_bytes.argtypes = [i32, i32]
+    L.b200gs_mesh_decimate.restype = C.c_int
+    L.b200gs_mesh_decimate.argtypes = [i32, i32, vp, vp, i32, vp, sz, vp, vp, C.POINTER(i64), C.POINTER(i32), vp]
     L.b200gs_last_cuda_error.restype = C.c_char_p
     L.b200gs_launch_count.restype = i64
     L.b200gs_profile_enable.restype = None; L.b200gs_profile_enable.argtypes = [C.c_int]

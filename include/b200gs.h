@@ -616,6 +616,27 @@ int b200gs_mesh_vertex_normals(int32_t n_frames, int32_t n_verts, int32_t n_face
 int b200gs_mesh_normal_image(int32_t n_views, int32_t height, int32_t width, int32_t n_verts, int32_t n_faces, const float *normals,
                              int32_t normals_per_view, const float *rast, const int32_t *tri, float *out, void *stream);
 
+/* ---- mesh cleanup and decimation (humangaussian_b200/mesh.py clean_mesh / decimate_mesh; DESIGN.md section 2) ------
+ * Both take a mesh vertices [n_verts,3] float32, faces [n_faces,3] int32 (device, 4-byte aligned) and write the result
+ * to out_vertices / out_faces, which hold at least n_verts and n_faces rows; counts (HOST int64 [2]) receives the output's
+ * vertex and face counts and rounds (HOST) the number of rounds.  Surviving vertices and faces keep their relative order.
+ * Unlike the other calls these wait on the host: after a check that every face index lies in [0, n_verts) (a face
+ * outside is B200GS_E_ARGS, and nothing reads through it), once per round, and once for the counts.  scratch: the
+ * *_scratch_bytes query, 16-byte aligned.  n_verts < 2^31 - 1 and n_faces < 2^24, else B200GS_E_RANGE.
+ * b200gs_mesh_clean: drops faces that repeat an index or an earlier face's vertex set, then every connected component
+ *   (faces sharing a vertex) with fewer than min_faces faces or a bounding-box diagonal below min_diameter times the
+ *   whole mesh's, then unreferenced vertices.  Vertex bytes are unchanged.  rounds: labelling rounds.
+ * b200gs_mesh_decimate: quadric edge collapse in parallel rounds to at most `target` faces (target >= 4, else
+ *   B200GS_E_ARGS); it stops early, above target, when a round finds no valid collapse.  Boundary and non-manifold
+ *   vertices stay.  rounds: rounds that collapsed at least one edge. */
+size_t b200gs_mesh_clean_scratch_bytes(int32_t n_verts, int32_t n_faces);
+int b200gs_mesh_clean(int32_t n_verts, int32_t n_faces, const float *vertices, const int32_t *faces, int32_t min_faces, double min_diameter,
+                      void *scratch, size_t scratch_bytes, float *out_vertices, int32_t *out_faces, int64_t *counts, int32_t *rounds,
+                      void *stream);
+size_t b200gs_mesh_decimate_scratch_bytes(int32_t n_verts, int32_t n_faces);
+int b200gs_mesh_decimate(int32_t n_verts, int32_t n_faces, const float *vertices, const int32_t *faces, int32_t target, void *scratch,
+                         size_t scratch_bytes, float *out_vertices, int32_t *out_faces, int64_t *counts, int32_t *rounds, void *stream);
+
 /* ---- per-stage device timing (CUDA events recorded on the launch stream around each stage) -----------------
  * enable, run any number of forward/backward calls, then read: accumulated milliseconds and call counts per stage
  * since the last read.  b200gs_profile_read synchronises on the recorded events. */
